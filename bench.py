@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — CT slices/sec @256x256 through the B200 engine, per the driver contract.
+"""bench.py — CT slices/sec @256x256 through the H100 engine.
 
     python bench.py --gpus N --steps K --warmup W              # this repo's engine, BASELINE config C2 (the headline)
     python bench.py --config C3|C4|C5 ...                       # the other BASELINE.json configurations
     python bench.py --mode shard --gpus N ...                   # ONE volume's slices sharded over the N GPUs (latency)
     python bench.py --impl reference ...                        # the CPU port of the reference path (oracle) on host cores
+    python bench.py ... --dump-outputs DIR                      # also write the last timed step's label volume(s) to DIR/*.npy
 
 One "step" = one full pass of the hot path (preprocess -> U-Net forward -> postprocess -> reshape) over the
 configuration's synthetic int16 CT volume(s) on every GPU:
@@ -28,6 +29,7 @@ import os
 os.environ.setdefault("NCCL_DEBUG_FILE", "/dev/stderr")   # NCCL's version / debug lines must not precede the JSON line on stdout
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -52,9 +54,8 @@ CONFIGS = {
                desc="R231 throughput: 8 volumes x 512 slices (256x256 int16, synthetic) per GPU and step = 64 volumes over 8 GPUs"),
 }
 WEIGHT_SEEDS = {3: 7, 6: 8}
-# mean dram__bytes_read.sum + dram__bytes_write.sum per conv_tc_kernel launch: taken from the newest committed ncu --set full
-# summary that tools/ncu_summarize.py wrote (profiles/*conv_traffic.json: per-layer table of one full 37-slice wave)
-TRAFFIC_FALLBACK = (188.7e6, "profiles/r01_ncu_summary_v5.md (4 launches of a 37-slice wave, layers down2/down3)")
+# --dump-outputs: at most this many slices of label volume per step are written (float32), chosen with a fixed seed
+DUMP_SLICES = 160
 
 
 def log(*a):
@@ -65,24 +66,11 @@ def rank_info():
     return int(os.environ.get("RANK", 0)), int(os.environ.get("LOCAL_RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
 
 
-def conv_traffic():
-    """(mean DRAM bytes per conv launch, source) from the newest per-layer table under profiles/."""
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_conv_traffic.json")))
-    if files:
-        try:
-            d = json.load(open(files[-1]))
-            return float(d["mean_bytes_per_launch"]), os.path.relpath(files[-1], ROOT) + " (%d launches of one wave)" % d["launches"]
-        except Exception:
-            pass
-    return TRAFFIC_FALLBACK
-
-
 def get_weights(K, seed, steps=60):
     """Seeded 'trained-looking' synthetic weights with the reference's layout (no network for the released .pth)."""
     import torch
     from oracle import synth
-    path = "/tmp/lm_b200_synth_K%d_s%d_t%d_r%s.pth" % (K, seed, steps, os.environ.get("LOCAL_RANK", "0"))
+    path = os.path.join(tempfile.gettempdir(), "lm_synth_det_K%d_s%d_t%d_r%s.pth" % (K, seed, steps, os.environ.get("LOCAL_RANK", "0")))
     if os.path.exists(path):
         return torch.load(path, map_location="cpu")
     t0 = time.time()
@@ -182,6 +170,19 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, d_outs):
+    """The uint8 label volume(s) the last timed step returned, as float32: a seeded, sorted sample of at most
+    DUMP_SLICES slices in all (every slice when they fit), with the sampled slice indices beside each volume."""
+    os.makedirs(out_dir, exist_ok=True)
+    per_vol = max(1, DUMP_SLICES // len(d_outs))
+    for i, d in enumerate(d_outs):
+        S = d.shape[0]
+        idx = np.arange(S) if S <= per_vol else np.sort(np.random.default_rng(1234 + i).choice(S, per_vol, replace=False))
+        labels = d.cpu().numpy()[idx].astype(np.float32)
+        np.save(os.path.join(out_dir, "labels_vol%d.npy" % i), labels)
+        np.save(os.path.join(out_dir, "labels_vol%d_slices.npy" % i), idx.astype(np.float64))
+
+
 def run_engine(args):
     import torch
     import torch.distributed as dist
@@ -205,7 +206,7 @@ def run_engine(args):
     sds = [get_weights(K, WEIGHT_SEEDS[K])] + ([get_weights(cfg["fill"], WEIGHT_SEEDS[cfg["fill"]])] if fused else [])
     paths = []
     for i, sd in enumerate(sds):
-        p = "/tmp/lm_b200_bench_%s_%d_rank%d.pth" % (args.config, i, local_rank)
+        p = os.path.join(tempfile.gettempdir(), "lm_bench_%s_%d_rank%d.pth" % (args.config, i, local_rank))
         torch.save(sd, p)
         paths.append(p)
     if fused:
@@ -268,6 +269,8 @@ def run_engine(args):
     barrier()
     wall_ms = (time.perf_counter() - t0) * 1e3
     sampler.stop_flag = True
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_outs)
     # every engine call ends with a stream synchronisation, so the bracketed wall time between the two synchronised
     # barriers IS the device-side duration of the K steps
     step_ms = wall_ms / args.steps
@@ -319,12 +322,11 @@ def run_engine(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
-        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (cuBLAS bf16, kernel timed inside a long step)" if peaks else "fallback 1.4 PFLOP/s sustained"
+        peak = peaks.get("bf16_tflops_sustained", 989.0)
+        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (cuBLAS bf16, kernel timed inside a long step)" if peaks else "H100 SXM data sheet, dense fp16 at 700 W"
         my_slices = (parallel.shard_range(S, 0, world)[1] if shard else nv * S)
         flops_timed = (cfg["gflop"] - STEM_GFLOP * (2 if fused else 1)) * 1e9 * my_slices * args.steps  # rank 0's convolutions
         achieved = flops_timed / (acc["conv_ms"] * 1e-3) / 1e12 if acc["conv_ms"] > 0 else None
-        traffic, traffic_src = conv_traffic()
         # CPU baseline + parity: the oracle port on this box's host cores on a bounded sample, the engine on the same sample
         n_cpu = 16 if not fused else 8
         sample = vols[0][:n_cpu]
@@ -361,8 +363,8 @@ def run_engine(args):
             "gpu_launches": int(acc["launches"]),
             "clocks": sampler.result(),
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                         "frac": (achieved / peak) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
-                         "kernel": "conv_tc kernels (tcgen05 kind::f16, 3 products per algorithmic MAC => ceiling 1/3 of the bf16 peak)",
+                         "frac": (achieved / peak) if achieved else None,
+                         "kernel": "conv_tc kernels (wgmma .f16, 3 products per algorithmic MAC => ceiling 1/3 of the fp16 peak)",
                          "launches_timed": int(acc["conv_launches"]), "avg_launch_ms": acc["conv_ms"] / max(1, acc["conv_launches"]),
                          "peak_source": peak_src, "algorithmic_flops_per_step": flops_timed / args.steps},
             "cpu_baseline": {"value": n_cpu / cpu_s, "unit": "slices/s", "cores": cores, "kind": "port",
@@ -382,6 +384,8 @@ def main():
     ap.add_argument("--impl", default="engine", choices=["engine", "reference"])
     ap.add_argument("--config", default="C2", choices=sorted(CONFIGS))
     ap.add_argument("--mode", default="replica", choices=["replica", "shard"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the label volume(s) of the last timed step to DIR/<name>.npy (float32, seeded slice sample)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* lungmask_b200 — C ABI of the B200-native lungmask hot path.
+/* lungmask_b200 — C ABI of the H100-native lungmask hot path.
  *
  * The reference (JoHof/lungmask) is pure Python and has no FFI for this path; the interface each
  * entry point replaces is therefore a Python function of the reference, cited per function
@@ -168,9 +168,8 @@ LM_API int lm_last_timings(const lm_engine* e, float* ms7, int64_t* kernel_launc
  * stream; read the sum with lm_last_conv_timing after an lm_apply_volume* call), "chunk_kb" (k-blocks
  * accumulated inside the tensor core between fp32 round-to-nearest adds; sets both layer classes),
  * "chunk_kb_wide" (the same for the layers with >= 128 output channels only; defaults: 1 for the 64-channel
- * layers, 2 for the wide ones), "dual_issue" (0/1: a second MMA-issuing thread per CTA on alternate chunks;
- * default 0), "cta_pairs" (0/1: the cta_group::2 convolution kernel: validated, on par, default 0),
- * "weight_mcast" (0 / 2: clusters of two CTAs share every weight stage through TMA multicast),
+ * layers, 2 for the wide ones), "weight_mcast" (0 / 2: clusters of two CTAs share every weight stage through TMA
+ * multicast; bit-identical, default 0),
  * "stem_v2" (0 = first stem kernel, 1 = register-resident, 2 = shared-memory tile, 3 = the same with the next tile's
  * samples fetched one tile ahead, the default; all bit-identical),
  * "graphs" (1, default: a volume's forward - every wave's ~26 launches - is captured once as a CUDA graph and replayed;

@@ -1,4 +1,4 @@
-"""Drop-in alias: `import lungmask` resolves to the B200 engine's mirror of the reference package.
+"""Drop-in alias: `import lungmask` resolves to the H100 engine's mirror of the reference package.
 
 `from lungmask import LMInferer`, `from lungmask.mask import MODEL_URLS, get_model, apply, apply_fused`,
 `from lungmask.utils import preprocess, postprocessing, ...` and `python -m lungmask IN OUT` all reach

@@ -26,7 +26,7 @@ def build_parser():
     p.add_argument("output", metavar="output", type=str, help="Filepath for output lungmask")
     p.add_argument("--modelname", choices=["R231", "LTRCLobes", "LTRCLobes_R231", "R231CovidWeb"], default="R231")
     p.add_argument("--modelpath", type=str, default=None, help="spcifies the path to the trained model")
-    p.add_argument("--cpu", action="store_true", help="not supported by the B200 engine (kept for flag compatibility)")
+    p.add_argument("--cpu", action="store_true", help="not supported by the H100 engine (kept for flag compatibility)")
     p.add_argument("--nopostprocess", action="store_true", help="Deactivates postprocessing")
     p.add_argument("--noHU", action="store_true", help=argparse.SUPPRESS)
     p.add_argument("--batchsize", type=int, default=20, help="Number of slices processed simultaneously")

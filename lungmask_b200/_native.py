@@ -24,7 +24,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeError(
-            "%s is missing: build it with `python -m lungmask_b200.build` (needs nvcc, sm_100a). "
+            "%s is missing: build it with `python -m lungmask_b200.build` (needs nvcc, sm_90a). "
             "lungmask_b200 has no CPU or eager-PyTorch fallback." % LIB_PATH)
     L = C.CDLL(LIB_PATH)
     vp, i32, u8p, i16p, i32p, f32p = C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p

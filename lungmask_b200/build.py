@@ -1,4 +1,4 @@
-"""Builds lungmask_b200/liblungmask_b200.so (sm_100a only) with nvcc, in-tree.
+"""Builds lungmask_b200/liblungmask_b200.so (sm_90a only) with nvcc, in-tree.
 
     python -m lungmask_b200.build [--force]
 """
@@ -9,8 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblungmask_b200.so")
-SOURCES = ["conv_tc.cu", "conv_tc_pair.cu", "forward_misc.cu", "preproc.cu", "postproc.cu", "shard.cu", "engine.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["conv_tc.cu", "forward_misc.cu", "preproc.cu", "postproc.cu", "shard.cu", "engine.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 
 
@@ -52,7 +52,7 @@ def build(force=False, verbose=True):
             raise RuntimeError("nvcc failed for %s:\n%s" % (src, out))
         if verbose and out.strip():
             print(out)
-    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// 3x3 / 1x1 convolution as an implicit GEMM on the sm_100a 5th-generation tensor cores.
+// 3x3 / 1x1 convolution as an implicit GEMM on the sm_90a tensor cores (wgmma).
 //
 // Replaces, for the U-Net of lungmask/resunet.py, every Conv2d(3x3,pad 1)+ReLU+BatchNorm2d pair
 // (resunet.py:93-105), the decoder's 1x1 convolutions (resunet.py:133, evaluated below the upsample),
@@ -12,376 +12,399 @@
 //   * A operand: ONE 5-D TMA box per BK-channel block - the patch plus its one-pixel halo,
 //     (BK ch, 10 x, 18 y, 2 planes, 1 image) = 180 rows of 128 B per plane - serves all nine taps: the tap
 //     (dy,dx) view is the same shared-memory tile entered at row (dy+1)*10 + (dx+1) with an 8-row-group
-//     stride of 10 rows.  UMMA shared-memory descriptors allow that: the 128B swizzle is a function of the
-//     absolute shared-memory address, so a start address at any 128-byte row and a stride-byte-offset of
-//     1280 B address the rows TMA wrote (checked on B200: profiles/r01_umma_rowoffset_probe.log).  This
-//     cuts the L2->SM traffic of the activations 6.4x versus one box per tap.  TMA zero-fills outside the
-//     image, which IS the convolution's zero padding.
-//   * B operand: one 4-D TMA box (BK cin, BN cout, 1 tap, 2 planes) per k-block.
-//   * both land 128B-swizzled, K-major, i.e. in the canonical tcgen05 shared-memory layout.
+//     stride of 10 rows (wgmma shared-memory descriptors allow that: the 128B swizzle is a function of the
+//     absolute shared-memory address).  TMA zero-fills outside the image, which IS the convolution's zero padding.
+//   * B operand: one 4-D TMA box (BK cin, BN cout, 1 tap, 2 planes) per k-block, into a ring of STAGES.
+//   * both land 128B-swizzled, K-major, i.e. in the canonical wgmma shared-memory layout.
 //   * fp32-class accuracy from 11-bit tensor-core operands: every fp32 value is pre-split into a hi and a lo plane
 //     (fp16 hi + fp16 lo * 2^-11 by default, tf32 hi + tf32 lo with LM_OPERAND_F16=0) and each k-step computes
-//     hi*hi, hi*lo and lo*hi - three exact products - with TWO instructions: the B tile's hi and lo planes are
-//     adjacent in shared memory, so  A_hi x [B_hi;B_lo]  is one N = 2*BN MMA whose left half of the accumulator is
-//     hi*hi and whose right half is hi*lo; A_lo x B_hi (N = BN) then adds lo*hi into that right half.  The
-//     tensor-core accumulator rounds toward zero (measured on B200: -6e-5 relative drift over K = 8192,
-//     profiles/r01_umma_probe.log), so the dominant hi*hi sum is kept apart from the 2^-11-times-smaller
-//     corrections and only `chunk_kb` k-blocks (4 MMA k-steps each) of hi*hi are accumulated in TMEM before the
-//     epilogue warps add that partial tile into fp32 registers with round-to-nearest, while the tensor core
-//     already works on the next chunk (NBUF TMEM accumulators of 2*BN columns in a ring).  The correction halves
-//     are NOT drained per chunk: each ring slot keeps accumulating its corrections for the whole tile (their
-//     drift is 2^-11 times smaller still) and is read once, with the slot's last chunk - so the per-chunk drain
-//     is BN columns, half of the accumulator.
-//   * persistent CTAs (one per SM), warp-specialised: warp 0 TMA producer, warp 1 (and optionally 3) MMA issuer
-//     - one elected lane running mma_issue_loop -, warp 2 TMEM allocator, warps 4-11 epilogue (TMEM lane quarter
-//     = warp % 4, two warps share a quarter and split the columns or, for BN = 64, take alternate tiles).
+//     hi*hi, hi*lo and lo*hi - three exact products - as three N = BN wgmmas, hi*hi into one accumulator and both
+//     corrections into another.  (One N = 2*BN wgmma over [hi*hi | hi*lo] would save an instruction, but its
+//     accumulator overlaps the lo*hi one and ptxas then serialises every wgmma of the kernel.)  The tensor
+//     core's fp32 accumulation does not round to nearest, so the dominant hi*hi sum is kept apart from the
+//     2^-11-times-smaller corrections: only `chunk_kb` k-blocks of hi*hi are accumulated by the tensor core before
+//     the partial sum is added, round-to-nearest, into a separate fp32 register sum.  The corrections accumulate in
+//     the tensor core for the whole tile.
+//   * persistent CTAs (one per SM), warp-specialised: warp 0 is the TMA producer, warpgroups 1 and 2 are consumers
+//     that each own 64 rows of the tile (image rows 0-7 / 8-15 of the patch): they issue the wgmmas, drain the
+//     chunks and run the epilogue of their rows straight from the accumulator registers.
 #include <atomic>
 #include <stdio.h>
 #include "conv_tc.cuh"
-#include "sm100_ptx.cuh"
-
-namespace lm {
-#ifdef LM_CONV_PROFILE
-// Role-level stall accounting for tools/conv_probe: cycles each role spends waiting on each barrier class.
-__device__ unsigned long long g_conv_prof[16];
-#endif
-}  // namespace lm
-#ifdef LM_CONV_PROFILE
-#define LM_PROF_T0() const long long prof_t0_ = clock64()
-#define LM_PROF_ADD(slot) atomicAdd(&g_conv_prof[slot], (unsigned long long)(clock64() - prof_t0_))
-#else
-#define LM_PROF_T0()
-#define LM_PROF_ADD(slot)
-#endif
-// LM_EXP: bit mask of timing-only ablations for tools/conv_probe (results are wrong with any bit set):
-//   1 no correction MMAs, 2 chunk drains skip their TMEM loads, 4 tile epilogue skips staging + TMA stores,
-//   8 single MMA issuer, 16 no wide MMAs (only the N = BN correction MMAs), 32 producer loads no weights after the first ring fill
-#ifndef LM_EXP
-#define LM_EXP 0
-#endif
-#include "conv_tc_common.cuh"
+#include "sm90_ptx.cuh"
 
 namespace lm {
 namespace {
 
-#if LM_OPERAND_F16
-#define LM_UMMA_C umma_f16_c
-#define LM_UMMA umma_f16
-#define LM_MAKE_IDESC make_idesc_f16
-#else
-#define LM_UMMA_C umma_tf32_c
-#define LM_UMMA umma_tf32
-#define LM_MAKE_IDESC make_idesc_tf32
-#endif
+constexpr int BM = 128, BK = kBK, TILE_H = 16, TILE_W = 8;
+constexpr int ROW_BYTES = 128;
+constexpr int HALO_W = TILE_W + 2, HALO_H = TILE_H + 2;
+constexpr int A_PLANE_BYTES_3x3 = HALO_W * HALO_H * ROW_BYTES;  // 180 rows x 128 B = 23040 B per plane
+constexpr int A_PLANE_BYTES_1x1 = BM * ROW_BYTES;               // 16 KB per plane
+constexpr int A_BUF_BYTES = 2 * A_PLANE_BYTES_3x3;              // 46080 B = 45 KB (both planes), 1024-aligned
+constexpr int NUM_A_BUFS = 2;
+constexpr int NUM_THREADS = 384;
+constexpr int NUM_CONSUMER_WARPS = 8;
+constexpr int MAX_CLASSES = 8;
+constexpr int REGS_PRODUCER = 40, REGS_CONSUMER = 232;   // 128 x 40 + 256 x 232 <= 65536
 
-struct IssueArgs {
-  uint32_t me;     // issuer 0 / 1
-  int first_tile, total_tiles, tile_step, num_cb, chunk_kb;
-  uint32_t tmem_base, smem_a, smem_b;
-  uint32_t full0, empty0, tfull0, tempty0, afull0, aempty0;  // mbarrier arrays (shared-memory addresses)
+template <int BN>
+struct Cfg {
+  static constexpr int B_PLANE_BYTES = BN * ROW_BYTES;
+  static constexpr int STAGE_BYTES = 2 * B_PLANE_BYTES;      // one weight tile (hi + lo planes) per k-block
+  static constexpr int STAGES = (BN == 64) ? 6 : 4;
+  // dynamic shared memory only (1024-aligned for the swizzled tiles): activation patches | weight ring | mbarriers | head
+  static constexpr int NUM_BARS = 2 * STAGES + 2 * NUM_A_BUFS;
+  static constexpr int OFF_B = NUM_A_BUFS * A_BUF_BYTES;
+  static constexpr int OFF_BARS = OFF_B + STAGES * STAGE_BYTES;
+  static constexpr int OFF_HEAD = OFF_BARS + NUM_BARS * 8;                         // BN = 64 only: head weights + bias
+  static constexpr int DYN_SMEM = OFF_HEAD + ((BN == 64) ? (MAX_CLASSES * 64 + MAX_CLASSES) * 4 : 0);
+  static_assert(DYN_SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
 };
 
-// The MMA issue loop of one issuer thread.  Chunk g (counted over all tiles of the CTA) lives in accumulator slot
-// g % NBUF and, with two issuers (DUAL), belongs to issuer g & 1; NBUF is even, so every slot is written by one
-// issuer only and the order of additions into each accumulator is fixed (bit-deterministic results).  With DUAL
-// both issuers wait on EVERY weight-stage and activation-buffer barrier in order (a wait that has already
-// completed costs a few instructions) so that their phase bits can never alias; only the owner of a k-block issues
-// its MMAs and releases its weight stage, both release every activation buffer (barrier count 2).
-//
-// Software pipelining: the tensor pipe's instruction queue is only a few MMAs deep, so the gap between the last MMA
-// of one k-block and the first MMA of the next must stay short.  The barrier waits and ring bookkeeping of k-block
-// i+1 (weight stage, activation buffer) are therefore executed in the MIDDLE of k-block i's MMA burst and the
-// burst's remaining MMAs then follow back to back with k-block i+1's first ones.
-template <int BN, int TAPS, bool DUAL, bool UNROLL = true, int MC = 1>
-__device__ __forceinline__ void mma_issue_loop(const IssueArgs& g) {
-  using C = Cfg<BN>;
-  constexpr uint32_t STAGES = C::STAGES, NBUF = C::NBUF;
-  constexpr int EGROUPS = C::EGROUPS;
-  constexpr int PATCH_W = (TAPS == 9) ? HALO_W : TILE_W;  // shared-memory rows per image row of the patch
-  constexpr uint32_t A_PLANE = (uint32_t)((TAPS == 9) ? A_PLANE_BYTES_3x3 : A_PLANE_BYTES_1x1) >> 4;
-  constexpr uint32_t B_PLANE = (uint32_t)C::B_PLANE_BYTES >> 4;
-  constexpr uint32_t idesc_wide = LM_MAKE_IDESC(BM, 2 * BN), idesc_corr = LM_MAKE_IDESC(BM, BN);
-  // shared-memory descriptors as (lo, hi) words: lo = start>>4 | LBO, hi = SBO | version | swizzle.
-  // A: K-major SW128 entered at an arbitrary 128-byte row, 8-row group stride = one patch row.
-  constexpr uint64_t hi_a = (uint64_t)((uint32_t)((PATCH_W * 128) >> 4) | (1u << 14) | (2u << 29)) << 32;
-  constexpr uint64_t hi_b = (uint64_t)((uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29)) << 32;
-  const uint32_t a_base_lo = ((g.smem_a & 0x3FFFFu) >> 4) | (1u << 16);
-  const uint32_t b_base_lo = ((g.smem_b & 0x3FFFFu) >> 4) | (1u << 16);
-  const uint32_t me = g.me;
-  const int num_kb = g.num_cb * TAPS, chunk_kb = g.chunk_kb;
-  if (g.first_tile >= g.total_tiles) return;
+struct TileCoord {
+  int n, y0, x0, n0;
+};
 
-  // state of the k-block whose barriers have been waited for ("current")
-  uint32_t s = 0, ph = 0, ab = 0, aph = 0;  // weight ring / activation ring position and phase
-  uint32_t gc = 0;                          // chunks closed by this CTA so far -> slot gc % NBUF, owner gc & 1
-  uint32_t tseq = 0;                        // tiles processed: the epilogue group (BN = 64) of a tile is tseq & 1
-  int kc = 0;                               // k-blocks already in the open chunk
-  int kb_left = num_kb;                     // k-blocks of the tile still to issue (including the current one)
-  uint32_t cit = 0;                         // chunks of this tile already closed
-  auto is_mine = [&](uint32_t chunk) { return !DUAL || ((chunk & 1u) == me); };
-  // waits of the first k-block
-  mbar_wait(g.afull0, 0);
-  if (is_mine(0)) mbar_wait(g.tempty0, 1);
-  mbar_wait(g.full0, 0);
-#ifdef LM_CONV_PROFILE
-  const long long prof_issue_t0 = clock64();
-#endif
+__device__ __forceinline__ TileCoord decode_tile(int tile, int n_tiles, int tiles_x, int tiles_img, int BN) {
+  TileCoord t;
+  const int mt = tile / n_tiles;
+  t.n0 = (tile - mt * n_tiles) * BN;
+  t.n = mt / tiles_img;
+  const int r = mt - t.n * tiles_img;
+  const int ty = r / tiles_x;
+  t.y0 = ty * TILE_H;
+  t.x0 = (r - ty * tiles_x) * TILE_W;
+  return t;
+}
 
-  for (int tile = g.first_tile; tile < g.total_tiles; tile += g.tile_step) {
-    const bool last_tile = tile + g.tile_step >= g.total_tiles;
-    for (int cb = 0; cb < g.num_cb; ++cb) {
-      const uint32_t a_cb = a_base_lo + ab * (uint32_t)(A_BUF_BYTES >> 4);
-      const uint32_t ab_cur = ab;
-      const bool last_cb = (cb == g.num_cb - 1);
-#pragma unroll(UNROLL ? TAPS : 1)
-      for (int tap = 0; tap < TAPS; ++tap) {
-        // tap (dy, dx) = the same patch entered (dy * PATCH_W + dx) rows further (16-byte units: 8 per row)
-        const uint32_t tap_off = (TAPS == 9) ? (uint32_t)(((tap / 3) * PATCH_W + (tap % 3)) * 8) : 0u;
-        const bool mine = is_mine(gc);
-        const uint32_t buf = gc % NBUF;
-        const uint32_t d_tmem = g.tmem_base + buf * (uint32_t)C::ACC_COLS;
-        const uint32_t alo = a_cb + tap_off;
-        const uint32_t blo = b_base_lo + s * (uint32_t)(C::STAGE_BYTES >> 4);
-        const bool first = (kc == 0);
-        const uint32_t s_cur = s;
-        // ---- first part of the burst
-        if (mine) {
-          LM_PROF_T0();
-          tc_fence_after();
-          if (first) {
-            // first k-step of a chunk: hi*hi restarts from zero; the corrections restart only at the slot's first
-            // chunk of the tile (cit < NBUF), so the two halves need separate instructions here
-            LM_UMMA_C<false>(d_tmem, hi_a | alo, hi_b | blo, idesc_corr);                              // hi*hi :=
-            LM_UMMA(d_tmem + BN, hi_a | alo, hi_b | (blo + B_PLANE), idesc_corr, cit >= NBUF ? 1u : 0u);  // hi*lo
-          } else {
-            LM_UMMA_C<true>(d_tmem, hi_a | alo, hi_b | blo, idesc_wide);                               // [hi*hi | hi*lo] +=
-          }
-          if (!(LM_EXP & 1)) LM_UMMA_C<true>(d_tmem + BN, hi_a | (alo + A_PLANE), hi_b | blo, idesc_corr);  // lo*hi
-          LM_UMMA_C<true>(d_tmem, hi_a | (alo + 2u), hi_b | (blo + 2u), idesc_wide);
-          if (!(LM_EXP & 1)) LM_UMMA_C<true>(d_tmem + BN, hi_a | (alo + A_PLANE + 2u), hi_b | (blo + 2u), idesc_corr);
-          LM_PROF_ADD(10);   // issuing the first two k-steps of the k-block (the thread blocks here when the MMA queue is full)
-        }
-        // ---- close the bookkeeping of this k-block, advance to the next one and wait for its barriers
-        --kb_left;
-        const bool chunk_end = (++kc == chunk_kb) || (kb_left == 0);
-        const uint32_t tfull_cur = g.tfull0 + 8 * ((EGROUPS == 2 ? (tseq & 1u) : 0u) * NBUF + buf);
-        if (chunk_end) { kc = 0; ++gc; ++cit; }
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-        bool has_next = true;
-        if (tap == TAPS - 1) {  // the next k-block opens a channel block (possibly of the next tile)
-          if (++ab == (uint32_t)NUM_A_BUFS) { ab = 0; aph ^= 1u; }
-          if (last_cb) {
-            has_next = !last_tile;
-            kb_left = num_kb; cit = 0; ++tseq;   // (kc is 0 here: a tile's last k-block closes its chunk)
-          }
-          if (has_next) { LM_PROF_T0(); mbar_wait(g.afull0 + 8 * ab, aph); LM_PROF_ADD(3); }
-        }
-        if (has_next) { LM_PROF_T0(); mbar_wait(g.full0 + 8 * s, ph); LM_PROF_ADD(4); }
-        // ---- rest of the burst, then the releases
-        if (mine) {
-          LM_PROF_T0();
-#pragma unroll
-          for (int k = 2; k < ROW_BYTES / 32; ++k) {
-            const uint32_t ko = (uint32_t)(k * 2);  // one MMA k-step = 32 B along K (16 fp16 / 8 tf32), >>4
-            LM_UMMA_C<true>(d_tmem, hi_a | (alo + ko), hi_b | (blo + ko), idesc_wide);
-            if (!(LM_EXP & 1)) LM_UMMA_C<true>(d_tmem + BN, hi_a | (alo + A_PLANE + ko), hi_b | (blo + ko), idesc_corr);
-          }
-          LM_PROF_ADD(11);   // the other two k-steps
-          {
-            LM_PROF_T0();
-            if (MC > 1) umma_commit_mcast(g.empty0 + 8 * s_cur, (uint16_t)((1u << MC) - 1u));  // ... in every CTA of the cluster
-            else umma_commit(g.empty0 + 8 * s_cur);      // weight stage consumed (only this issuer read it)
-            if (chunk_end) umma_commit(tfull_cur);       // chunk complete -> the tile's epilogue group may drain it
-            LM_PROF_ADD(12);
-          }
-        }
-        if (tap == TAPS - 1) umma_commit(g.aempty0 + 8 * ab_cur);  // arrives once this issuer's MMAs on the buffer have retired
-        // the accumulator slot of the next chunk is awaited LAST: with a two-slot ring it is the one hand-shake that
-        // regularly blocks (the epilogue drains chunk i-1 while chunk i executes), and blocking in the middle of the
-        // burst would leave the tensor pipe with half a k-block queued (measured: 8 % slower on the BN = 128 layers)
-        if (has_next && kc == 0 && is_mine(gc)) { LM_PROF_T0(); mbar_wait(g.tempty0 + 8 * (gc % NBUF), (((gc / NBUF) & 1u) ^ 1u)); LM_PROF_ADD(2); }
-      }
-    }
+// The CTA's tiles.  MC = 1: every CTA on its own, tile = item.  MC = 2: the two CTAs of a cluster take two pixel tiles of
+// the SAME output-channel block in lock step (work item = tile pair; every level has an even number of pixel tiles), so
+// that they can share every weight stage.
+template <int MC>
+struct WorkItems {
+  int first, step, total, n_tiles;
+  uint32_t rank;
+  __device__ WorkItems(int total_tiles, int n_tiles_) : n_tiles(n_tiles_) {
+    rank = (MC > 1) ? cluster_ctarank() : 0u;
+    first = (int)blockIdx.x / MC;
+    step = (int)gridDim.x / MC;
+    total = total_tiles / MC;
   }
-#ifdef LM_CONV_PROFILE
-  atomicAdd(&g_conv_prof[5], (unsigned long long)(clock64() - prof_issue_t0));   // the issuer's whole loop (waits included)
+  __device__ int tile(int item) const {
+    if (MC == 1) return item;
+    const int mtp = item / n_tiles;
+    return (MC * mtp + (int)rank) * n_tiles + (item - mtp * n_tiles);
+  }
+};
+
+// the hi / lo operand planes of two adjacent channels (c even) of one pixel
+__device__ __forceinline__ void store_split_pair(op_t* dst, size_t plane_stride, float a, float b) {
+#if LM_OPERAND_F16
+  uint32_t hi, lo;
+  split_f16x2(a, b, hi, lo);
+  *reinterpret_cast<uint32_t*>(dst) = hi;
+  *reinterpret_cast<uint32_t*>(dst + plane_stride) = lo;
+#else
+  float ha, la, hb, lb;
+  split_tf32(a, ha, la);
+  split_tf32(b, hb, lb);
+  *reinterpret_cast<float2*>(dst) = make_float2(ha, hb);
+  *reinterpret_cast<float2*>(dst + plane_stride) = make_float2(la, lb);
 #endif
 }
 
-// MC = 1: independent CTAs.  MC = 2: weight multicast - the two CTAs of a cluster work on two pixel tiles of the SAME
-// output-channel block in lock step per weight stage: CTA r loads plane r (hi / lo) of every stage with a TMA multicast
-// into both CTAs' rings, both CTAs' full barriers count the bytes of both loads, a stage is free again when BOTH issuers'
-// MMAs on it have retired (multicast commit on both CTAs' empty barriers, count 2).  Half the L2 -> SM weight bytes per MAC:
-// the deep layers sit at the chip's L2 throughput cap (DESIGN.md section 4.1).  Everything else - activations, MMAs
-// (cta_group::1), epilogue - is per CTA and unchanged.
-template <int BN, int MC>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBX,
-               const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmPool, const ConvParams p) {
+__device__ __forceinline__ float2 ldg2_or_zero(const float* p, int c) {
+  return p ? __ldg(reinterpret_cast<const float2*>(p + c)) : make_float2(0.f, 0.f);
+}
+
+// One consumer warpgroup: the wgmma loop over every tile of the CTA for its 64 rows, then the tile's epilogue.
+// The accumulator fragment of a thread covers two pixels - image rows y and y + 1 of column x - and BN / 4 channels
+// (pairs c, c + 1 at c = n0 + 8 j + 2 (lane % 4)).
+template <int BN, int TAPS, int MC>
+__device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem_a, uint32_t smem_b, uint32_t full0,
+                                              uint32_t empty0, uint32_t afull0, uint32_t aempty0, const float* s_head_w,
+                                              const float* s_head_b) {
   using C = Cfg<BN>;
+  constexpr int NA = BN / 2;  // accumulator registers per thread for BN columns
   constexpr int STAGES = C::STAGES;
-  constexpr int NBUF = C::NBUF;
-  constexpr int HALVES = C::HALVES, EGROUPS = C::EGROUPS;
-  constexpr int NC = BN / HALVES;  // accumulator columns held by one epilogue thread (64)
-
-  extern __shared__ __align__(1024) uint8_t smem[];   // layout: Cfg<BN> (conv_tc_common.cuh); no static shared memory
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BARS);
-  uint32_t& tmem_base_s = *reinterpret_cast<uint32_t*>(smem + C::OFF_TMEM);
-  float* s_head_w = reinterpret_cast<float*>(smem + C::OFF_HEAD);          // present for BN = 64 only (kModeHead)
-  float* s_head_b = s_head_w + MAX_CLASSES * 64;
-
-  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[STAGES]);
-  const uint32_t tfull0 = smem_u32(&bars[2 * STAGES]), tempty0 = smem_u32(&bars[2 * STAGES + EGROUPS * NBUF]);
-  const uint32_t afull0 = smem_u32(&bars[2 * STAGES + (EGROUPS + 1) * NBUF]), aempty0 = afull0 + 8 * NUM_A_BUFS;
-  uint8_t* smem_b = smem + C::OFF_B;
-  uint8_t* smem_out = smem + C::OFF_STG;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
+  constexpr int PATCH_W = (TAPS == 9) ? HALO_W : TILE_W;  // shared-memory rows per image row of the patch
+  constexpr uint32_t A_PLANE = (uint32_t)((TAPS == 9) ? A_PLANE_BYTES_3x3 : A_PLANE_BYTES_1x1);
+  constexpr uint32_t SBO_A = PATCH_W * ROW_BYTES;
+  const int tid = threadIdx.x - 128;
+  const int half = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
+  const int g = lane >> 2, qd = lane & 3;
   const int tiles_x = p.W / TILE_W, tiles_img = tiles_x * (p.H / TILE_H);
   const int n_tiles = p.Cout / BN;
   const int total_tiles = p.N * tiles_img * n_tiles;
-  const int taps = p.taps;
   const int num_cb = (p.C0 + p.C1) / BK;
-  const int num_kb = num_cb * taps;
-  const int a_plane_bytes = taps == 9 ? A_PLANE_BYTES_3x3 : A_PLANE_BYTES_1x1;
-  const int halo = taps == 9 ? 1 : 0;
-  const int chunk_kb = p.chunk_kb;
-  const int num_chunks = (num_kb + chunk_kb - 1) / chunk_kb;
-  // Two MMA-issuing warps take alternate chunks unless a chunk spans a whole weight ring (then the issuer that
-  // does not own it could fall a full ring behind and its phase bit would alias); see mma_issue_loop.
-  const bool dual_issue = (MC == 1) && p.dual_issue && (chunk_kb <= STAGES - 1) && (num_chunks >= 2);
-  // work items: tiles (MC = 1) or clusters' tile groups (MC pixel tiles of one channel block, this CTA takes pixel tile
-  // MC * group + rank); every CTA of a cluster walks the same item sequence
-  const uint32_t rank = (MC > 1) ? cluster_ctarank() : 0u;
-  const int first_item = (int)blockIdx.x / MC, item_step = (int)gridDim.x / MC, total_items = total_tiles / MC;
-  auto tile_of = [&](int q) { if (MC == 1) return q; const int mtp = q / n_tiles; return (MC * mtp + (int)rank) * n_tiles + (q - mtp * n_tiles); };
+  const int num_kb = num_cb * TAPS, chunk_kb = p.chunk_kb;
+  const uint32_t a_half = (uint32_t)(8 * half * PATCH_W * ROW_BYTES);
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, MC); }
-    for (int s = 0; s < NUM_A_BUFS; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, dual_issue ? 2 : 1); }
-    for (int b = 0; b < EGROUPS * NBUF; ++b) mbar_init(tfull0 + 8 * b, 1);
-    for (int b = 0; b < NBUF; ++b) mbar_init(tempty0 + 8 * b, NUM_EPI_THREADS / 32 / EGROUPS);
-    fence_mbar_init();
-    tma_prefetch_desc(&tmA0); tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmOut); tma_prefetch_desc(&tmPool);
+  const WorkItems<MC> items(total_tiles, n_tiles);
+  float S[NA], P[NA], Q[NA];   // round-to-nearest sum of hi*hi | open chunk of hi*hi | corrections (x 2^11 for fp16)
+  uint32_t s = 0, ph = 0, ab = 0, aph = 0;
+  auto release = [&](uint32_t st, int a) {   // a weight stage (and an activation buffer, a >= 0) may be refilled
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(empty0 + 8 * st);
+      if (MC > 1) mbar_arrive_cluster(empty0 + 8 * st, items.rank ^ 1u);   // the peer's producer also fills this stage
+      if (a >= 0) mbar_arrive(aempty0 + 8 * a);
+    }
+  };
+  auto mma_one = [&](float (&D)[NA], uint64_t da, uint64_t db, int acc) {
+    if constexpr (BN == 128) wgmma_n128(D, da, db, acc); else wgmma_n64(D, da, db, acc);
+  };
+
+  for (int item = items.first; item < items.total; item += items.step) {
+    const TileCoord t = decode_tile(items.tile(item), n_tiles, tiles_x, tiles_img, BN);
+#pragma unroll
+    for (int i = 0; i < NA; ++i) { S[i] = 0.f; Q[i] = 0.f; }
+    // Chunks of chunk_kb k-blocks.  Inside a chunk every k-block is one committed wgmma group and the wait is for the
+    // PREVIOUS group only, so the tensor core always has the next group queued; the chunk ends with an unconditional
+    // wait for all groups before its hi*hi partial sum is read (every path to a read of P or Q passes a full wait, so
+    // ptxas keeps the wgmmas asynchronous).
+    for (int kb0 = 0; kb0 < num_kb; kb0 += chunk_kb) {
+      const int kb1 = min(kb0 + chunk_kb, num_kb);
+      uint32_t pend_s = 0;
+      int pend_a = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const int tap = (TAPS == 9) ? kb % 9 : 0;
+        if (tap == 0) mbar_spin(afull0 + 8 * ab, aph);
+        // tap (dy, dx) = the channel block's patch entered (dy * PATCH_W + dx) rows further
+        const uint32_t a_tap = smem_a + ab * (uint32_t)A_BUF_BYTES + a_half + (uint32_t)(((tap / 3) * PATCH_W + (tap % 3)) * ROW_BYTES);
+        const uint32_t b_st = smem_b + s * (uint32_t)C::STAGE_BYTES;
+        mbar_spin(full0 + 8 * s, ph);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < ROW_BYTES / 32; ++k) {
+          const uint64_t ah = make_desc_sw128(a_tap + 32 * k, SBO_A), al = make_desc_sw128(a_tap + A_PLANE + 32 * k, SBO_A);
+          const uint64_t bh = make_desc_sw128(b_st + 32 * k, 1024), bl = make_desc_sw128(b_st + C::B_PLANE_BYTES + 32 * k, 1024);
+          mma_one(P, ah, bh, k != 0 || kb != kb0);   // hi*hi (a chunk's first k-step restarts it from zero)
+          mma_one(Q, ah, bl, 1);                      // hi*lo
+          mma_one(Q, al, bh, 1);                      // lo*hi
+        }
+        wgmma_commit();
+        if (kb > kb0) {
+          wgmma_wait<1>();           // the previous k-block's group is done: its stage can be refilled
+          release(pend_s, pend_a);
+        }
+        pend_s = s;
+        pend_a = (tap == TAPS - 1) ? (int)ab : -1;   // a channel block's last tap frees its activation buffer
+        if (++s == STAGES) { s = 0; ph ^= 1u; }
+        if (tap == TAPS - 1 && ++ab == NUM_A_BUFS) { ab = 0; aph ^= 1u; }
+      }
+      wgmma_wait<0>();
+      release(pend_s, pend_a);
+#pragma unroll
+      for (int i = 0; i < NA; ++i) S[i] += P[i];
+    }
+#pragma unroll
+    for (int i = 0; i < NA; ++i) S[i] += Q[i] * kLoUnscale;   // exact power-of-two rescale of hi*lo + lo*hi
+
+    // ---- epilogue.  acc * in_unscale undoes the operands' power-of-two scales (1.0 unless the engine rescaled a
+    // tensor); the product is exact, so fma(acc, unscale, bias) rounds exactly like the separate multiply and add.
+    const float unscale = p.in_unscale;
+    const int y = t.y0 + 8 * half + 2 * wq, x = t.x0 + g;   // registers 4j, 4j+1: row y; 4j+2, 4j+3: row y + 1
+    const int c0 = t.n0 + 2 * qd;
+    if (p.mode == kModeLinear) {
+      float* out = static_cast<float*>(p.out);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = c0 + 8 * j;
+        const float2 b = ldg2_or_zero(p.bias, c);
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          *reinterpret_cast<float2*>(out + (((size_t)t.n * p.H + y + r) * p.W + x) * p.Cout + c) =
+              make_float2(__fmaf_rn(S[4 * j + 2 * r], unscale, b.x), __fmaf_rn(S[4 * j + 2 * r + 1], unscale, b.y));
+      }
+      continue;
+    }
+    // y = relu(acc + bias) * scale + shift   (Conv -> ReLU -> BatchNorm(eval), resunet.py:93-105).  The stored planes
+    // hold y * out_scale: the power-of-two factor goes into scale and shift (it commutes with every rounding involved);
+    // the head consumes y itself.
+    const float cscale = (p.mode == kModeHead) ? 1.f : p.out_scale;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = c0 + 8 * j;
+      const float2 b = ldg2_or_zero(p.bias, c), sc = ldg2_or_zero(p.scale, c), sh = ldg2_or_zero(p.shift, c);
+      const float s0 = sc.x * cscale, s1 = sc.y * cscale, h0 = sh.x * cscale, h1 = sh.y * cscale;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float& v0 = S[4 * j + 2 * r];
+        float& v1 = S[4 * j + 2 * r + 1];
+        v0 = __fadd_rn(__fmul_rn(fmaxf(__fmaf_rn(v0, unscale, b.x), 0.f), s0), h0);
+        v1 = __fadd_rn(__fmul_rn(fmaxf(__fmaf_rn(v1, unscale, b.y), 0.f), s1), h1);
+      }
+    }
+    if (BN == 64 && p.mode == kModeHead) {
+      // 1x1 head (resunet.py:69): the four lanes of a quad hold a pixel's 64 channels (16 each)
+      float lg[2][MAX_CLASSES];
+#pragma unroll
+      for (int k = 0; k < MAX_CLASSES; ++k) {
+        float d0 = 0.f, d1 = 0.f;
+        if (k < p.K) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float w = s_head_w[k * 64 + 8 * j + 2 * qd + e];
+              d0 = fmaf(w, S[4 * j + e], d0);
+              d1 = fmaf(w, S[4 * j + 2 + e], d1);
+            }
+          }
+        }
+        d0 += __shfl_xor_sync(0xffffffffu, d0, 1);
+        d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
+        d0 += __shfl_xor_sync(0xffffffffu, d0, 2);
+        d1 += __shfl_xor_sync(0xffffffffu, d1, 2);
+        lg[0][k] = (k < p.K) ? d0 + s_head_b[k] : -INFINITY;
+        lg[1][k] = (k < p.K) ? d1 + s_head_b[k] : -INFINITY;
+      }
+      if (qd == 0) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float mx = -INFINITY;
+#pragma unroll
+          for (int k = 0; k < MAX_CLASSES; ++k) mx = fmaxf(mx, lg[r][k]);
+          float se = 0.f;
+#pragma unroll
+          for (int k = 0; k < MAX_CLASSES; ++k) if (k < p.K) se += expf(lg[r][k] - mx);
+          const float lse = logf(se);
+          int best = 0;
+          float bestv = -INFINITY;
+#pragma unroll
+          for (int k = 0; k < MAX_CLASSES; ++k) {
+            if (k < p.K) {
+              const float sc = (lg[r][k] - mx) - lse;  // LogSoftmax(dim=1), resunet.py:70
+              if (sc > bestv) { bestv = sc; best = k; }  // first index wins ties (mask.py:185)
+              if (p.scores) p.scores[(((size_t)t.n * p.K + k) * p.H + y + r) * p.W + x] = sc;
+            }
+          }
+          p.labels[((size_t)t.n * p.H + y + r) * p.W + x] = (uint8_t)best;
+        }
+      }
+      continue;
+    }
+#if LM_OPERAND_F16
+    {  // fp16 saturates: report instead of storing inf (the engine lowers out_scale and runs again)
+      bool ovf = false;
+#pragma unroll
+      for (int i = 0; i < NA; ++i) ovf |= !(fabsf(S[i]) <= kOpMax);
+      if (__any_sync(0xffffffffu, ovf) && lane == 0 && p.range_flag) *p.range_flag = 1;
+    }
+#endif
+    {
+      const size_t plane = (size_t)p.H * p.W * p.Cout;
+      op_t* img = static_cast<op_t*>(p.out) + (size_t)t.n * 2 * plane;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+          store_split_pair(img + ((size_t)(y + r) * p.W + x) * p.Cout + c0 + 8 * j, plane, S[4 * j + 2 * r], S[4 * j + 2 * r + 1]);
+    }
+    if (p.mode == kModeReluBnPool) {
+      // 2x2 average (resunet.py:64): a thread holds rows y and y + 1 of column x, lane ^ 4 holds column x ^ 1;
+      // (top-left + top-right) + (bottom-left + bottom-right), stored by the even-x lane
+      const int Hp = p.H / 2, Wp = p.W / 2;
+      const size_t plane = (size_t)Hp * Wp * p.Cout;
+      op_t* img = static_cast<op_t*>(p.out_pool) + (size_t)t.n * 2 * plane + ((size_t)(y >> 1) * Wp + (x >> 1)) * p.Cout + c0;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        float pv[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float top = S[4 * j + e] + __shfl_xor_sync(0xffffffffu, S[4 * j + e], 4);
+          const float bot = S[4 * j + 2 + e] + __shfl_xor_sync(0xffffffffu, S[4 * j + 2 + e], 4);
+          pv[e] = (top + bot) * 0.25f;
+        }
+        if ((g & 1) == 0) store_split_pair(img + 8 * j, plane, pv[0], pv[1]);
+      }
+    }
   }
-  if (warp == 2) tmem_alloc(smem_u32(&tmem_base_s), C::TMEM_COLS);
+}
+
+// MC = 1: independent CTAs.  MC = 2 (weight multicast): clusters of two CTAs work on two pixel tiles of the same
+// output-channel block in lock step; CTA r loads plane r (hi / lo) of every weight stage with one TMA multicast into both
+// CTAs' rings, each CTA's full barrier counts the bytes of both loads, and a stage is free again when the consumers of BOTH
+// CTAs have released it (empty barriers count the local and the remote arrivals).  Half the L2 -> SM weight bytes per MAC;
+// activations, wgmmas and epilogue are per CTA and unchanged, so the results are bit-identical to MC = 1.
+template <int BN, int MC>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBX, const ConvParams p) {
+  using C = Cfg<BN>;
+  constexpr int STAGES = C::STAGES;
+  extern __shared__ __align__(1024) uint8_t smem[];   // layout: Cfg<BN>; no static shared memory
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BARS);
+  float* s_head_w = reinterpret_cast<float*>(smem + C::OFF_HEAD);          // present for BN = 64 only (kModeHead)
+  float* s_head_b = s_head_w + MAX_CLASSES * 64;
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = full0 + 8 * STAGES;
+  const uint32_t afull0 = full0 + 16 * STAGES, aempty0 = afull0 + 8 * NUM_A_BUFS;
+  const uint32_t smem_a = smem_u32(smem), smem_b = smem_a + C::OFF_B;
+  const int warp = threadIdx.x >> 5;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, MC * NUM_CONSUMER_WARPS); }
+    for (int s = 0; s < NUM_A_BUFS; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, NUM_CONSUMER_WARPS); }
+    fence_mbar_init();
+    tma_prefetch_desc(&tmA0); tma_prefetch_desc(&tmA1); tma_prefetch_desc(MC > 1 ? &tmBX : &tmB);
+  }
   if (BN == 64 && p.mode == kModeHead) {
     for (int i = threadIdx.x; i < p.K * 64; i += NUM_THREADS) s_head_w[i] = p.head_w[i];
     if (threadIdx.x < p.K) s_head_b[threadIdx.x] = p.head_b[threadIdx.x];
   }
-  tc_fence_before();
   __syncthreads();
-  if (MC > 1) cluster_sync_all();  // the peer's barriers are initialised before any multicast load / commit signals them
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-#ifdef LM_CONV_PROFILE
-  const long long prof_kernel_t0 = clock64();
-#endif
+  if (MC > 1) cluster_sync_all();   // the peer's barriers are initialised before any multicast load or remote arrive
 
-  // Both single-issuer roles run as warp-uniform loops (all 32 lanes execute the control flow and poll the
-  // barriers, one elected lane issues the TMA / MMA / commit): loop state then lives in uniform registers
-  // and the issue thread is not throttled by divergent-code bookkeeping.
-  // Register reallocation (setmaxnreg): warps 0-3 (producer, issuer(s), TMEM allocator) give registers to the two epilogue
-  // warpgroups, whose chunk drains hold 3 x 64 fp32 values per thread: 128 x LM_REGS_LOW + 256 x LM_REGS_HIGH <= 384 x 168.
-  // Each branch starts with its warpgroups' setmaxnreg and the branches only meet again at the kernel's last barrier.
-  if (warp >= EPI_WARP0) {
-#if LM_SETMAXNREG
-    setmaxnreg_inc<LM_REGS_HIGH>();
-#endif
-    // ------------------------------------------------------------------ epilogue warps
-    conv_epilogue_warps<BN, false>(p, &tmOut, &tmPool, tmem_base, tfull0, tempty0, smem_out, reinterpret_cast<float*>(smem + C::OFF_CONST), s_head_w, s_head_b, first_item,
-                                   total_items, item_step, tile_of, num_chunks);
-    tc_fence_before();
-    __syncthreads();   // the kernel's last barrier (the other warps arrive at it from their own branch)
-    if (MC > 1) cluster_sync_all();
-    return;
+  if (warp >= 4) {
+    setmaxnreg_inc<REGS_CONSUMER>();
+    if (p.taps == 9) conv_consumer<BN, 9, MC>(p, smem_a, smem_b, full0, empty0, afull0, aempty0, s_head_w, s_head_b);
+    else conv_consumer<BN, 1, MC>(p, smem_a, smem_b, full0, empty0, afull0, aempty0, s_head_w, s_head_b);
   } else {
-#if LM_SETMAXNREG
-    setmaxnreg_dec<LM_REGS_LOW>();
-#endif
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    uint32_t s = 0, ph = 0, ab = 0, aph = 0;
-    const uint32_t a_tx = 2u * (uint32_t)a_plane_bytes;
-    for (int item = first_item; item < total_items; item += item_step) {
-      const int tile = tile_of(item);
-      const TileCoord t = decode_tile(tile, n_tiles, tiles_x, tiles_img, BN);
-      int c = 0;
-      for (int cb = 0; cb < num_cb; ++cb, c += BK) {
-        // the activation patch (+ halo) of this channel block, both planes, once for all taps
-        { LM_PROF_T0(); mbar_wait(aempty0 + 8 * ab, aph ^ 1); if (lane == 0) LM_PROF_ADD(0); }
-        if (elect_one()) {
-          mbar_arrive_expect_tx(afull0 + 8 * ab, a_tx);
-          const uint32_t dst = smem_u32(smem) + ab * A_BUF_BYTES;
-          if (c < p.C0) tma_load_5d(dst, &tmA0, afull0 + 8 * ab, c, t.x0 - halo, t.y0 - halo, 0, t.n);
-          else          tma_load_5d(dst, &tmA1, afull0 + 8 * ab, c - p.C0, t.x0 - halo, t.y0 - halo, 0, t.n);
-        }
-        __syncwarp();
-        if (++ab == NUM_A_BUFS) { ab = 0; aph ^= 1; }
-        for (int tap = 0; tap < taps; ++tap) {
-          { LM_PROF_T0(); mbar_wait(empty0 + 8 * s, ph ^ 1); if (lane == 0) LM_PROF_ADD(1); }
+    setmaxnreg_dec<REGS_PRODUCER>();
+    if (warp == 0) {
+      // -------------------------------------------------------------- TMA producer (warp 0, one elected lane issues)
+      const int tiles_x = p.W / TILE_W, tiles_img = tiles_x * (p.H / TILE_H);
+      const int n_tiles = p.Cout / BN;
+      const WorkItems<MC> items(p.N * tiles_img * n_tiles, n_tiles);
+      const int taps = p.taps, halo = taps == 9 ? 1 : 0;
+      const int num_cb = (p.C0 + p.C1) / BK;
+      const uint32_t a_tx = 2u * (uint32_t)(taps == 9 ? A_PLANE_BYTES_3x3 : A_PLANE_BYTES_1x1);
+      uint32_t s = 0, ph = 0, ab = 0, aph = 0;
+      for (int item = items.first; item < items.total; item += items.step) {
+        const TileCoord t = decode_tile(items.tile(item), n_tiles, tiles_x, tiles_img, BN);
+        int c = 0;
+        for (int cb = 0; cb < num_cb; ++cb, c += BK) {
+          // the activation patch (+ halo) of this channel block, both planes, once for all taps
+          mbar_wait_inline(aempty0 + 8 * ab, aph ^ 1);
           if (elect_one()) {
-            if ((LM_EXP & 32) && (tile != (int)blockIdx.x || cb > 0 || tap >= STAGES)) {
-              mbar_arrive(full0 + 8 * s);  // ablation: reuse whatever the stage holds
-            } else if (MC > 1) {
-              // this CTA's plane of the stage, into both CTAs' rings; the local barrier expects both planes
-              mbar_arrive_expect_tx(full0 + 8 * s, C::STAGE_BYTES);
-              tma_load_4d_mcast(smem_u32(smem_b) + s * C::STAGE_BYTES + rank * (uint32_t)C::B_PLANE_BYTES, &tmBX, full0 + 8 * s, c, t.n0, tap,
-                                (int)rank, (uint16_t)((1u << MC) - 1u));
-            } else {
-              mbar_arrive_expect_tx(full0 + 8 * s, C::STAGE_BYTES);
-              tma_load_4d(smem_u32(smem_b) + s * C::STAGE_BYTES, &tmB, full0 + 8 * s, c, t.n0, tap, 0);
-            }
+            mbar_arrive_expect_tx(afull0 + 8 * ab, a_tx);
+            const uint32_t dst = smem_a + ab * A_BUF_BYTES;
+            if (c < p.C0) tma_load_5d(dst, &tmA0, afull0 + 8 * ab, c, t.x0 - halo, t.y0 - halo, 0, t.n);
+            else          tma_load_5d(dst, &tmA1, afull0 + 8 * ab, c - p.C0, t.x0 - halo, t.y0 - halo, 0, t.n);
           }
           __syncwarp();
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+          if (++ab == NUM_A_BUFS) { ab = 0; aph ^= 1; }
+          for (int tap = 0; tap < taps; ++tap) {
+            mbar_wait_inline(empty0 + 8 * s, ph ^ 1);
+            if (elect_one()) {
+              mbar_arrive_expect_tx(full0 + 8 * s, C::STAGE_BYTES);   // MC = 2: this CTA's plane and the peer's
+              if (MC > 1)
+                tma_load_4d_mcast(smem_b + s * C::STAGE_BYTES + items.rank * (uint32_t)C::B_PLANE_BYTES, &tmBX, full0 + 8 * s, c, t.n0,
+                                  tap, (int)items.rank, (uint16_t)((1u << MC) - 1u));
+              else
+                tma_load_4d(smem_b + s * C::STAGE_BYTES, &tmB, full0 + 8 * s, c, t.n0, tap, 0);
+            }
+            __syncwarp();
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
         }
       }
     }
-    if (MC > 1) {
-      // cluster tail: the releases of the last STAGES k-blocks (commits from BOTH CTAs' issuers) have landed on this CTA's
-      // barriers before it may exit - no signal is left in flight towards shared memory that a later CTA could own
-      for (int i = 0; i < STAGES; ++i) {
-        mbar_wait(empty0 + 8 * s, ph ^ 1);
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == 1 || warp == 3) {
-    // ------------------------------------------------------------------ MMA issuers (two warps, one lane each)
-    // ncu (profiles/r01_ncu_conv_issuer.md) showed the previous warp-uniform issue loops spending ~60 % of their
-    // time in per-k-block bookkeeping (~150 scalar instructions at ~8 cycles each for a lone warp), with the tensor
-    // pipe idle meanwhile.  The loop therefore runs in ONE lane, the nine taps are unrolled with compile-time
-    // descriptor offsets, and the state per k-block is a ring index, a phase bit and a chunk counter.
-    if (elect_one()) {  // (elect.sync, not lane == 0: the compiler then knows the region is single-lane and
-                        //  feeds the MMA's uniform-register operands without per-lane broadcast loops)
-      const uint32_t me = (warp == 3) ? 1u : 0u;
-      if (dual_issue || me == 0u) {
-        IssueArgs ia;
-        ia.me = me; ia.first_tile = first_item; ia.total_tiles = total_items; ia.tile_step = item_step;
-        ia.num_cb = num_cb; ia.chunk_kb = chunk_kb; ia.tmem_base = tmem_base;
-        ia.smem_a = smem_u32(smem); ia.smem_b = smem_u32(smem_b);
-        ia.full0 = full0; ia.empty0 = empty0; ia.tfull0 = tfull0; ia.tempty0 = tempty0; ia.afull0 = afull0; ia.aempty0 = aempty0;
-        if (dual_issue) { if (taps == 9) mma_issue_loop<BN, 9, true>(ia); else mma_issue_loop<BN, 1, true>(ia); }
-        else if (taps != 9) mma_issue_loop<BN, 1, false, true, MC>(ia);
-        else if (LM_TAP_LOOP == 2 || (LM_TAP_LOOP == 1 && BN == 64 && num_cb == 1)) mma_issue_loop<BN, 9, false, false, MC>(ia);
-        else mma_issue_loop<BN, 9, false, true, MC>(ia);
-      }
-    }
-    __syncwarp();
   }
-  }
-  tc_fence_before();
-  __syncthreads();
-#ifdef LM_CONV_PROFILE
-  if (threadIdx.x == 0) atomicAdd(&g_conv_prof[9], (unsigned long long)(clock64() - prof_kernel_t0));
-#endif
+  // MC = 2: no CTA leaves while its peer may still multicast into its shared memory or arrive on its barriers
   if (MC > 1) cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -440,46 +463,14 @@ int make_conv_maps(ConvMaps* maps, const void* src0, const void* src1, const voi
   r = (p.C1 > 0) ? make_act_map(&maps->a1, src1, n_capacity, p.H, p.W, p.C1, p.taps)
                  : make_act_map(&maps->a1, src0, n_capacity, p.H, p.W, p.C0, p.taps);
   if (r) return r;
-  // TMA-store maps: one epilogue warp's rows per store
-  if (p.mode == kModeReluBn || p.mode == kModeReluBnPool) {
-    cuuint64_t od[5] = {(cuuint64_t)p.Cout, (cuuint64_t)p.W, (cuuint64_t)p.H, 2, (cuuint64_t)n_capacity};
-    cuuint64_t os[4] = {(cuuint64_t)p.Cout * E, (cuuint64_t)p.W * p.Cout * E, (cuuint64_t)p.H * p.W * p.Cout * E,
-                        (cuuint64_t)2 * p.H * p.W * p.Cout * E};
-    cuuint32_t ob[5] = {BK, TILE_W, 4, 1, 1};  // one epilogue warp: BK channels (128 B) x 8 x 4 pixels of one plane
-    r = encode(&maps->out, kOpType, p.out, 5, od, os, ob);
-    if (r) return r;
-  } else if (p.mode == kModeLinear) {
-    cuuint64_t od[4] = {(cuuint64_t)p.Cout, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)n_capacity};
-    cuuint64_t os[3] = {(cuuint64_t)p.Cout * 4, (cuuint64_t)p.W * p.Cout * 4, (cuuint64_t)p.H * p.W * p.Cout * 4};
-    cuuint32_t ob[4] = {F32_ROW_CH, TILE_W, 4, 1};
-    r = encode(&maps->out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.out, 4, od, os, ob);
-    if (r) return r;
-  } else {
-    maps->out = maps->a0;
-  }
-  if (p.mode == kModeReluBnPool) {
-    const int Hp = p.H / 2, Wp = p.W / 2;
-    cuuint64_t od[5] = {(cuuint64_t)p.Cout, (cuuint64_t)Wp, (cuuint64_t)Hp, 2, (cuuint64_t)n_capacity};
-    cuuint64_t os[4] = {(cuuint64_t)p.Cout * E, (cuuint64_t)Wp * p.Cout * E, (cuuint64_t)Hp * Wp * p.Cout * E,
-                        (cuuint64_t)2 * Hp * Wp * p.Cout * E};
-    cuuint32_t ob[5] = {BK, TILE_W / 2, 2, 1, 1};
-    r = encode(&maps->pool, kOpType, p.out_pool, 5, od, os, ob);
-    if (r) return r;
-  } else {
-    maps->pool = maps->a0;
-  }
   const int Cin = p.C0 + p.C1;
   cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)p.Cout, (cuuint64_t)p.taps, 2};
   cuuint64_t strides[3] = {(cuuint64_t)Cin * E, (cuuint64_t)p.Cout * Cin * E, (cuuint64_t)p.taps * p.Cout * Cin * E};
-  cuuint32_t box[4] = {BK, (cuuint32_t)BN, 1, 2};
+  cuuint32_t box[4] = {BK, (cuuint32_t)BN, 1, 2}, box_x[4] = {BK, (cuuint32_t)BN, 1, 1};   // both planes / one plane
   r = encode(&maps->b, kOpType, weights, 4, dims, strides, box);
-  if (r) return r;
-  // weight boxes of the CTA-pair kernel (optional: a failure only disables that kernel)
-  cuuint32_t box_x[4] = {BK, (cuuint32_t)BN, 1, 1}, box_yw[4] = {BK, (cuuint32_t)(BN / 2), 1, 2};
-  maps->pair_ok = (encode(&maps->bx, kOpType, weights, 4, dims, strides, box_x) == 0 &&
-                   encode(&maps->byw, kOpType, weights, 4, dims, strides, box_yw) == 0) ? 1 : 0;
-  return 0;
+  return r ? r : encode(&maps->bx, kOpType, weights, 4, dims, strides, box_x);
 }
+
 
 template <int BN, int MC>
 static int launch_impl(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t stream) {
@@ -488,18 +479,11 @@ static int launch_impl(const ConvMaps& maps, const ConvParams& p, int num_sms, c
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return -9;
   if (!((attr_set_mask.load(std::memory_order_acquire) >> dev) & 1ull)) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg<BN>::DYN_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::DYN_SMEM);
     if (e != cudaSuccess) return (int)e;
     attr_set_mask.fetch_or(1ull << dev, std::memory_order_release);
   }
   const int total = p.N * (p.H / TILE_H) * (p.W / TILE_W) * (p.Cout / BN);
-  if (MC == 1) {
-    const int grid = total < num_sms ? total : num_sms;
-    conv_tc_kernel<BN, 1><<<grid, NUM_THREADS, Cfg<BN>::DYN_SMEM, stream>>>(maps.a0, maps.a1, maps.b, maps.bx, maps.out, maps.pool, p);
-    return (int)cudaGetLastError();
-  }
-  // clusters of MC CTAs: MC pixel tiles of one channel block per work item (every level has an even number of pixel tiles)
   const int groups = total / MC, sm_groups = num_sms / MC;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(MC * (groups < sm_groups ? groups : sm_groups)), 1, 1);
@@ -511,14 +495,9 @@ static int launch_impl(const ConvMaps& maps, const ConvParams& p, int num_sms, c
   attr[0].val.clusterDim.x = MC; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, MC>, maps.a0, maps.a1, maps.b, maps.bx, maps.out, maps.pool, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, MC>, maps.a0, maps.a1, maps.b, maps.bx, p);
   return (int)(e != cudaSuccess ? e : cudaGetLastError());
 }
-
-#ifdef LM_CONV_PROFILE
-void conv_prof_reset() { unsigned long long z[16] = {}; cudaMemcpyToSymbol(g_conv_prof, z, sizeof(z)); }
-void conv_prof_read(unsigned long long* out) { cudaMemcpyFromSymbol(out, g_conv_prof, 16 * sizeof(unsigned long long)); }
-#endif
 
 // Sets the kernels' > 48 KB dynamic shared-memory opt-in on the current device (lm_create calls it, so that no launch -
 // in particular none inside a CUDA-graph capture - has to).
@@ -535,8 +514,7 @@ int launch_conv_tc(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaS
   if (p.chunk_kb < 1) return -5;
   if (p.weight_mcast == 2)
     return conv_tile_n(p) == 128 ? launch_impl<128, 2>(maps, p, num_sms, stream) : launch_impl<64, 2>(maps, p, num_sms, stream);
-  return conv_tile_n(p) == 128 ? launch_impl<128, 1>(maps, p, num_sms, stream)
-                               : launch_impl<64, 1>(maps, p, num_sms, stream);
+  return conv_tile_n(p) == 128 ? launch_impl<128, 1>(maps, p, num_sms, stream) : launch_impl<64, 1>(maps, p, num_sms, stream);
 }
 
 }  // namespace lm

@@ -6,15 +6,15 @@
 #include <stdint.h>
 
 // Operand format of the tensor-core convolutions (compile-time, one format per build):
-//   1 (default)  fp16 pairs, tcgen05 kind::f16:  x = hi + lo * 2^-11, hi = fp16(x), lo = fp16((x - hi) * 2^11).
+//   1 (default)  fp16 pairs, wgmma .f16:  x = hi + lo * 2^-11, hi = fp16(x), lo = fp16((x - hi) * 2^11).
 //                Both halves carry 11 significant bits (as tf32 does), every product is exact in fp32, and an
-//                MMA instruction covers K = 16 at the rate kind::tf32 covers K = 8: the 3-product scheme runs
+//                MMA instruction covers K = 16 at the rate .tf32 covers K = 8: the 3-product scheme runs
 //                at twice the tf32 rate and moves half the bytes.  The scaled low half keeps the residuals
 //                of small values out of the fp16 subnormal range; the hi*lo + lo*hi accumulator is multiplied
 //                by 2^-11 when it is read.  fp16 saturates at 65504: the epilogues raise ConvParams::range_flag
 //                when a value leaves that range; the engine then lowers that tensor's power-of-two scale
 //                (ConvParams::out_scale) and runs the forward again - exact, and never a wrong mask.
-//   0            tf32 pairs, kind::tf32 (round 1's first scheme; no range limit, half the throughput).
+//   0            tf32 pairs, wgmma .tf32 (no range limit, half the throughput).
 #ifndef LM_OPERAND_F16
 #define LM_OPERAND_F16 1
 #endif
@@ -52,11 +52,10 @@ struct ConvParams {
   int taps;           // 9 (3x3, pad 1) or 1 (1x1)
   int mode;           // ConvMode
   int chunk_kb;       // k-blocks (kBK channels x 1 tap) accumulated inside the tensor core before the
-                      // partial sum is added, round-to-nearest, into fp32 registers
-  int dual_issue;     // 1: two MMA-issuing threads take alternate chunks (0: one issuer)
-  int weight_mcast;   // 2: clusters of two CTAs share every weight stage through TMA multicast (conv_tc.cu, MC = 2); 0 / 1: off
-  int tile_n;         // output-channel tile: 0 = conv_tile_n(Cout); 64 forces the BN = 64 kernel (two epilogue groups on
-                      // alternate tiles) for a layer with Cout >= 128 - must be set before make_conv_maps
+                      // partial sum is added, round-to-nearest, into an fp32 register sum
+  int weight_mcast;   // 2: clusters of two CTAs share every weight stage through TMA multicast (conv_tc.cu, MC = 2); 0: off
+  int tile_n;         // output-channel tile: 0 = conv_tile_n(Cout); 64 forces the BN = 64 kernel for a layer with
+                      // Cout >= 128 - must be set before make_conv_maps
   const float* bias;  // [Cout]
   const float* scale; // [Cout]  folded BN:  y = relu(.) * scale + shift
   const float* shift; // [Cout]
@@ -78,11 +77,7 @@ struct ConvParams {
 // Tensor maps for one launch (built once per layer by make_conv_maps).
 struct ConvMaps {
   CUtensorMap a0, a1, b;
-  CUtensorMap out, pool;  // TMA-store maps of the output tile (mode 0/1/2) and of the pooled tile (mode 1)
-  // weight boxes of the CTA-pair kernel (conv_tc_pair.cu): bx = (BK cin, BN cout, 1 tap, 1 plane),
-  // byw = (BK cin, BN/2 cout, 1 tap, 2 planes); pair_ok = both were encoded
-  CUtensorMap bx, byw;
-  int pair_ok;
+  CUtensorMap bx;  // weights, one plane per box: the per-CTA half of a multicast weight stage (weight_mcast = 2)
 };
 
 // Builds the TMA descriptors. src1 may be nullptr when C1 == 0. Returns 0 on success.
@@ -92,12 +87,8 @@ int make_conv_maps(ConvMaps* maps, const void* src0, const void* src1, const voi
 // Launches the convolution on `stream`. Returns a cudaError_t value (0 = ok).
 int launch_conv_tc(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t stream);
 
-// CTA-pair variant (conv_tc_pair.cu, tcgen05 cta_group::2; experimental, see the file header). Same contract.
-int launch_conv_tc_pair(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t stream);
-
 // Per-device preparation (dynamic shared-memory opt-in of every kernel variant); returns a cudaError_t value.
 int conv_tc_prepare();
-int conv_tc_pair_prepare();
 
 // BN (output-channel tile) chosen for a given Cout.
 inline int conv_tile_n(int cout) { return cout >= 128 ? 128 : 64; }

@@ -199,18 +199,14 @@ struct lm_engine {
   int use_graphs = 1;     // 0: launch every kernel individually (also whenever per-launch conv timing or score taps are on)
   int64_t graph_launches = 0, graph_hits = 0;
   unsigned bn64_mask = 0; // bit i: layer i of LAYERS uses BN = 64 output-channel tiles although Cout >= 128 (read at lm_load_weights)
-  int dual_issue = 0;     // 1: two MMA-issuing threads per CTA on alternate chunks (conv_tc.cu)
-  int weight_mcast = 0;   // 2: clusters of two CTAs share each weight stage through TMA multicast (conv_tc.cu, MC = 2)
-  int cta_pairs = 0;      // 1: the cta_group::2 kernel (conv_tc_pair.cu): bit-identical on hardware, but slower than one CTA per tile
-                          //    so far (r02: 14.3 vs 8.7 ms per 37-slice wave, profiles/r02_*) - opt-in
   int stem_v2 = 3;        // stem kernel version: 0 stem_kernel, 1 stem_kernel_v2 - weights in registers, 4-pixel quads
                           // (bit-identical to stem_kernel, r02 GPU tests), 2 stem_kernel_v3 - shared input tile and weights,
                           // 3 (default) stem_kernel_v3 with the next tile's samples fetched one tile ahead
   int upsample_v2 = 2;    // 2 (default): upsample2x_cells_kernel<true> - one load per output sample, corners indexed statically;
                           // 1: the same with run-time corner selection, 0: upsample2x_kernel (all three bit-identical)
-  int chunk_kb = 1;       // k-blocks per TMEM chunk for the 64-channel layers (ring of 4 slots)
-  int chunk_kb_wide = 2;  // ... for the layers with Cout >= 128 (ring of 2 slots: chunk 1 leaves the tensor pipe waiting
-                          // for the drain; chunk 2 costs < 1e-5 of score accuracy there, tools/debug_gpu.py)
+  int weight_mcast = 0;   // 2: clusters of two CTAs share each weight stage through TMA multicast (conv_tc.cu, MC = 2)
+  int chunk_kb = 1;       // k-blocks per tensor-core chunk of hi*hi (conv_tc.cu) for the 64-channel layers
+  int chunk_kb_wide = 2;  // ... for the layers with Cout >= 128
 };
 
 namespace {
@@ -268,12 +264,11 @@ int forward_batch(lm_engine* e, Slot& s, const void* d_in, bool in_f32, int n, u
     ConvParams p = s.params[i];
     p.N = n;
     p.chunk_kb = (p.Cout >= 128) ? e->chunk_kb_wide : e->chunk_kb;
+    p.weight_mcast = e->weight_mcast;
     const LayerSpec& L = LAYERS[i];
     p.range_flag = L.dst >= 0 ? range + L.dst : nullptr;
     p.in_unscale = 1.f / (s.act_scale[L.src0] * s.lw[i].w_scale);   // src1 (virtual concat) shares src0's scale group
     p.out_scale = (L.mode == kModeReluBn || L.mode == kModeReluBnPool) ? s.act_scale[L.dst] : 1.f;
-    p.dual_issue = e->dual_issue;
-    p.weight_mcast = (e->weight_mcast == 2 && s.maps[i].pair_ok) ? 2 : 0;
     if (p.mode == kModeHead) { p.labels = d_labels; p.scores = d_scores; }
     if (time_convs) {
       if (e->ev_used + 2 > e->ev_pool.size()) {
@@ -281,7 +276,7 @@ int forward_batch(lm_engine* e, Slot& s, const void* d_in, bool in_f32, int n, u
       }
       cudaEventRecord(e->ev_pool[e->ev_used], e->st);
     }
-    RC(e->cta_pairs ? launch_conv_tc_pair(s.maps[i], p, e->num_sms, e->st) : launch_conv_tc(s.maps[i], p, e->num_sms, e->st));
+    RC(launch_conv_tc(s.maps[i], p, e->num_sms, e->st));
     if (time_convs) { cudaEventRecord(e->ev_pool[e->ev_used + 1], e->st); e->ev_used += 2; }
     e->launches++;
     if (up < 4 && UPS[up].after_layer == i) {
@@ -620,7 +615,8 @@ int lm_create(int device, int batch_capacity, lm_engine** out) {
   CU(cudaSetDevice(device));
   cudaDeviceProp prop;
   CU(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(-3, "lm_create: device %s is sm_%d%d; this build is sm_100a only", prop.name, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(-3, "lm_create: device %s is sm_%d%d; this build is sm_90a only", prop.name, prop.major, prop.minor);
   lm_engine* e = new lm_engine();
   e->device = device;
   e->B = batch_capacity;
@@ -640,9 +636,7 @@ int lm_create(int device, int batch_capacity, lm_engine** out) {
 static int create_resources(lm_engine* e) {
   const int batch_capacity = e->B;
   if (const char* c = getenv("LM_CHUNK_KB")) { int v = atoi(c); if (v >= 1) e->chunk_kb = e->chunk_kb_wide = v; }
-  if (const char* c = getenv("LM_DUAL_ISSUE")) e->dual_issue = atoi(c) != 0;
-  if (const char* c = getenv("LM_CTA_PAIRS")) e->cta_pairs = atoi(c) != 0;
-  if (const char* c = getenv("LM_WEIGHT_MCAST")) e->weight_mcast = atoi(c);
+  if (const char* c = getenv("LM_WEIGHT_MCAST")) e->weight_mcast = atoi(c) == 2 ? 2 : 0;
   if (const char* c = getenv("LM_GRAPHS")) e->use_graphs = atoi(c) != 0;
   if (const char* c = getenv("LM_BN64_MASK")) e->bn64_mask = (unsigned)strtoul(c, nullptr, 0);
   if (const char* c = getenv("LM_STEM_V2")) { const int v = atoi(c); e->stem_v2 = v < 0 ? 0 : (v > 3 ? 3 : v); }
@@ -651,7 +645,6 @@ static int create_resources(lm_engine* e) {
   if (const char* c = getenv("LM_MERGE_CTAS")) e->post.merge_ctas = atoi(c) > 0 ? atoi(c) : 0;
   if (const char* c = getenv("LM_CHUNK_KB_WIDE")) { int v = atoi(c); if (v >= 1) e->chunk_kb_wide = v; }
   RC(conv_tc_prepare());
-  RC(conv_tc_pair_prepare());
   CU(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
   for (int i = 0; i < 8; ++i) CU(cudaEventCreate(&e->ev[i]));
   for (int i = 0; i < 2; ++i) CU(cudaEventCreate(&e->ev_conv[i]));
@@ -1248,8 +1241,6 @@ int lm_set_option(lm_engine* e, const char* key, int value) {
   if (!strcmp(key, "time_convs")) { e->time_convs = value != 0; e->ev_used = 0; return 0; }
   if (!strcmp(key, "post_debug_stage")) { e->post.debug_stage = value; return 0; }
   if (!strcmp(key, "chunk_kb")) { if (value < 1) return fail(-1, "chunk_kb must be >= 1"); e->chunk_kb = e->chunk_kb_wide = value; return 0; }
-  if (!strcmp(key, "dual_issue")) { e->dual_issue = value != 0; return 0; }
-  if (!strcmp(key, "cta_pairs")) { e->cta_pairs = value != 0; return 0; }
   if (!strcmp(key, "weight_mcast")) { if (value != 0 && value != 2) return fail(-1, "weight_mcast must be 0 or 2"); e->weight_mcast = value; return 0; }
   if (!strcmp(key, "stem_v2")) { if (value < 0 || value > 3) return fail(-1, "stem_v2 must be 0, 1, 2 or 3"); e->stem_v2 = value; return 0; }
   if (!strcmp(key, "upsample_v2")) { e->upsample_v2 = value < 0 ? 0 : (value > 2 ? 2 : value); return 0; }

@@ -8,7 +8,7 @@
 // All are HBM-bound streaming kernels: each thread produces 16 bytes of each plane (CPT = 8 fp16 / 4 tf32
 // channels) so that every warp store instruction writes fully coalesced 128-byte runs.
 #include "forward_misc.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace lm {
 namespace {

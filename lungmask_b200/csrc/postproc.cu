@@ -1215,7 +1215,7 @@ int postprocess_device(PostScratch& ws, const uint8_t* d_labels, int S, int H, i
   // many CTAs when the device can co-schedule a grid (cooperative launch), else the one-CTA loop
   bool launched = false;
   if (ws.merge_ctas != 1) {
-    static std::atomic<int> coop_ok{-1};   // -1 unknown, 0 no, 1 yes (per process: every engine device is a B200)
+    static std::atomic<int> coop_ok{-1};   // -1 unknown, 0 no, 1 yes (per process: every engine device is an H100)
     if (coop_ok.load() < 0) {
       int dev = 0, v = 0;
       if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess) coop_ok.store(v ? 1 : 0);

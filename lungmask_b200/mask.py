@@ -1,4 +1,4 @@
-"""Host-side mirror of lungmask/mask.py for the B200 engine.
+"""Host-side mirror of lungmask/mask.py for the H100 engine.
 
 Same public names, arguments and error behaviour as the reference (`MODEL_URLS`, `get_model`,
 `LMInferer`, deprecated `apply` / `apply_fused`; lungmask/mask.py:22-35,38-68,71-232,235-279), but the
@@ -132,8 +132,8 @@ class LMInferer:
         """Same arguments as the reference (lungmask/mask.py:72-82) plus `device` (CUDA ordinal, default
         LOCAL_RANK or 0) and `wave_slices`.  The reference's `batch_size` only bounds memory (slices are
         independent, mask.py:172-187; the engine is batch-invariant, tests/test_gpu_forward.py); the engine
-        runs the forward in waves of `wave_slices` slices, default 37 when batch_size >= 20 because
-        37 x 16 tiles = 4 x 148 SMs fills every level of the U-Net with whole waves of CTAs (6 GB of
+        runs the forward in waves of `wave_slices` slices, default 33 when batch_size >= 20 because
+        33 x 16 tiles = 4 x 132 SMs fills every level of the U-Net with whole waves of CTAs (about 5 GB of
         activations), else batch_size."""
         assert modelname in MODEL_URLS, "Modelname not found. Please choose from: {}".format(MODEL_URLS.keys())
         if fillmodel is not None:
@@ -143,7 +143,7 @@ class LMInferer:
         if fillmodel_path is not None:
             fillmodel = os.path.basename(fillmodel_path)
         if force_cpu:
-            raise RuntimeError("lungmask_b200 is a B200 (sm_100a) engine and has no CPU path; "
+            raise RuntimeError("lungmask_b200 is an H100 (sm_90a) engine and has no CPU path; "
                                "use the reference package for force_cpu=True")
         self.fillmodel = fillmodel
         self.modelname = modelname
@@ -157,8 +157,8 @@ class LMInferer:
 
         self.model = get_model(self.modelname, modelpath)
         if wave_slices is None:
-            wave_slices = 37 if batch_size >= 20 else batch_size
-            if batch_size >= 20 and os.environ.get("LM_WAVE_SLICES"):   # measurement hook: 74 = eight CTA rounds per level
+            wave_slices = 33 if batch_size >= 20 else batch_size
+            if batch_size >= 20 and os.environ.get("LM_WAVE_SLICES"):   # measurement hook: 66 = eight CTA rounds per level
                 wave_slices = max(1, min(1024, int(os.environ["LM_WAVE_SLICES"])))
         self.wave_slices = wave_slices
         self.engine = _native.Engine(device=device, batch_capacity=wave_slices)

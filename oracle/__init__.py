@@ -9,7 +9,7 @@ CPU fallback.
 
 Pinning status (see DESIGN.md "Oracle"):
   * `oracle.restate` is checked in this container against the reference's own modules imported
-    verbatim from /root/reference (`oracle.ref_loader`) and against the reference's known-answer
+    verbatim from a reference checkout (`oracle.ref_loader`) and against the reference's known-answer
     tests (tests/test_utils.py:58-63,73-107,124-159), and against fixtures in tests/golden/ that
     were generated from the verbatim reference by `oracle/make_golden.py`.
   * The reference's third-party natives skimage / fill_voids are NOT installed here; their

@@ -1,8 +1,8 @@
-"""Import the UNMODIFIED reference modules from /root/reference (this container only).
+"""Import the UNMODIFIED reference modules from a reference checkout (LUNGMASK_REFERENCE_ROOT).
 
 TEST INFRASTRUCTURE ONLY.  Used by oracle/make_golden.py and by the `not gpu` tests that validate
-`oracle.restate` against the reference itself.  /root/reference does not exist on the GPU box, so
-nothing on a `-m gpu` test, smoke() or bench.py path may call this.
+`oracle.restate` against the reference itself.  Tests, smoke() and bench.py read the fixtures it
+produced (tests/golden/) and never call this.
 """
 import importlib
 import os
@@ -10,11 +10,13 @@ import sys
 
 from . import standins
 
-REFERENCE_ROOT = os.environ.get("LUNGMASK_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("LUNGMASK_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, "lungmask", "mask.py"))
+    """True when LUNGMASK_REFERENCE_ROOT names a directory holding the reference's lungmask/mask.py (no default: an
+    unset or empty value never falls back to whatever the current directory holds)."""
+    return bool(REFERENCE_ROOT) and os.path.isabs(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, "lungmask", "mask.py"))
 
 
 _cached = None
@@ -26,7 +28,7 @@ def load():
     if _cached is not None:
         return _cached
     if not available():
-        raise RuntimeError("reference tree not present at %s" % REFERENCE_ROOT)
+        raise RuntimeError("set LUNGMASK_REFERENCE_ROOT to the absolute path of a reference checkout (now %r)" % REFERENCE_ROOT)
     standins.install()
     # The reference imports itself as `lungmask`; this repo ships a same-named drop-in shim, so
     # park whatever is registered under that name while the reference is being imported.

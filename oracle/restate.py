@@ -1,6 +1,6 @@
 """CPU restatement of the lungmask hot path.  TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
-Every function cites the reference lines (relative to /root/reference/) it follows.  Integer /
+Every function cites the reference lines (relative to the reference root) it follows.  Integer /
 boolean stages use numpy + scipy.ndimage exactly where the reference does (so that timing this
 port on host cores is a fair stand-in for the reference's own force_cpu path); the U-Net forward is
 a plain fp32 torch-functional evaluation straight from the state_dict (no nn.Module).

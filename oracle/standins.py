@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
-The reference (`/root/reference/lungmask/utils.py:5-11`, `mask.py:6-11`) imports
+The reference (`lungmask/utils.py:5-11`, `mask.py:6-11`) imports
 `skimage.measure`, `skimage.morphology`, `fill_voids`, `more_itertools`, `SimpleITK`, `pydicom`
 (un-pinned in `requirements.txt:1-9`).  None of them is installed here and there is no network, so
 the behaviour used on the hot path is restated below from the packages' documented semantics on

@@ -140,7 +140,22 @@ def random_state_dict(K: int, seed: int, calibrate_on: np.ndarray = None, head_g
     return sd
 
 
-def _forward_train(x, sd, momentum):
+def _upsample2x(x):
+    """nn.Upsample(scale_factor=2, mode="bilinear", align_corners=False) from slices and weighted sums, whose backward
+    is deterministic on CUDA (F.interpolate's backward accumulates with atomics): output 2i = x[i] * 0.75 + x[i-1] * 0.25,
+    output 2i+1 = x[i] * 0.75 + x[i+1] * 0.25, neighbours clamped at the border; along W, then along H."""
+    def along(x, d):
+        n = x.shape[d]
+        prev = torch.cat([x.narrow(d, 0, 1), x.narrow(d, 0, n - 1)], d)
+        nxt = torch.cat([x.narrow(d, 1, n - 1), x.narrow(d, n - 1, 1)], d)
+        even, odd = x * 0.75 + prev * 0.25, x * 0.75 + nxt * 0.25
+        shape = list(x.shape)
+        shape[d] *= 2
+        return torch.stack([even, odd], d + 1).reshape(shape)
+    return along(along(x, 3), 2)
+
+
+def _forward_train(x, sd, momentum, upsample=None):
     """Same graph as restate.unet_forward but with BN in training mode (updates running stats)."""
     def block(x, p):
         for conv, bn in ((0, 2), (3, 5)):
@@ -156,7 +171,7 @@ def _forward_train(x, sd, momentum):
             skips.append(x)
             x = F.avg_pool2d(x, 2)
     for j in range(4):
-        up = F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=False)
+        up = upsample(x) if upsample else F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=False)
         up = F.conv2d(up, sd[f"up_path.{j}.up.1.weight"], sd[f"up_path.{j}.up.1.bias"])
         x = block(torch.cat([up, skips[-j - 1]], 1), f"up_path.{j}.conv_block.block")
     return F.log_softmax(F.conv2d(x, sd["last.weight"], sd["last.bias"]), dim=1)
@@ -189,14 +204,24 @@ def train_state_dict(K: int, seed: int, steps: int = 60, device: str = None, n_s
     for k in params:
         sd[k].requires_grad_(True)
     opt = torch.optim.Adam([sd[k] for k in params], lr=lr)
-    for step in range(steps):
-        idx = torch.randint(0, n_slices, (batch,), generator=g).to(device)
-        loss = F.nll_loss(_forward_train(x_all[idx], sd, momentum=0.1), y_all[idx])
-        opt.zero_grad(set_to_none=True)
-        loss.backward()
-        opt.step()
-        if log is not None and (step % 10 == 0 or step == steps - 1):
-            log(f"train K={K} step {step} loss {loss.item():.4f}")
+    # The same seed gives the same weights on every run: deterministic algorithms only (cuDNN included), the upsample
+    # and the loss written with ops whose CUDA backward / forward does not accumulate with atomics.
+    saved = (torch.are_deterministic_algorithms_enabled(), torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark)
+    torch.use_deterministic_algorithms(True)
+    torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = True, False
+    try:
+        for step in range(steps):
+            idx = torch.randint(0, n_slices, (batch,), generator=g).to(device)
+            logp = _forward_train(x_all[idx], sd, momentum=0.1, upsample=_upsample2x)
+            loss = -logp.gather(1, y_all[idx].long()[:, None]).mean()   # = F.nll_loss(logp, y)
+            opt.zero_grad(set_to_none=True)
+            loss.backward()
+            opt.step()
+            if log is not None and (step % 10 == 0 or step == steps - 1):
+                log(f"train K={K} step {step} loss {loss.item():.4f}")
+    finally:
+        torch.use_deterministic_algorithms(saved[0])
+        torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = saved[1], saved[2]
     for k in params:
         sd[k].requires_grad_(False)
     with torch.no_grad():  # re-calibrate BN on a fixed batch, in eval-compatible form

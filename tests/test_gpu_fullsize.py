@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def big_engine():
     from lungmask_b200 import _native
-    eng = _native.Engine(device=0, batch_capacity=37)
+    eng = _native.Engine(device=0, batch_capacity=33)
     yield eng
     eng.close()
 
@@ -75,7 +75,7 @@ def test_c4_fusion_300_slices(big_engine):
 
 
 def test_c2_r231_300_slices_through_lminferer(tmp_path):
-    """C2 through the public surface: default LMInferer on a 300-slice volume == the capacity-37 engine."""
+    """C2 through the public surface: default LMInferer on a 300-slice volume == the capacity-33 engine."""
     import torch
     from lungmask_b200 import LMInferer
     sd = synth.random_state_dict(3, seed=33, head_gain=0.3)

@@ -1,5 +1,5 @@
 """The CPU oracle (oracle/restate.py) against fixtures generated from the UNMODIFIED reference by
-oracle/make_golden.py (tests/golden/).  Runs anywhere (no GPU, no /root/reference)."""
+oracle/make_golden.py (tests/golden/).  Runs anywhere (no GPU, no reference checkout)."""
 import json
 import os
 import zlib
