@@ -170,6 +170,8 @@ LM_API int lm_last_timings(const lm_engine* e, float* ms7, int64_t* kernel_launc
  * "chunk_kb_wide" (the same for the layers with >= 128 output channels only; defaults: 1 for the 64-channel
  * layers, 2 for the wide ones), "weight_mcast" (0 / 2: clusters of two CTAs share every weight stage through TMA
  * multicast; bit-identical, default 0),
+ * "conv64_cm" (1, default: the three 3x3 layers with 64 output channels at full resolution run as channel-major
+ * 16x16-pixel tiles, conv_cm64_kernel; 0: the BN = 64 kernel; bit-identical; environment LM_CONV64_CM at lm_create),
  * "stem_v2" (0 = first stem kernel, 1 = register-resident, 2 = shared-memory tile, 3 = the same with the next tile's
  * samples fetched one tile ahead, the default; all bit-identical),
  * "graphs" (1, default: a volume's forward - every wave's ~26 launches - is captured once as a CUDA graph and replayed;

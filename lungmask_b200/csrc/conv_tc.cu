@@ -28,6 +28,8 @@
 //   * persistent CTAs (one per SM), warp-specialised: warp 0 is the TMA producer, warpgroups 1 and 2 are consumers
 //     that each own 64 rows of the tile (image rows 0-7 / 8-15 of the patch): they issue the wgmmas, drain the
 //     chunks and run the epilogue of their rows straight from the accumulator registers.
+//   * the 3x3 layers with 64 output channels run conv_cm64_kernel (below) unless ConvParams::conv64_cm is 0: the same
+//     scheme with the GEMM roles swapped (M = output channels, N = pixels), bit-identical results.
 #include <atomic>
 #include <stdio.h>
 #include "conv_tc.cuh"
@@ -407,6 +409,301 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   if (MC > 1) cluster_sync_all();
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Channel-major tile for the 3x3 layers with 64 output channels (conv_cm64_fits), fp16-pair operands only.  The GEMM
+// roles of conv_tc_kernel swapped:
+//   * A operand = the weight stage, M = the 64 output channels (the BN = 64 kernel's weight box and descriptor).
+//   * B operand = activations, N = 128 pixels per warpgroup.  A CTA takes 16 x 16 pixels of one image, warpgroup h the
+//     columns 8h..8h+7 of all 16 rows, so that every 8-row group of the descriptor is one image row.  ONE 5-D TMA box per
+//     64-channel block, (64 ch, 18 x, 18 y, 2 planes, 1 image) = 324 rows of 128 B per plane, serves all nine taps: tap
+//     (dy, dx) of warpgroup h starts at row dy * 18 + dx + 8h with an 8-row-group stride of 18 rows.
+//   * every wgmma is m64n128k16 (the BN = 64 kernel issues m64n64k16 with the same 4 KB of operands per instruction:
+//     0.047 instead of 0.0625 B of shared-memory operand reads per MAC); per output pixel half the weight bytes and 1.27
+//     instead of 1.41 input rows.
+//   * the same three exact products per k-step, accumulated in the same order (hi*hi into P; act_hi*w_lo, then act_lo*w_hi
+//     into Q), the same chunks and the same epilogue operations per element: the results equal the BN = 64 kernel's.
+// Thread (warp w, g = lane / 4, qd = lane % 4) of warpgroup h holds in register 4j + e output channel 16w + g + 8 (e / 2)
+// of pixel (row j, column 8h + 2qd + e % 2) of the tile.
+constexpr int CM_TILE = 16, CM_HALO = CM_TILE + 2;
+constexpr int CM_A_PLANE = CM_HALO * CM_HALO * ROW_BYTES;  // 324 rows x 128 B = 41472 B per plane
+constexpr int CM_A_BUF = 2 * CM_A_PLANE;                   // 82944 B (both planes), 1024-aligned
+constexpr int CM_STAGES = 3;
+constexpr int CM_STAGE_BYTES = Cfg<64>::STAGE_BYTES;       // 16 KB: 64 cout x 64 cin, hi + lo planes
+constexpr int CM_NUM_BARS = 2 * CM_STAGES + 2 * NUM_A_BUFS;
+constexpr int CM_OFF_B = NUM_A_BUFS * CM_A_BUF;
+constexpr int CM_OFF_BARS = CM_OFF_B + CM_STAGES * CM_STAGE_BYTES;
+constexpr int CM_OFF_HEAD = CM_OFF_BARS + CM_NUM_BARS * 8;
+constexpr int CM_DYN_SMEM = CM_OFF_HEAD + (MAX_CLASSES * 64 + MAX_CLASSES) * 4;   // 217200 B
+static_assert(CM_DYN_SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
+constexpr int CM_Y_STRIDE = 65;   // head: the tile's fp32 y staged [pixel][channel], padded against bank conflicts
+static_assert(CM_TILE * CM_TILE * CM_Y_STRIDE * 4 <= CM_A_BUF, "the head's staging fits one activation buffer");
+
+#if LM_OPERAND_F16
+struct CmTile {
+  int n, y0, x0;
+};
+__device__ __forceinline__ CmTile cm_tile(int tile, int tiles_x, int tiles_img) {
+  CmTile t;
+  t.n = tile / tiles_img;
+  const int r = tile - t.n * tiles_img;
+  const int ty = r / tiles_x;
+  t.y0 = ty * CM_TILE;
+  t.x0 = (r - ty * tiles_x) * CM_TILE;
+  return t;
+}
+
+__device__ __forceinline__ void cm64_consumer(const ConvParams& p, uint8_t* smem, uint32_t smem_a, uint32_t smem_b,
+                                              uint32_t full0, uint32_t empty0, uint32_t afull0, uint32_t aempty0,
+                                              const float* s_head_w, const float* s_head_b) {
+  constexpr uint32_t SBO_X = CM_HALO * ROW_BYTES;
+  const int tid = threadIdx.x - 128;
+  const int half = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
+  const int g = lane >> 2, qd = lane & 3;
+  const int tiles_x = p.W / CM_TILE, tiles_img = tiles_x * (p.H / CM_TILE);
+  const int total_tiles = p.N * tiles_img;
+  const int num_kb = (p.C0 + p.C1) / BK * 9, chunk_kb = p.chunk_kb;
+  const bool head = p.mode == kModeHead;
+  const uint32_t x_half = (uint32_t)(8 * half * ROW_BYTES);
+
+  float S[64], P[64], Q[64];   // round-to-nearest sum of hi*hi | open chunk of hi*hi | corrections (x 2^11)
+  uint32_t s = 0, ph = 0, ab = 0, aph = 0;
+  auto release = [&](uint32_t st, int a) {   // a weight stage (and an activation buffer, a >= 0) may be refilled
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(empty0 + 8 * st);
+      if (a >= 0) mbar_arrive(aempty0 + 8 * a);
+    }
+  };
+
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const CmTile t = cm_tile(tile, tiles_x, tiles_img);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { S[i] = 0.f; Q[i] = 0.f; }
+    // the k loop of conv_consumer (chunks, wait discipline, releases); the head keeps the tile's last activation buffer
+    // until its epilogue has staged y through it
+    for (int kb0 = 0; kb0 < num_kb; kb0 += chunk_kb) {
+      const int kb1 = min(kb0 + chunk_kb, num_kb);
+      uint32_t pend_s = 0;
+      int pend_a = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const int tap = kb % 9;
+        if (tap == 0) mbar_spin(afull0 + 8 * ab, aph);
+        const uint32_t x_tap = smem_a + ab * (uint32_t)CM_A_BUF + x_half + (uint32_t)(((tap / 3) * CM_HALO + (tap % 3)) * ROW_BYTES);
+        const uint32_t w_st = smem_b + s * (uint32_t)CM_STAGE_BYTES;
+        mbar_spin(full0 + 8 * s, ph);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < ROW_BYTES / 32; ++k) {
+          const uint64_t wh = make_desc_sw128(w_st + 32 * k, 1024), wl = make_desc_sw128(w_st + Cfg<64>::B_PLANE_BYTES + 32 * k, 1024);
+          const uint64_t xh = make_desc_sw128(x_tap + 32 * k, SBO_X), xl = make_desc_sw128(x_tap + CM_A_PLANE + 32 * k, SBO_X);
+          wgmma_n128(P, wh, xh, k != 0 || kb != kb0);   // hi*hi (a chunk's first k-step restarts it from zero)
+          wgmma_n128(Q, wl, xh, 1);                      // act hi * w lo
+          wgmma_n128(Q, wh, xl, 1);                      // act lo * w hi
+        }
+        wgmma_commit();
+        if (kb > kb0) {
+          wgmma_wait<1>();
+          release(pend_s, pend_a);
+        }
+        pend_s = s;
+        pend_a = (tap == 8 && !(head && kb == num_kb - 1)) ? (int)ab : -1;
+        if (++s == CM_STAGES) { s = 0; ph ^= 1u; }
+        if (tap == 8 && ++ab == NUM_A_BUFS) { ab = 0; aph ^= 1u; }
+      }
+      wgmma_wait<0>();
+      release(pend_s, pend_a);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) S[i] += P[i];
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) S[i] += Q[i] * kLoUnscale;
+
+    // ---- epilogue: conv_consumer's operations per element, for the two channels c0 (e = 0, 1) and c0 + 8 (e = 2, 3)
+    const float unscale = p.in_unscale;
+    const float cscale = head ? 1.f : p.out_scale;
+    const int c0 = 16 * wq + g;
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int c = c0 + 8 * u;
+      const float b = p.bias ? __ldg(p.bias + c) : 0.f;
+      const float sc = (p.scale ? __ldg(p.scale + c) : 0.f) * cscale, sh = (p.shift ? __ldg(p.shift + c) : 0.f) * cscale;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = S[4 * j + 2 * u + e];
+          v = __fadd_rn(__fmul_rn(fmaxf(__fmaf_rn(v, unscale, b), 0.f), sc), sh);
+        }
+    }
+    if (head) {
+      // 1x1 head, log-softmax, argmax: one pixel per thread, from y staged in the tile's last activation buffer (the
+      // wgmmas of both warpgroups have read it once both pass the first barrier).  The four partial sums over channels
+      // 8j + 2q + e and their pairwise additions are those of conv_consumer's quad reduction.
+      const int y_buf = (int)(ab ^ 1u);   // the buffer of the tile's last channel block
+      float* ys = reinterpret_cast<float*>(smem + y_buf * CM_A_BUF);
+      named_bar_sync(1, 256);
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          ys[(16 * j + 8 * half + 2 * qd + (e & 1)) * CM_Y_STRIDE + c0 + 8 * (e >> 1)] = S[4 * j + e];
+      named_bar_sync(1, 256);
+      const float* yp = ys + tid * CM_Y_STRIDE;
+      float lg[MAX_CLASSES];
+#pragma unroll
+      for (int k = 0; k < MAX_CLASSES; ++k) {
+        float d[4] = {0.f, 0.f, 0.f, 0.f};
+        if (k < p.K) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) d[q] = fmaf(s_head_w[k * 64 + 8 * j + 2 * q + e], yp[8 * j + 2 * q + e], d[q]);
+        }
+        lg[k] = (k < p.K) ? ((d[0] + d[1]) + (d[2] + d[3])) + s_head_b[k] : -INFINITY;
+      }
+      fence_proxy_async_smem();   // the producer's next TMA load into this buffer comes after these accesses
+      __syncwarp();
+      if (lane == 0) mbar_arrive(aempty0 + 8 * y_buf);
+      const int y = t.y0 + (tid >> 4), x = t.x0 + (tid & 15);
+      float mx = -INFINITY;
+#pragma unroll
+      for (int k = 0; k < MAX_CLASSES; ++k) mx = fmaxf(mx, lg[k]);
+      float se = 0.f;
+#pragma unroll
+      for (int k = 0; k < MAX_CLASSES; ++k) if (k < p.K) se += expf(lg[k] - mx);
+      const float lse = logf(se);
+      int best = 0;
+      float bestv = -INFINITY;
+#pragma unroll
+      for (int k = 0; k < MAX_CLASSES; ++k) {
+        if (k < p.K) {
+          const float sc = (lg[k] - mx) - lse;  // LogSoftmax(dim=1), resunet.py:70
+          if (sc > bestv) { bestv = sc; best = k; }  // first index wins ties (mask.py:185)
+          if (p.scores) p.scores[(((size_t)t.n * p.K + k) * p.H + y) * p.W + x] = sc;
+        }
+      }
+      p.labels[((size_t)t.n * p.H + y) * p.W + x] = (uint8_t)best;
+      continue;
+    }
+    {  // fp16 saturates: report instead of storing inf (the engine lowers out_scale and runs again)
+      bool ovf = false;
+#pragma unroll
+      for (int i = 0; i < 64; ++i) ovf |= !(fabsf(S[i]) <= kOpMax);
+      if (__any_sync(0xffffffffu, ovf) && lane == 0 && p.range_flag) *p.range_flag = 1;
+    }
+    // Split planes.  Per image row j and channel octet u the warp holds an 8 x 8 matrix (channel g, pixel column 2qd + e)
+    // in the movmatrix fragment layout; its transpose gives lane (g, qd) channels 16w + 8u + 2qd, +1 of column 8h + g,
+    // stored as one hi and one lo pair like conv_consumer's.
+    {
+      const size_t plane = (size_t)p.H * p.W * 64;
+      op_t* dst = static_cast<op_t*>(p.out) + (size_t)t.n * 2 * plane + ((size_t)t.y0 * p.W + t.x0 + 8 * half + g) * 64 + 16 * wq + 2 * qd;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          uint32_t hi, lo;
+          split_f16x2(S[4 * j + 2 * u], S[4 * j + 2 * u + 1], hi, lo);
+          op_t* d = dst + (size_t)j * p.W * 64 + 8 * u;
+          *reinterpret_cast<uint32_t*>(d) = movmatrix_trans(hi);
+          *reinterpret_cast<uint32_t*>(d + plane) = movmatrix_trans(lo);
+        }
+    }
+    if (p.mode == kModeReluBnPool) {
+      // 2x2 average, ((top-left + top-right) + (bottom-left + bottom-right)) * 0.25, inside the thread: pooled pixel (row i,
+      // column 4h + qd).  Pooled rows 2m and 2m + 1 pack into one matrix (channel g, column 2qd + r); after the transpose
+      // lane (g, qd) holds channels 16w + 8u + 2qd, +1 of pooled pixel (row 2m + g % 2, column 4h + g / 2).
+      const int Wp = p.W / 2;
+      const size_t plane = (size_t)(p.H / 2) * Wp * 64;
+      op_t* dst = static_cast<op_t*>(p.out_pool) + (size_t)t.n * 2 * plane +
+                  ((size_t)(t.y0 / 2 + (g & 1)) * Wp + t.x0 / 2 + 4 * half + (g >> 1)) * 64 + 16 * wq + 2 * qd;
+#pragma unroll
+      for (int m = 0; m < 4; ++m)
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          float pv[2];
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int jt = 2 * (2 * m + r);
+            const float top = S[4 * jt + 2 * u] + S[4 * jt + 2 * u + 1];
+            const float bot = S[4 * (jt + 1) + 2 * u] + S[4 * (jt + 1) + 2 * u + 1];
+            pv[r] = (top + bot) * 0.25f;
+          }
+          uint32_t hi, lo;
+          split_f16x2(pv[0], pv[1], hi, lo);
+          op_t* d = dst + (size_t)(2 * m) * Wp * 64 + 8 * u;
+          *reinterpret_cast<uint32_t*>(d) = movmatrix_trans(hi);
+          *reinterpret_cast<uint32_t*>(d + plane) = movmatrix_trans(lo);
+        }
+    }
+  }
+}
+
+// conv_tc_kernel's warp roles and mbarrier protocol (MC = 1) with the channel-major consumer; 3 weight stages.
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+conv_cm64_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
+                 const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];   // activation buffers | weight ring | mbarriers | head
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CM_OFF_BARS);
+  float* s_head_w = reinterpret_cast<float*>(smem + CM_OFF_HEAD);
+  float* s_head_b = s_head_w + MAX_CLASSES * 64;
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = full0 + 8 * CM_STAGES;
+  const uint32_t afull0 = full0 + 16 * CM_STAGES, aempty0 = afull0 + 8 * NUM_A_BUFS;
+  const uint32_t smem_a = smem_u32(smem), smem_b = smem_a + CM_OFF_B;
+  const int warp = threadIdx.x >> 5;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < CM_STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, NUM_CONSUMER_WARPS); }
+    for (int s = 0; s < NUM_A_BUFS; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, NUM_CONSUMER_WARPS); }
+    fence_mbar_init();
+    tma_prefetch_desc(&tmA0); tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmB);
+  }
+  if (p.mode == kModeHead) {
+    for (int i = threadIdx.x; i < p.K * 64; i += NUM_THREADS) s_head_w[i] = p.head_w[i];
+    if (threadIdx.x < p.K) s_head_b[threadIdx.x] = p.head_b[threadIdx.x];
+  }
+  __syncthreads();
+
+  if (warp >= 4) {
+    setmaxnreg_inc<REGS_CONSUMER>();
+    cm64_consumer(p, smem, smem_a, smem_b, full0, empty0, afull0, aempty0, s_head_w, s_head_b);
+  } else {
+    setmaxnreg_dec<REGS_PRODUCER>();
+    if (warp == 0) {
+      // -------------------------------------------------------------- TMA producer (warp 0, one elected lane issues)
+      const int tiles_x = p.W / CM_TILE, tiles_img = tiles_x * (p.H / CM_TILE);
+      const int num_cb = (p.C0 + p.C1) / BK;
+      uint32_t s = 0, ph = 0, ab = 0, aph = 0;
+      for (int tile = blockIdx.x; tile < p.N * tiles_img; tile += gridDim.x) {
+        const CmTile t = cm_tile(tile, tiles_x, tiles_img);
+        int c = 0;
+        for (int cb = 0; cb < num_cb; ++cb, c += BK) {
+          mbar_wait_inline(aempty0 + 8 * ab, aph ^ 1);
+          if (elect_one()) {
+            mbar_arrive_expect_tx(afull0 + 8 * ab, (uint32_t)CM_A_BUF);
+            const uint32_t dst = smem_a + ab * CM_A_BUF;
+            if (c < p.C0) tma_load_5d(dst, &tmA0, afull0 + 8 * ab, c, t.x0 - 1, t.y0 - 1, 0, t.n);
+            else          tma_load_5d(dst, &tmA1, afull0 + 8 * ab, c - p.C0, t.x0 - 1, t.y0 - 1, 0, t.n);
+          }
+          __syncwarp();
+          if (++ab == NUM_A_BUFS) { ab = 0; aph ^= 1; }
+          for (int tap = 0; tap < 9; ++tap) {
+            mbar_wait_inline(empty0 + 8 * s, ph ^ 1);
+            if (elect_one()) {
+              mbar_arrive_expect_tx(full0 + 8 * s, CM_STAGE_BYTES);
+              tma_load_4d(smem_b + s * CM_STAGE_BYTES, &tmB, full0 + 8 * s, c, 0, tap, 0);
+            }
+            __syncwarp();
+            if (++s == CM_STAGES) { s = 0; ph ^= 1; }
+          }
+        }
+      }
+    }
+  }
+}
+#endif  // LM_OPERAND_F16
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                   CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
@@ -440,13 +737,13 @@ int encode(CUtensorMap* m, CUtensorMapDataType dtype, const void* base, int rank
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
-int make_act_map(CUtensorMap* m, const void* base, int n_cap, int H, int W, int Cch, int taps) {
+// activation boxes of box_w x box_h pixels (tile + halo), BK channels, both planes, one image
+int make_act_map(CUtensorMap* m, const void* base, int n_cap, int H, int W, int Cch, int box_w, int box_h) {
   const cuuint64_t E = kOpBytes;
   cuuint64_t dims[5] = {(cuuint64_t)Cch, (cuuint64_t)W, (cuuint64_t)H, 2, (cuuint64_t)n_cap};
   cuuint64_t strides[4] = {(cuuint64_t)Cch * E, (cuuint64_t)W * Cch * E, (cuuint64_t)H * W * Cch * E,
                            (cuuint64_t)2 * H * W * Cch * E};
-  const cuuint32_t halo = taps == 9 ? 2 : 0;
-  cuuint32_t box[5] = {BK, TILE_W + halo, TILE_H + halo, 2, 1};
+  cuuint32_t box[5] = {BK, (cuuint32_t)box_w, (cuuint32_t)box_h, 2, 1};
   return encode(m, kOpType, base, 5, dims, strides, box);
 }
 
@@ -458,11 +755,20 @@ int make_conv_maps(ConvMaps* maps, const void* src0, const void* src1, const voi
   if (p.H % TILE_H || p.W % TILE_W || p.C0 % BK || p.C1 % BK || (p.taps != 1 && p.taps != 9)) return -2;
   const int BN = conv_tile_n(p);
   if (p.Cout % BN) return -3;
-  int r = make_act_map(&maps->a0, src0, n_capacity, p.H, p.W, p.C0, p.taps);
+  const int halo = p.taps == 9 ? 2 : 0;
+  // src1 absent: a1 repeats a0 (never read)
+  const void* s1 = p.C1 > 0 ? src1 : src0;
+  const int c1 = p.C1 > 0 ? p.C1 : p.C0;
+  int r = make_act_map(&maps->a0, src0, n_capacity, p.H, p.W, p.C0, TILE_W + halo, TILE_H + halo);
   if (r) return r;
-  r = (p.C1 > 0) ? make_act_map(&maps->a1, src1, n_capacity, p.H, p.W, p.C1, p.taps)
-                 : make_act_map(&maps->a1, src0, n_capacity, p.H, p.W, p.C0, p.taps);
+  r = make_act_map(&maps->a1, s1, n_capacity, p.H, p.W, c1, TILE_W + halo, TILE_H + halo);
   if (r) return r;
+  if (conv_cm64_fits(p)) {
+    r = make_act_map(&maps->a0cm, src0, n_capacity, p.H, p.W, p.C0, CM_HALO, CM_HALO);
+    if (r) return r;
+    r = make_act_map(&maps->a1cm, s1, n_capacity, p.H, p.W, c1, CM_HALO, CM_HALO);
+    if (r) return r;
+  }
   const int Cin = p.C0 + p.C1;
   cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)p.Cout, (cuuint64_t)p.taps, 2};
   cuuint64_t strides[3] = {(cuuint64_t)Cin * E, (cuuint64_t)p.Cout * Cin * E, (cuuint64_t)p.taps * p.Cout * Cin * E};
@@ -506,12 +812,22 @@ int conv_tc_prepare() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::DYN_SMEM);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<128>::DYN_SMEM);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_tc_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<64>::DYN_SMEM);
+#if LM_OPERAND_F16
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_cm64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CM_DYN_SMEM);
+#endif
   return (int)e;
 }
 
 int launch_conv_tc(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaStream_t stream) {
   if (p.mode == kModeHead && (p.Cout != 64 || p.K > MAX_CLASSES)) return -4;
   if (p.chunk_kb < 1) return -5;
+#if LM_OPERAND_F16
+  if (p.conv64_cm && conv_cm64_fits(p)) {   // conv_tc_prepare has set the kernel's shared-memory opt-in
+    const int total = p.N * (p.H / CM_TILE) * (p.W / CM_TILE);
+    conv_cm64_kernel<<<total < num_sms ? total : num_sms, NUM_THREADS, CM_DYN_SMEM, stream>>>(maps.a0cm, maps.a1cm, maps.b, p);
+    return (int)cudaGetLastError();
+  }
+#endif
   if (p.weight_mcast == 2)
     return conv_tile_n(p) == 128 ? launch_impl<128, 2>(maps, p, num_sms, stream) : launch_impl<64, 2>(maps, p, num_sms, stream);
   return conv_tile_n(p) == 128 ? launch_impl<128, 1>(maps, p, num_sms, stream) : launch_impl<64, 1>(maps, p, num_sms, stream);

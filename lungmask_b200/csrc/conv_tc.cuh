@@ -56,6 +56,8 @@ struct ConvParams {
   int weight_mcast;   // 2: clusters of two CTAs share every weight stage through TMA multicast (conv_tc.cu, MC = 2); 0: off
   int tile_n;         // output-channel tile: 0 = conv_tile_n(Cout); 64 forces the BN = 64 kernel for a layer with
                       // Cout >= 128 - must be set before make_conv_maps
+  int conv64_cm;      // 1: layers that conv_cm64_fits runs as channel-major 16x16-pixel tiles (conv_tc.cu,
+                      // conv_cm64_kernel); 0: the BN = 64 kernel (same results bit for bit)
   const float* bias;  // [Cout]
   const float* scale; // [Cout]  folded BN:  y = relu(.) * scale + shift
   const float* shift; // [Cout]
@@ -78,7 +80,14 @@ struct ConvParams {
 struct ConvMaps {
   CUtensorMap a0, a1, b;
   CUtensorMap bx;  // weights, one plane per box: the per-CTA half of a multicast weight stage (weight_mcast = 2)
+  CUtensorMap a0cm, a1cm;  // activations in 16x16-pixel boxes (+ halo) for conv_cm64_kernel; built when conv_cm64_fits
 };
+
+// Layers the channel-major kernel serves: 3x3, 64 output channels, 16x16 tiles, fp16-pair operands, a split-plane
+// (or head) epilogue.
+inline bool conv_cm64_fits(const ConvParams& p) {
+  return LM_OPERAND_F16 && p.Cout == 64 && p.taps == 9 && p.mode != kModeLinear && p.H % 16 == 0 && p.W % 16 == 0;
+}
 
 // Builds the TMA descriptors. src1 may be nullptr when C1 == 0. Returns 0 on success.
 int make_conv_maps(ConvMaps* maps, const void* src0, const void* src1, const void* weights,

@@ -207,6 +207,7 @@ struct lm_engine {
   int weight_mcast = 0;   // 2: clusters of two CTAs share each weight stage through TMA multicast (conv_tc.cu, MC = 2)
   int chunk_kb = 1;       // k-blocks per tensor-core chunk of hi*hi (conv_tc.cu) for the 64-channel layers
   int chunk_kb_wide = 2;  // ... for the layers with Cout >= 128
+  int conv64_cm = 1;      // 1: the 3x3 layers with 64 output channels run conv_cm64_kernel; 0: the BN = 64 kernel (bit-identical)
 };
 
 namespace {
@@ -265,6 +266,7 @@ int forward_batch(lm_engine* e, Slot& s, const void* d_in, bool in_f32, int n, u
     p.N = n;
     p.chunk_kb = (p.Cout >= 128) ? e->chunk_kb_wide : e->chunk_kb;
     p.weight_mcast = e->weight_mcast;
+    p.conv64_cm = e->conv64_cm;
     const LayerSpec& L = LAYERS[i];
     p.range_flag = L.dst >= 0 ? range + L.dst : nullptr;
     p.in_unscale = 1.f / (s.act_scale[L.src0] * s.lw[i].w_scale);   // src1 (virtual concat) shares src0's scale group
@@ -637,6 +639,7 @@ static int create_resources(lm_engine* e) {
   const int batch_capacity = e->B;
   if (const char* c = getenv("LM_CHUNK_KB")) { int v = atoi(c); if (v >= 1) e->chunk_kb = e->chunk_kb_wide = v; }
   if (const char* c = getenv("LM_WEIGHT_MCAST")) e->weight_mcast = atoi(c) == 2 ? 2 : 0;
+  if (const char* c = getenv("LM_CONV64_CM")) e->conv64_cm = atoi(c) != 0;
   if (const char* c = getenv("LM_GRAPHS")) e->use_graphs = atoi(c) != 0;
   if (const char* c = getenv("LM_BN64_MASK")) e->bn64_mask = (unsigned)strtoul(c, nullptr, 0);
   if (const char* c = getenv("LM_STEM_V2")) { const int v = atoi(c); e->stem_v2 = v < 0 ? 0 : (v > 3 ? 3 : v); }
@@ -1242,6 +1245,7 @@ int lm_set_option(lm_engine* e, const char* key, int value) {
   if (!strcmp(key, "post_debug_stage")) { e->post.debug_stage = value; return 0; }
   if (!strcmp(key, "chunk_kb")) { if (value < 1) return fail(-1, "chunk_kb must be >= 1"); e->chunk_kb = e->chunk_kb_wide = value; return 0; }
   if (!strcmp(key, "weight_mcast")) { if (value != 0 && value != 2) return fail(-1, "weight_mcast must be 0 or 2"); e->weight_mcast = value; return 0; }
+  if (!strcmp(key, "conv64_cm")) { if (value != 0 && value != 1) return fail(-1, "conv64_cm must be 0 or 1"); e->conv64_cm = value; return 0; }
   if (!strcmp(key, "stem_v2")) { if (value < 0 || value > 3) return fail(-1, "stem_v2 must be 0, 1, 2 or 3"); e->stem_v2 = value; return 0; }
   if (!strcmp(key, "upsample_v2")) { e->upsample_v2 = value < 0 ? 0 : (value > 2 ? 2 : value); return 0; }
   if (!strcmp(key, "ccl_rule")) { e->post.ccl_rule = value != 0; return 0; }

@@ -115,6 +115,21 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank)
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 
+// ---------------------------------------------------------------- warp / CTA
+// barrier `id` among the first `threads` threads that reach it (a multiple of 32; id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// generic-proxy shared-memory accesses before it are ordered before later async-proxy (TMA) writes to the same memory
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// 8x8 matrix of 16-bit elements held one row per lane quad (lane l: row l / 4, columns 2 (l % 4), +1 packed low / high)
+// -> its transpose in the same layout
+__device__ __forceinline__ uint32_t movmatrix_trans(uint32_t x) {
+  uint32_t y;
+  asm volatile("movmatrix.sync.aligned.m8n8.trans.b16 %0, %1;" : "=r"(y) : "r"(x));
+  return y;
+}
+
 // ---------------------------------------------------------------- wgmma
 // Register reallocation between warpgroups (setmaxnreg: all four warps of a warpgroup execute it together).
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
