@@ -103,6 +103,25 @@ LM_API int lm_preprocess_float(lm_engine* e, const void* vol, int is_f64, int S,
 LM_API int lm_apply_volume_oriented(lm_engine* e, int slot, int slot_fill, const int16_t* vol, int n0, int n1, int n2,
                                     const int* perm, const int* flip, int flags, uint8_t* out);
 
+/* The mask AND the per-class probabilities of one model, from one forward pass (the reference's `inferer.model(x)`
+ * gives the same log-softmax at network resolution).  `vol` (n0,n1,n2) of element type `dtype`: LM_DTYPE_I16 takes the
+ * int16 path of lm_apply_volume; LM_DTYPE_F32 / LM_DTYPE_F64 keep their dtype through pre-processing as
+ * lm_apply_volume_float does.  perm / flip as lm_apply_volume_oriented; both NULL: the array is already LPS.
+ *   out    (n0,n1,n2) uint8: bit-identical to lm_apply_volume / lm_apply_volume_float / lm_apply_volume_oriented with the
+ *          same flags (LM_FLAG_NO_POSTPROCESS honoured).
+ *   probs  (K,n0,n1,n2) float32 in the native orientation: p_k = expf(s_k), s_k the head's fp32 log-softmax score (the
+ *          value lm_forward returns) of the network pixel that the mask's own order-0 resampling (utils.reshape_mask,
+ *          utils.py:114-129) places at the voxel.  Voxels that resampling sets to 0 (outside the crop box, or scipy's
+ *          constant-mode last row / column) have p_0 = 1 and p_k = 0 for k > 0.  The probabilities are the network's
+ *          output BEFORE post-processing, whatever `flags` says; with LM_FLAG_NO_POSTPROCESS argmax_k p_k equals `out`.
+ * Device memory: the scores of the whole volume (S * K * 256 * 256 * 4 bytes, S = slices of the LPS volume) and the
+ * probabilities (K * n0 * n1 * n2 * 4 bytes) stay allocated in the engine for the next call.  No fusion (slot_fill). */
+#define LM_DTYPE_I16 0
+#define LM_DTYPE_F32 1
+#define LM_DTYPE_F64 2
+LM_API int lm_apply_volume_probs(lm_engine* e, int slot, const void* vol, int dtype, int n0, int n1, int n2,
+                                 const int* perm, const int* flip, int flags, uint8_t* out, float* probs);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -1,13 +1,14 @@
 """`lungmask INPUT OUTPUT` command line (flags as lungmask/__main__.py:26-76).
 
 Inputs are read by lungmask_b200/io.py (DICOM series directory, NIfTI, MetaImage, .npy - no SimpleITK needed); the
-mask is written with the input's geometry as .nii / .nii.gz / .mha / .npy.
+mask is written with the input's geometry as .nii / .nii.gz / .mha / .npy.  `--probabilities PATH` also writes the
+model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_with_probabilities).
 """
 import argparse
 import os
 import sys
 
-from .io import load_input_image, save_mask
+from .io import check_probabilities_path, load_input_image, save_mask, save_probabilities
 from .logger import logger
 from .mask import LMInferer
 
@@ -33,11 +34,18 @@ def build_parser():
     p.add_argument("--noprogress", action="store_true", help="If set, no tqdm progress bar will be shown")
     p.add_argument("--version", action="version", version=__version__)
     p.add_argument("--removemetadata", action="store_true", help="Do not keep study/patient metadata of the input")
+    p.add_argument("--probabilities", metavar="PATH", type=str, default=None,
+                   help="Also write the model's per-class probabilities (before post-processing) with the mask's geometry: "
+                        ".npy, or a 4-D .nii / .nii.gz with the classes as 4th dimension. Not for LTRCLobes_R231")
     return p
 
 
 def main(argv=None):
     args = build_parser().parse_args(argv)
+    if args.probabilities is not None:
+        if args.modelname == "LTRCLobes_R231":
+            sys.exit("--probabilities: the LTRCLobes_R231 fusion has no class probabilities; use LTRCLobes or R231")
+        check_probabilities_path(args.probabilities)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -48,11 +56,18 @@ def main(argv=None):
     else:
         inferer = LMInferer(modelname=args.modelname, modelpath=args.modelpath, force_cpu=args.cpu, batch_size=batchsize,
                             volume_postprocessing=not args.nopostprocess, tqdm_disable=args.noprogress)
-    result = inferer.apply(image)      # a Volume: orientation handled as for a SimpleITK image (mask.py:157-164, 189-197)
+    probs = None
+    if args.probabilities is None:
+        result = inferer.apply(image)  # a Volume: orientation handled as for a SimpleITK image (mask.py:157-164, 189-197)
+    else:
+        result, probs = inferer.apply_with_probabilities(image)
     logger.info(f"Save result to: {args.output}")
     if not args.removemetadata and image.meta.get("SeriesInstanceUID"):
         logger.info("DICOM tags are never copied into the output by this build (as with --removemetadata)")
     save_mask(args.output, result, image)
+    if probs is not None:
+        logger.info(f"Save probabilities to: {args.probabilities}")
+        save_probabilities(args.probabilities, probs, image)
 
 
 if __name__ == "__main__":

@@ -9,6 +9,7 @@ LIB_PATH = os.path.join(_HERE, "liblungmask_b200.so")
 
 NET_RES = 256
 FLAG_NO_POSTPROCESS = 1
+DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2   # LM_DTYPE_* of lm_apply_volume_probs
 
 _lib = None
 
@@ -43,6 +44,7 @@ def lib():
         "lm_apply_volume_float": ([vp, i32, i32, vp, i32, i32, i32, i32, i32, u8p], i32),
         "lm_preprocess_float": ([vp, vp, i32, i32, i32, i32, f32p, i32p], i32),
         "lm_apply_volume_oriented": ([vp, i32, i32, i16p, i32, i32, i32, vp, vp, i32, u8p], i32),
+        "lm_apply_volume_probs": ([vp, i32, vp, i32, i32, i32, i32, vp, vp, i32, u8p, f32p], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -72,7 +74,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -200,6 +202,35 @@ class Engine:
         _check(lib().lm_apply_volume_oriented(self._h, slot, int(slot_fill), _ptr(vol), n0, n1, n2, pa, fa,
                                               0 if postprocess else FLAG_NO_POSTPROCESS, _ptr(out)))
         return out
+
+    def apply_volume_probs(self, slot, vol, perm=None, flip=None, postprocess=True):
+        """-> (mask, probs) of one model from one forward pass (lm_apply_volume_probs).  `vol`: int16 (other integer
+        widths must fit int16), float32 or float64, in its native orientation; (perm, flip) =
+        lungmask_b200.orient.array_transform_to_lps(code), or both None for an LPS array.  `mask` (uint8, vol.shape) is
+        what apply_volume / apply_volume_float / apply_volume_oriented return with the same `postprocess`.  `probs`
+        (float32, (K,) + vol.shape) are the network's class probabilities BEFORE post-processing, resampled to the
+        input like the mask (order 0, p_0 = 1 outside the crop box)."""
+        vol = np.asarray(vol)
+        if vol.dtype == np.float32 or vol.dtype == np.float64:
+            dtype = DTYPE_F32 if vol.dtype == np.float32 else DTYPE_F64
+            vol = _as(vol, vol.dtype, 3)
+        else:
+            dtype = DTYPE_I16
+            vol = _as(vol, np.int16, 3)
+        if (perm is None) != (flip is None):
+            raise ValueError("apply_volume_probs: give both perm and flip, or neither")
+        if slot not in self.n_classes:
+            raise NativeError("apply_volume_probs: weight slot %d not loaded" % slot)
+        out = np.empty(vol.shape, np.uint8)
+        probs = np.empty((self.n_classes[slot],) + vol.shape, np.float32)
+        pa = fa = None
+        if perm is not None:
+            pa = (C.c_int * 3)(*[int(x) for x in perm])
+            fa = (C.c_int * 3)(*[1 if x else 0 for x in flip])
+        n0, n1, n2 = vol.shape
+        _check(lib().lm_apply_volume_probs(self._h, slot, _ptr(vol), dtype, n0, n1, n2, pa, fa,
+                                           0 if postprocess else FLAG_NO_POSTPROCESS, _ptr(out), _ptr(probs)))
+        return out, probs
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

@@ -178,8 +178,10 @@ struct lm_engine {
   DevBuf<uint8_t> d_lps_out, d_native_l, d_native_r;
   DevBuf<int32_t> d_boxes;
   DevBuf<uint8_t> d_labels, d_post, d_out, d_out2, d_fused, d_mask;
-  DevBuf<float> d_scores, d_norm;
+  DevBuf<float> d_scores, d_norm;   // d_scores: one wave of lm_forward's tap, or a whole volume of lm_apply_volume_probs
+  DevBuf<float> d_probs;            // lm_apply_volume_probs: (K, n0, n1, n2) probabilities
   DevBuf<uint8_t> d_fvol;   // float volumes (float32 / float64), raw bytes
+  DevBuf<uint8_t> d_fnative;  // lm_apply_volume_probs: a float volume in its native orientation, raw bytes
   DevBuf<uint32_t> d_scratch;
   PostScratch post;
   cudaEvent_t ev[8] = {};
@@ -192,8 +194,9 @@ struct lm_engine {
   float last_ms[7] = {};
   int64_t launches = 0;
   // CUDA graphs of whole forwards (all waves of one volume: ~26 launches per wave), keyed by slot / buffers / slice count /
-  // input type and valid for one configuration epoch (weights, options and activation scales bump it)
-  struct FwdGraph { int slot; const void* in; uint8_t* labels; int S; bool f32; uint64_t epoch; cudaGraphExec_t exec; int64_t launches; };
+  // input type and valid for one configuration epoch (weights, options and activation scales bump it).  scores: the
+  // volume-sized score buffer the head writes (lm_apply_volume_probs), nullptr for score-less forwards.
+  struct FwdGraph { int slot; const void* in; uint8_t* labels; float* scores; int S; bool f32; uint64_t epoch; cudaGraphExec_t exec; int64_t launches; };
   std::vector<FwdGraph> graphs;
   uint64_t graph_epoch = 1;
   int use_graphs = 1;     // 0: launch every kernel individually (also whenever per-launch conv timing or score taps are on)
@@ -315,10 +318,12 @@ void drop_graphs(lm_engine* e) {
 // Replays (or first captures) the kernel sequence of one volume's forward - every wave's stem, 21 tensor-core
 // convolutions and 4 upsamples - as ONE graph launch on the engine stream.  Returns 0 when the graph was launched,
 // 1 when graphs cannot be used (the caller launches the kernels one by one), < 0 on a real error.
-int forward_graph(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labels, bool in_f32) {
+// d_vol_scores: nullptr, or the (S, K, 256, 256) buffer the head writes every slice's log-softmax scores to.
+int forward_graph(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labels, bool in_f32, float* d_vol_scores) {
   Slot& s = e->slots[slot];
   for (auto& g : e->graphs) {
-    if (g.slot == slot && g.in == d_in && g.labels == d_labels && g.S == S && g.f32 == in_f32 && g.epoch == e->graph_epoch) {
+    if (g.slot == slot && g.in == d_in && g.labels == d_labels && g.scores == d_vol_scores && g.S == S && g.f32 == in_f32 &&
+        g.epoch == e->graph_epoch) {
       CU(cudaGraphLaunch(g.exec, e->st));
       e->launches += g.launches;
       e->graph_hits++;
@@ -333,7 +338,8 @@ int forward_graph(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_la
     const int n = S - s0 < e->B ? S - s0 : e->B;
     const void* in_wave = in_f32 ? static_cast<const void*>(static_cast<const float*>(d_in) + (size_t)s0 * R * R)
                                  : static_cast<const void*>(static_cast<const int16_t*>(d_in) + (size_t)s0 * R * R);
-    rc = forward_batch(e, s, in_wave, in_f32, n, d_labels + (size_t)s0 * R * R, nullptr, false);
+    rc = forward_batch(e, s, in_wave, in_f32, n, d_labels + (size_t)s0 * R * R,
+                       d_vol_scores ? d_vol_scores + (size_t)s0 * s.K * R * R : nullptr, false);
   }
   cudaGraph_t graph = nullptr;
   const cudaError_t ce = cudaStreamEndCapture(e->st, &graph);
@@ -349,15 +355,17 @@ int forward_graph(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_la
   const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
   cudaGraphDestroy(graph);
   if (ie != cudaSuccess || !exec) { cudaGetLastError(); e->use_graphs = 0; return 1; }
-  e->graphs.push_back({slot, d_in, d_labels, S, in_f32, e->graph_epoch, exec, captured});
+  e->graphs.push_back({slot, d_in, d_labels, d_vol_scores, S, in_f32, e->graph_epoch, exec, captured});
   CU(cudaGraphLaunch(exec, e->st));
   e->launches += captured;
   e->graph_launches++;
   return 0;
 }
 
+// h_scores: the parity tap (host, synchronised per wave, plain launches).  d_vol_scores: a device buffer of the whole
+// volume's scores (S, K, 256, 256); each wave's head writes its slices at offset s0 * K * 256 * 256, graph-captured.
 int forward_all(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labels, float* h_scores,
-                float* conv_ms, bool in_f32 = false) {
+                float* conv_ms, bool in_f32 = false, float* d_vol_scores = nullptr) {
   if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
   Slot& s = e->slots[slot];
   float* d_scores = nullptr;
@@ -367,7 +375,7 @@ int forward_all(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labe
   }
   const bool timing = conv_ms != nullptr || e->time_convs;
   if (e->use_graphs && !timing && !h_scores) {
-    int gr = forward_graph(e, slot, d_in, S, d_labels, in_f32);
+    int gr = forward_graph(e, slot, d_in, S, d_labels, in_f32, d_vol_scores);
     if (gr == 0) {
       CU(cudaMemcpyAsync(e->h_range, e->d_range, LM_MAX_SLOTS * RANGE_STRIDE * sizeof(int), cudaMemcpyDeviceToHost, e->st));
       e->range_slot = slot;
@@ -379,7 +387,8 @@ int forward_all(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labe
     const int n = S - s0 < e->B ? S - s0 : e->B;
     const void* in_wave = in_f32 ? static_cast<const void*>(static_cast<const float*>(d_in) + (size_t)s0 * R * R)
                                  : static_cast<const void*>(static_cast<const int16_t*>(d_in) + (size_t)s0 * R * R);
-    RC(forward_batch(e, s, in_wave, in_f32, n, d_labels + (size_t)s0 * R * R, d_scores, conv_ms != nullptr || e->time_convs));
+    float* const wave_scores = d_vol_scores ? d_vol_scores + (size_t)s0 * s.K * R * R : d_scores;
+    RC(forward_batch(e, s, in_wave, in_f32, n, d_labels + (size_t)s0 * R * R, wave_scores, conv_ms != nullptr || e->time_convs));
     if (h_scores) {
       CU(cudaMemcpyAsync(h_scores + (size_t)s0 * s.K * R * R, d_scores, (size_t)n * s.K * R * R * sizeof(float),
                          cudaMemcpyDeviceToHost, e->st));
@@ -396,10 +405,17 @@ int forward_all(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labe
   return 0;
 }
 
+// Probability output of inference_dev (lm_apply_volume_probs): the head writes the volume's scores to `scores`
+// (S, K, 256, 256), and after the mask reshape probs_device writes (K, n0, n1, n2) to `probs` in the native orientation
+// given by perm / flip (identity: the volume is LPS).
+struct ProbOut { float* scores; float* probs; int perm[3]; int flip[3]; };
+
 // preprocess -> forward -> postprocess -> reshape, all device-resident. d_out: (S,H,W) uint8.
 // vtype: 0 = int16 HU volume, 1 = float32, 2 = float64 (float volumes keep their dtype through the reference's
 // pre-processing and normalisation; preproc.cu resize_kernel)
-int inference_dev(lm_engine* e, int slot, const void* d_vol, int S, int H, int W, int flags, uint8_t* d_out, int vtype = 0) {
+int inference_dev(lm_engine* e, int slot, const void* d_vol, int S, int H, int W, int flags, uint8_t* d_out, int vtype = 0,
+                  const ProbOut* prob = nullptr) {
+  float* const d_vol_scores = prob ? prob->scores : nullptr;
   const size_t nr = (size_t)S * R * R;
   RC(e->d_boxes.reserve((size_t)S * 4));
   if (vtype == 0) RC(e->d_resized.reserve(nr)); else RC(e->d_norm.reserve(nr));
@@ -415,8 +431,8 @@ int inference_dev(lm_engine* e, int slot, const void* d_vol, int S, int H, int W
   }
   e->launches += 2;
   CU(cudaEventRecord(e->ev[2], e->st));
-  if (vtype == 0) RC(forward_all(e, slot, e->d_resized.p, S, e->d_labels.p, nullptr, nullptr));
-  else RC(forward_all(e, slot, e->d_norm.p, S, e->d_labels.p, nullptr, nullptr, true));
+  if (vtype == 0) RC(forward_all(e, slot, e->d_resized.p, S, e->d_labels.p, nullptr, nullptr, false, d_vol_scores));
+  else RC(forward_all(e, slot, e->d_norm.p, S, e->d_labels.p, nullptr, nullptr, true, d_vol_scores));
   CU(cudaEventRecord(e->ev[3], e->st));
   const uint8_t* masks = e->d_labels.p;
   if (!(flags & LM_FLAG_NO_POSTPROCESS)) {
@@ -428,6 +444,11 @@ int inference_dev(lm_engine* e, int slot, const void* d_vol, int S, int H, int W
   CU(cudaEventRecord(e->ev[4], e->st));
   RC(reshape_device(masks, e->d_boxes.p, S, H, W, R, R, d_out, e->num_sms, e->st));
   e->launches++;
+  if (prob) {
+    const int dl[3] = {S, H, W};
+    RC(probs_device(prob->scores, e->d_boxes.p, e->slots[slot].K, R, R, dl, prob->perm, prob->flip, prob->probs, e->num_sms, e->st));
+    e->launches++;
+  }
   CU(cudaEventRecord(e->ev[5], e->st));
   return 0;
 }
@@ -679,7 +700,7 @@ void lm_destroy(lm_engine* e) {
     cudaFree(s.stem_w); cudaFree(s.stem_bias); cudaFree(s.stem_scale); cudaFree(s.stem_shift); cudaFree(s.head_w); cudaFree(s.head_b);
     for (auto& l : s.lw) { cudaFree(l.w); cudaFree(l.bias); cudaFree(l.scale); cudaFree(l.shift); }
   }
-  e->d_norm.release(); e->d_fvol.release();
+  e->d_norm.release(); e->d_fvol.release(); e->d_fnative.release(); e->d_probs.release();
   e->d_native.release(); e->d_lps_out.release(); e->d_native_l.release(); e->d_native_r.release();
   e->d_vol.release(); e->d_resized.release(); e->d_boxes.release(); e->d_labels.release(); e->d_post.release();
   e->d_out.release(); e->d_out2.release(); e->d_fused.release(); e->d_mask.release(); e->d_scores.release(); e->d_scratch.release();
@@ -966,6 +987,73 @@ int lm_apply_volume_oriented(lm_engine* e, int slot, int slot_fill, const int16_
       result = e->d_fused.p;
     }
     CU(cudaMemcpyAsync(out, result, n, cudaMemcpyDeviceToHost, e->st));
+    CU(cudaEventRecord(e->ev[6], e->st));
+    return 0;
+  }));
+  collect_timings(e);
+  return 0;
+}
+
+int lm_apply_volume_probs(lm_engine* e, int slot, const void* vol, int dtype, int n0, int n1, int n2, const int* perm,
+                          const int* flip, int flags, uint8_t* out, float* probs) {
+  if (!e || !vol || !out || !probs) return fail(-1, "lm_apply_volume_probs: NULL argument");
+  if ((perm == nullptr) != (flip == nullptr)) return fail(-1, "lm_apply_volume_probs: perm and flip must both be given or both be NULL");
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_volume_probs: empty volume");
+  if (dtype != LM_DTYPE_I16 && dtype != LM_DTYPE_F32 && dtype != LM_DTYPE_F64)
+    return fail(-1, "lm_apply_volume_probs: dtype %d is not LM_DTYPE_I16, LM_DTYPE_F32 or LM_DTYPE_F64", dtype);
+  int pm[3] = {0, 1, 2}, fl[3] = {0, 0, 0};
+  if (perm) {
+    int seen = 0;
+    for (int k = 0; k < 3; ++k) {
+      if (perm[k] < 0 || perm[k] > 2) return fail(-1, "lm_apply_volume_probs: perm is not a permutation");
+      seen |= 1 << perm[k];
+      pm[k] = perm[k];
+      fl[k] = flip[k] != 0;
+    }
+    if (seen != 7) return fail(-1, "lm_apply_volume_probs: perm is not a permutation");
+  }
+  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
+  CU(cudaSetDevice(e->device));
+  const bool lps = pm[0] == 0 && pm[1] == 1 && pm[2] == 2 && !fl[0] && !fl[1] && !fl[2];
+  const int dn[3] = {n0, n1, n2};
+  const int dl[3] = {dn[pm[0]], dn[pm[1]], dn[pm[2]]};   // the LPS array: (slices, rows, columns) of the path
+  const int K = e->slots[slot].K;
+  const size_t n = (size_t)n0 * n1 * n2, esz = dtype == LM_DTYPE_I16 ? 2 : (dtype == LM_DTYPE_F32 ? 4 : 8);
+  const int vtype = dtype == LM_DTYPE_I16 ? 0 : (dtype == LM_DTYPE_F32 ? 1 : 2);
+  void* d_lps_in = nullptr;     // the LPS volume the path reads
+  void* d_native_in = nullptr;  // the upload target when the volume is not LPS
+  if (vtype == 0) {
+    RC(e->d_vol.reserve(n));
+    d_lps_in = e->d_vol.p;
+    if (!lps) { RC(e->d_native.reserve(n)); d_native_in = e->d_native.p; }
+  } else {
+    RC(e->d_fvol.reserve(n * esz));
+    d_lps_in = e->d_fvol.p;
+    if (!lps) { RC(e->d_fnative.reserve(n * esz)); d_native_in = e->d_fnative.p; }
+  }
+  RC(e->d_out.reserve(n));
+  if (!lps) RC(e->d_lps_out.reserve(n));
+  RC(e->d_scores.reserve((size_t)dl[0] * K * R * R));
+  RC(e->d_probs.reserve((size_t)K * n));
+  ProbOut po{e->d_scores.p, e->d_probs.p, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]}};
+  RC(run_checked(e, [&]() -> int {
+    e->launches = 0;
+    e->ev_used = 0;
+    CU(cudaEventRecord(e->ev[0], e->st));
+    CU(cudaMemcpyAsync(lps ? d_lps_in : d_native_in, vol, n * esz, cudaMemcpyHostToDevice, e->st));
+    if (!lps) {   // sitk.DICOMOrient(image, "LPS"), mask.py:163
+      if (vtype == 0) RC(launch_orient_i16(static_cast<const int16_t*>(d_native_in), static_cast<int16_t*>(d_lps_in), dl, pm, fl, 1,
+                                           e->num_sms, e->st));
+      else RC(launch_orient_float(d_native_in, d_lps_in, vtype == 2, dl, pm, fl, 1, e->num_sms, e->st));
+      e->launches++;
+    }
+    RC(inference_dev(e, slot, d_lps_in, dl[0], dl[1], dl[2], flags, lps ? e->d_out.p : e->d_lps_out.p, vtype, &po));
+    if (!lps) {   // the mask back to the native orientation, mask.py:204-208
+      RC(launch_orient_u8(e->d_lps_out.p, e->d_out.p, dl, pm, fl, 0, e->num_sms, e->st));
+      e->launches++;
+    }
+    CU(cudaMemcpyAsync(out, e->d_out.p, n, cudaMemcpyDeviceToHost, e->st));
+    CU(cudaMemcpyAsync(probs, e->d_probs.p, (size_t)K * n * sizeof(float), cudaMemcpyDeviceToHost, e->st));
     CU(cudaEventRecord(e->ev[6], e->st));
     return 0;
   }));

@@ -27,6 +27,7 @@
 #include <string.h>
 #include <cooperative_groups.h>
 #include "postproc.cuh"
+#include "preproc.cuh"   // OrientMap, orient_lps_of_native (probs_kernel)
 
 namespace cg = cooperative_groups;
 
@@ -1013,6 +1014,33 @@ __global__ void reshape_kernel(const uint8_t* __restrict__ masks, const int32_t*
     out[i] = v;
   }
 }
+// Per-class probabilities at the input's resolution, in its native orientation (lm_apply_volume_probs): one thread per
+// native voxel finds its LPS voxel (orient_lps_of_native) and the network pixel reshape_kernel samples there, and writes
+// p_k = expf(score_k) of that pixel for every class k, (K, n0, n1, n2).  Voxels reshape_kernel sets to 0 (outside the
+// crop box, or scipy's constant-mode last row / column) get p_0 = 1, p_k = 0.  scores: (S, K, MH, MW) log-softmax.
+__global__ void __launch_bounds__(256) probs_kernel(const float* __restrict__ scores, const int32_t* __restrict__ boxes, OrientMap m,
+                                                    int K, int MH, int MW, float* __restrict__ probs) {
+  int dn[3];   // native dims, dn[perm[k]] = dl[k] (selects: a run-time index would put dn in local memory)
+  for (int j = 0; j < 3; ++j) dn[j] = m.perm[0] == j ? m.dl[0] : (m.perm[1] == j ? m.dl[1] : m.dl[2]);
+  const size_t n = (size_t)m.dl[0] * m.dl[1] * m.dl[2], plane = (size_t)MH * MW;
+  for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < n; t += (size_t)gridDim.x * blockDim.x) {
+    int i[3];
+    orient_lps_of_native(m, dn, t, i);
+    const int s = i[0], y = i[1], x = i[2];
+    const int32_t* b = boxes + 4 * s;
+    int iy = -1, ix = -1;
+    if (y >= b[0] && y < b[2] && x >= b[1] && x < b[3]) {
+      iy = nn_index_f64(MH, b[2] - b[0], y - b[0]);
+      ix = nn_index_f64(MW, b[3] - b[1], x - b[1]);
+    }
+    if (iy >= 0 && ix >= 0) {
+      const float* sc = scores + (size_t)s * K * plane + (size_t)iy * MW + ix;
+      for (int k = 0; k < K; ++k) probs[(size_t)k * n + t] = expf(sc[(size_t)k * plane]);
+    } else {
+      for (int k = 0; k < K; ++k) probs[(size_t)k * n + t] = k == 0 ? 1.f : 0.f;
+    }
+  }
+}
 __global__ void max_u8_kernel(const uint8_t* __restrict__ a, size_t n, uint32_t* __restrict__ mx) {
   uint32_t m = 0;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) m = max(m, (uint32_t)a[i]);
@@ -1350,6 +1378,15 @@ int reshape_device(const uint8_t* d_masks, const int32_t* d_boxes, int S, int H,
   const size_t n = (size_t)S * H * W;
   if (n < 0xFFFFFFF0ull) reshape_kernel<uint32_t><<<grid_for(n, 256, num_sms), 256, 0, st>>>(d_masks, d_boxes, S, H, W, MH, MW, d_out);
   else reshape_kernel<size_t><<<grid_for(n, 256, num_sms), 256, 0, st>>>(d_masks, d_boxes, S, H, W, MH, MW, d_out);
+  return (int)cudaGetLastError();
+}
+
+int probs_device(const float* d_scores, const int32_t* d_boxes, int K, int MH, int MW, const int dims_lps[3], const int perm[3],
+                 const int flip[3], float* d_probs, int num_sms, cudaStream_t st) {
+  OrientMap m;
+  for (int k = 0; k < 3; ++k) { m.dl[k] = dims_lps[k]; m.perm[k] = perm[k]; m.flip[k] = flip[k]; }
+  const size_t n = (size_t)dims_lps[0] * dims_lps[1] * dims_lps[2];
+  probs_kernel<<<grid_for(n, 256, num_sms), 256, 0, st>>>(d_scores, d_boxes, m, K, MH, MW, d_probs);
   return (int)cudaGetLastError();
 }
 

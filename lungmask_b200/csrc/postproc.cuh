@@ -61,6 +61,11 @@ int keep_largest_component_device(PostScratch& ws, const uint8_t* d_mask, int S,
 // utils.reshape_mask for every slice: (S,MH,MW) masks + (S,4) boxes -> (S,H,W).
 int reshape_device(const uint8_t* d_masks, const int32_t* d_boxes, int S, int H, int W, int MH, int MW, uint8_t* d_out,
                    int num_sms, cudaStream_t st);
+// Per-class probabilities in the native orientation: d_scores (S,K,MH,MW) log-softmax of the LPS volume's slices, boxes
+// of those slices -> d_probs (K, n0, n1, n2) float32, p_k = expf(score_k) of the pixel reshape_device samples for the voxel
+// (p_0 = 1 where it writes 0).  dims_lps / perm / flip as launch_orient_* (identity perm, no flips: the volume is LPS).
+int probs_device(const float* d_scores, const int32_t* d_boxes, int K, int MH, int MW, const int dims_lps[3], const int perm[3],
+                 const int flip[3], float* d_probs, int num_sms, cudaStream_t st);
 // mask.py:228-230 in place on d_res_l; the spare label value (uint8 arithmetic: max + 1) is left in d_spare_out[0]
 // (device int32) for postprocess_device.  No host synchronisation.
 int fuse_device(uint8_t* d_res_l, const uint8_t* d_res_r, size_t n, uint32_t* d_scratch, int32_t* d_spare_out, int num_sms,

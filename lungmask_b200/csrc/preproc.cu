@@ -339,16 +339,13 @@ resize_kernel(const VT* __restrict__ vol, int S, int H, int W, const int32_t* __
   }
 }
 
-// Axis permutation + flips between an array in its native orientation and the LPS array the path works on
-// (sitk.DICOMOrient, mask.py:157-164,204-208; lungmask_b200/orient.py states the index map):
-//   lps[i0][i1][i2] = native[c],  c[perm[k]] = flip[k] ? dims_lps[k] - 1 - i_k : i_k.
+// Native orientation <-> LPS (OrientMap, preproc.cuh).
 // to_lps != 0: threads walk the LPS array (coalesced writes) and gather; to_lps == 0: threads walk the native array
-// (coalesced writes) and gather from the LPS array - the inverse map.
-struct OrientMap { int dl[3]; int perm[3]; int flip[3]; };
+// (coalesced writes) and gather from the LPS array - the inverse map, orient_lps_of_native.
 template <typename T>
 __global__ void __launch_bounds__(256) orient_kernel(const T* __restrict__ src, T* __restrict__ dst, OrientMap m, int to_lps) {
-  int dn[3];  // native dims: dn[perm[k]] = dl[k]
-  for (int k = 0; k < 3; ++k) dn[m.perm[k]] = m.dl[k];
+  int dn[3];  // native dims: dn[perm[k]] = dl[k] (selects: a run-time index would put dn in local memory)
+  for (int j = 0; j < 3; ++j) dn[j] = m.perm[0] == j ? m.dl[0] : (m.perm[1] == j ? m.dl[1] : m.dl[2]);
   const size_t n = (size_t)m.dl[0] * m.dl[1] * m.dl[2];
   for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < n; t += (size_t)gridDim.x * blockDim.x) {
     if (to_lps) {
@@ -356,16 +353,13 @@ __global__ void __launch_bounds__(256) orient_kernel(const T* __restrict__ src, 
       i[2] = (int)(t % m.dl[2]);
       i[1] = (int)((t / m.dl[2]) % m.dl[1]);
       i[0] = (int)(t / ((size_t)m.dl[2] * m.dl[1]));
-      int c[3];
-      for (int k = 0; k < 3; ++k) c[m.perm[k]] = m.flip[k] ? m.dl[k] - 1 - i[k] : i[k];
+      int v[3], c[3];   // c[perm[k]] = v[k]
+      for (int k = 0; k < 3; ++k) v[k] = m.flip[k] ? m.dl[k] - 1 - i[k] : i[k];
+      for (int j = 0; j < 3; ++j) c[j] = m.perm[0] == j ? v[0] : (m.perm[1] == j ? v[1] : v[2]);
       dst[t] = src[((size_t)c[0] * dn[1] + c[1]) * dn[2] + c[2]];
     } else {
-      int c[3];
-      c[2] = (int)(t % dn[2]);
-      c[1] = (int)((t / dn[2]) % dn[1]);
-      c[0] = (int)(t / ((size_t)dn[2] * dn[1]));
       int i[3];
-      for (int k = 0; k < 3; ++k) i[k] = m.flip[k] ? m.dl[k] - 1 - c[m.perm[k]] : c[m.perm[k]];
+      orient_lps_of_native(m, dn, t, i);
       dst[t] = src[((size_t)i[0] * m.dl[1] + i[1]) * m.dl[2] + i[2]];
     }
   }
@@ -392,6 +386,13 @@ int launch_orient_i16(const int16_t* src, int16_t* dst, const int dims_lps[3], c
 int launch_orient_u8(const uint8_t* src, uint8_t* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
                      int num_sms, cudaStream_t stream) {
   return launch_orient_t<uint8_t>(src, dst, dims_lps, perm, flip, to_lps, num_sms, stream);
+}
+int launch_orient_float(const void* src, void* dst, int is_f64, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
+                        int num_sms, cudaStream_t stream) {
+  return is_f64 ? launch_orient_t<double>(static_cast<const double*>(src), static_cast<double*>(dst), dims_lps, perm, flip, to_lps,
+                                          num_sms, stream)
+                : launch_orient_t<float>(static_cast<const float*>(src), static_cast<float*>(dst), dims_lps, perm, flip, to_lps,
+                                         num_sms, stream);
 }
 
 int preproc_smem_bytes() { return (int)sizeof(Smem); }

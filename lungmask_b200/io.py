@@ -13,8 +13,9 @@ handling of mask.py:157-164) and enough geometry to write the mask back next to 
   * MetaImage (.mha, and .mhd + raw), uncompressed;
   * .npy (array only, identity geometry);
 
-and writes masks as .nii / .nii.gz / .mha / .npy with the input's geometry.  DICOM tags are never copied into the
-output (what `--removemetadata` asks for is therefore always the case here).
+and writes masks as .nii / .nii.gz / .mha / .npy with the input's geometry, and per-class probability maps as .npy or
+4-D .nii / .nii.gz.  DICOM tags are never copied into the output (what `--removemetadata` asks for is therefore always
+the case here).
 """
 import gzip
 import os
@@ -268,17 +269,18 @@ def _read_nifti(path):
 
 
 def _write_nifti(path, arr, like):
+    """(z, y, x) array -> 3-D image; (n, z, y, x) -> 4-D image of n volumes (dim[4] = n), same spatial header."""
     arr = np.ascontiguousarray(arr)
     code = {v: k for k, v in _NII_DTYPES.items()}[arr.dtype.type]
-    nz, ny, nx = arr.shape
+    nt, (nz, ny, nx) = (arr.shape[0], arr.shape[1:]) if arr.ndim == 4 else (1, arr.shape)
     D = np.asarray(like.direction, dtype=np.float64).reshape(3, 3)
     M = _LPS_FLIP @ (D * np.asarray(like.spacing, dtype=np.float64))
     t = _LPS_FLIP @ np.asarray(like.origin, dtype=np.float64)
     hdr = bytearray(352)
     struct.pack_into("<i", hdr, 0, 348)
-    struct.pack_into("<8h", hdr, 40, 3, nx, ny, nz, 1, 1, 1, 1)
+    struct.pack_into("<8h", hdr, 40, arr.ndim, nx, ny, nz, nt, 1, 1, 1)
     struct.pack_into("<hh", hdr, 70, code, arr.dtype.itemsize * 8)
-    struct.pack_into("<8f", hdr, 76, 1.0, *[float(s) for s in like.spacing], 0.0, 0.0, 0.0, 0.0)
+    struct.pack_into("<8f", hdr, 76, 1.0, *[float(s) for s in like.spacing], 1.0 if arr.ndim == 4 else 0.0, 0.0, 0.0, 0.0)
     struct.pack_into("<f", hdr, 108, 352.0)
     struct.pack_into("<2f", hdr, 112, 1.0, 0.0)
     hdr[123] = 2                                                       # xyzt_units: mm
@@ -378,3 +380,28 @@ def save_mask(path, mask, like=None):
         _write_mha(path, mask, like)
     else:
         raise SystemExit("unsupported output format (use .nii, .nii.gz, .mha or .npy): %s" % path)
+
+
+def check_probabilities_path(path):
+    """Refuses, before any work is done, an output path save_probabilities cannot write."""
+    low = path.lower()
+    if low.endswith(".mha"):
+        raise SystemExit("probability maps are 4-D (class, z, y, x); MetaImage output is not supported for them, "
+                         "use .nii, .nii.gz or .npy: %s" % path)
+    if not low.endswith((".npy", ".nii", ".nii.gz")):
+        raise SystemExit("unsupported probability output format (use .nii, .nii.gz or .npy): %s" % path)
+
+
+def save_probabilities(path, probs, like=None):
+    """Writes the float32 class probabilities (K, z, y, x) of LMInferer.apply_with_probabilities: .npy as is, or a 4-D
+    NIfTI-1 image (dim[0] = 4, dim[4] = K) whose spatial header (sform, spacing, origin) is the one save_mask writes
+    for the mask of the same `like`."""
+    probs = np.asarray(probs)
+    if probs.ndim != 4:
+        raise ValueError("expected (classes, z, y, x) probabilities, got shape %s" % (probs.shape,))
+    check_probabilities_path(path)
+    like = like if like is not None else Volume(probs[0])
+    if path.lower().endswith(".npy"):
+        np.save(path, probs)
+    else:
+        _write_nifti(path, probs, like)

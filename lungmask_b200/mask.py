@@ -207,18 +207,42 @@ class LMInferer:
         own orientation (mask.py:157-164,204-208)."""
         return self._run(array, orient.orientation_from_direction(direction))
 
+    def _array_and_orientation(self, image, caller: str = "apply"):
+        """(array (z, y, x), orientation code) of what `apply` accepts: a numpy array is taken as LPS; a
+        lungmask_b200.io.Volume or a SimpleITK image carries its direction cosines."""
+        if isinstance(image, np.ndarray):
+            return image, "LPS"
+        from .io import Volume
+        if isinstance(image, Volume):       # what lungmask_b200.io.load_input_image returns
+            return image.array, orient.orientation_from_direction(image.GetDirection())
+        sitk = self._sitk()
+        if sitk is None or not isinstance(image, sitk.Image):
+            raise TypeError("%s() expects a numpy array, a SimpleITK image or a lungmask_b200.io.Volume" % caller)
+        return sitk.GetArrayFromImage(image), orient.orientation_from_direction(image.GetDirection())
+
     def apply(self, image) -> np.ndarray:
         """Segments a volume: numpy (slices, H, W), sitk.Image or lungmask_b200.io.Volume -> uint8 labels of the same shape
         (lungmask/mask.py:212-232).  The input is not modified."""
-        if isinstance(image, np.ndarray):
-            return self._run(image)
-        from .io import Volume
-        if isinstance(image, Volume):       # what lungmask_b200.io.load_input_image returns
-            return self.apply_oriented(image.array, image.GetDirection())
-        sitk = self._sitk()
-        if sitk is None or not isinstance(image, sitk.Image):
-            raise TypeError("apply() expects a numpy array, a SimpleITK image or a lungmask_b200.io.Volume")
-        return self.apply_oriented(sitk.GetArrayFromImage(image), image.GetDirection())
+        return self._run(*self._array_and_orientation(image))
+
+    def apply_with_probabilities(self, image):
+        """The mask and the per-class probabilities of the model from one forward pass: image as for `apply` ->
+        (mask, probabilities).
+
+        `mask` is bit-identical to `apply(image)`, `volume_postprocessing` included.  `probabilities` is float32 of shape
+        (K, *mask.shape), in the input's own geometry and orientation: probabilities[k] = exp of the network's
+        log-softmax score of class k (what the reference's `inferer.model(x)` returns), taken from the network pixel
+        that the mask's order-0 resampling (utils.reshape_mask) puts at that voxel.  Voxels outside the slice's body
+        crop box are background with probability 1.  The probabilities are the network's output BEFORE
+        post-processing; with volume_postprocessing=False, their argmax is the mask.  Needs K * mask.size * 4 bytes on
+        the device and on the host.  Not defined for a fill model (the reference's fusion has no probabilities)."""
+        if self.fillmodel is not None:
+            raise ValueError("apply_with_probabilities: the fusion with a fill model (%s) has no class probabilities; "
+                             "use an LMInferer without fillmodel" % self.fillmodel)
+        array, code = self._array_and_orientation(image, "apply_with_probabilities")
+        vol = _to_engine_volume(array)
+        perm, flip = (None, None) if code == "LPS" else orient.array_transform_to_lps(code)
+        return self.engine.apply_volume_probs(0, vol, perm, flip, postprocess=self.volume_postprocessing)
 
 
 def apply(image, model=None, force_cpu=False, batch_size=20, volume_postprocessing=True, tqdm_disable=False):
