@@ -122,6 +122,35 @@ LM_API int lm_apply_volume_oriented(lm_engine* e, int slot, int slot_fill, const
 LM_API int lm_apply_volume_probs(lm_engine* e, int slot, const void* vol, int dtype, int n0, int n1, int n2,
                                  const int* perm, const int* flip, int flags, uint8_t* out, float* probs);
 
+/* The general device-resident entry point: lm_apply_volume / _float / _oriented / _fused / _probs on device memory, for
+ * callers that keep their volumes and results on the GPU (a PyTorch pipeline: LMInferer.apply on a CUDA tensor).
+ *   d_vol    (n0,n1,n2) C-contiguous on the engine's device, element type `dtype`, in its NATIVE orientation; perm / flip
+ *            as lm_apply_volume_oriented, both NULL: the array is LPS.  Never written.  LM_DTYPE_I16 / F32 / F64 take
+ *            the paths of the host entry points.  The integer codes (and bool as LM_DTYPE_U8) are clipped to
+ *            [-1024, 600] into int16, LM_DTYPE_F16 / BF16 are widened to float32 (LMInferer does the same on the host).
+ *   d_out    (n0,n1,n2) uint8 on the device: bit-identical to what the host entry points return for the same volume,
+ *            flags and orientation; slot_fill >= 0 selects the fusion (lm_apply_fused / lm_apply_volume_oriented).
+ *   d_probs  NULL, or (K,n0,n1,n2) float32 on the device: bit-identical to the probs of lm_apply_volume_probs.  Not with
+ *            slot_fill >= 0 (the fusion has no probabilities).
+ *   stream   the caller's cudaStream_t (NULL = the legacy default stream).  The engine records an event on it and makes
+ *            its own stream wait for that event before it reads d_vol, so work the caller queued on `stream` before the
+ *            call (the producer of d_vol) is complete first.  The call returns after the engine stream has
+ *            synchronised: d_out and d_probs are complete on return and `stream` needs no further wait.
+ * No host<->device copy.  An I16 / F32 / F64 volume in LPS is read in place; any other volume is converted and / or
+ * re-oriented into an engine buffer in one pass.  The engine allocates no probability buffer for this call; it keeps
+ * its usual work buffers (the whole volume's scores, S * K * 256 * 256 * 4 bytes, when d_probs is given).
+ * lm_last_timings: [0] is the wait for `stream` plus the conversion / orientation pass, [5] is the orientation of the
+ * results back to the native orientation (with slot_fill >= 0 also the fusion and its post-processing; there is no D2H
+ * copy); the other slots as for the host entry points. */
+#define LM_DTYPE_U8 3   /* also bool */
+#define LM_DTYPE_I8 4
+#define LM_DTYPE_I32 5
+#define LM_DTYPE_I64 6
+#define LM_DTYPE_F16 7
+#define LM_DTYPE_BF16 8
+LM_API int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol, int dtype, int n0, int n1, int n2,
+                        const int* perm, const int* flip, int flags, uint8_t* d_out, float* d_probs, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous
@@ -178,8 +207,8 @@ LM_API int lm_keep_largest_component(lm_engine* e, const uint8_t* mask, int S, i
 LM_API int lm_reshape_masks(lm_engine* e, const uint8_t* masks, int mask_h, int mask_w, const int32_t* boxes, int S,
                             int H, int W, uint8_t* out);
 
-/* Per-stage device time (ms, CUDA events on the engine stream) of the last lm_apply_volume*:
- * [0] H2D, [1] preprocess, [2] forward, [3] postprocess, [4] reshape, [5] D2H, [6] total.
+/* Per-stage device time (ms, CUDA events on the engine stream) of the last lm_apply_volume* / lm_apply_dev:
+ * [0] H2D, [1] preprocess, [2] forward, [3] postprocess, [4] reshape, [5] D2H, [6] total (lm_apply_dev: see there).
  * Also the number of kernels the engine launched in that call. */
 LM_API int lm_last_timings(const lm_engine* e, float* ms7, int64_t* kernel_launches);
 

@@ -10,6 +10,7 @@ LIB_PATH = os.path.join(_HERE, "liblungmask_b200.so")
 NET_RES = 256
 FLAG_NO_POSTPROCESS = 1
 DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2   # LM_DTYPE_* of lm_apply_volume_probs
+DTYPE_U8, DTYPE_I8, DTYPE_I32, DTYPE_I64, DTYPE_F16, DTYPE_BF16 = 3, 4, 5, 6, 7, 8   # lm_apply_dev only (U8 also bool)
 
 _lib = None
 
@@ -45,6 +46,7 @@ def lib():
         "lm_preprocess_float": ([vp, vp, i32, i32, i32, i32, f32p, i32p], i32),
         "lm_apply_volume_oriented": ([vp, i32, i32, i16p, i32, i32, i32, vp, vp, i32, u8p], i32),
         "lm_apply_volume_probs": ([vp, i32, vp, i32, i32, i32, i32, vp, vp, i32, u8p, f32p], i32),
+        "lm_apply_dev": ([vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, i32, u8p, f32p, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -74,7 +76,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -231,6 +233,24 @@ class Engine:
         _check(lib().lm_apply_volume_probs(self._h, slot, _ptr(vol), dtype, n0, n1, n2, pa, fa,
                                            0 if postprocess else FLAG_NO_POSTPROCESS, _ptr(out), _ptr(probs)))
         return out, probs
+
+    def apply_dev(self, slot, d_vol_ptr, dtype_code, shape, d_out_ptr, perm=None, flip=None, slot_fill=-1, d_probs_ptr=None,
+                  postprocess=True, stream=0):
+        """lm_apply_dev: the whole path on device memory of this engine's device.  `d_vol_ptr`: a C-contiguous `shape`
+        volume of element type `dtype_code` (DTYPE_*) in its native orientation; (perm, flip) as for apply_volume_probs.
+        Writes the uint8 mask to `d_out_ptr` and, if given, the (K,) + shape float32 probabilities to `d_probs_ptr` (not
+        with slot_fill >= 0).  `stream`: the caller's cudaStream_t as an int (0 = the legacy default stream); the engine
+        waits for the work queued on it before it reads the volume, and the results are complete when this returns."""
+        if (perm is None) != (flip is None):
+            raise ValueError("apply_dev: give both perm and flip, or neither")
+        pa = fa = None
+        if perm is not None:
+            pa = (C.c_int * 3)(*[int(x) for x in perm])
+            fa = (C.c_int * 3)(*[1 if x else 0 for x in flip])
+        n0, n1, n2 = (int(x) for x in shape)
+        _check(lib().lm_apply_dev(self._h, int(slot), int(slot_fill), C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2, pa, fa,
+                                  0 if postprocess else FLAG_NO_POSTPROCESS, C.c_void_p(d_out_ptr),
+                                  C.c_void_p(d_probs_ptr) if d_probs_ptr else None, C.c_void_p(int(stream)) if stream else None))
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

@@ -179,9 +179,9 @@ struct lm_engine {
   DevBuf<int32_t> d_boxes;
   DevBuf<uint8_t> d_labels, d_post, d_out, d_out2, d_fused, d_mask;
   DevBuf<float> d_scores, d_norm;   // d_scores: one wave of lm_forward's tap, or a whole volume of lm_apply_volume_probs
-  DevBuf<float> d_probs;            // lm_apply_volume_probs: (K, n0, n1, n2) probabilities
-  DevBuf<uint8_t> d_fvol;   // float volumes (float32 / float64), raw bytes
-  DevBuf<uint8_t> d_fnative;  // lm_apply_volume_probs: a float volume in its native orientation, raw bytes
+  DevBuf<float> d_probs;            // lm_apply_volume_probs: (K, n0, n1, n2) probabilities (lm_apply_dev writes the caller's)
+  DevBuf<uint8_t> d_fvol;   // float volumes (float32 / float64), raw bytes; also volume_enqueue's converted / LPS float volume
+  DevBuf<uint8_t> d_fnative;  // lm_apply_volume_probs: the uploaded float volume in its native orientation, raw bytes
   DevBuf<uint32_t> d_scratch;
   PostScratch post;
   cudaEvent_t ev[8] = {};
@@ -191,6 +191,7 @@ struct lm_engine {
   bool time_convs = false;
   float last_conv_ms = 0.f;
   int64_t last_conv_launches = 0;
+  cudaEvent_t ev_in = nullptr;       // lm_apply_dev: recorded on the caller's stream, waited for by the engine stream
   float last_ms[7] = {};
   int64_t launches = 0;
   // CUDA graphs of whole forwards (all waves of one volume: ~26 launches per wave), keyed by slot / buffers / slice count /
@@ -615,6 +616,117 @@ void collect_timings(lm_engine* e) {
   e->last_ms[6] = ms;
 }
 
+// perm / flip of the oriented entry points -> pm / fl; both NULL: the identity (an LPS array).
+int parse_orientation(const char* fn, const int* perm, const int* flip, int pm[3], int fl[3]) {
+  for (int k = 0; k < 3; ++k) { pm[k] = k; fl[k] = 0; }
+  if ((perm == nullptr) != (flip == nullptr)) return fail(-1, "%s: perm and flip must both be given or both be NULL", fn);
+  if (!perm) return 0;
+  int seen = 0;
+  for (int k = 0; k < 3; ++k) {
+    if (perm[k] < 0 || perm[k] > 2) return fail(-1, "%s: perm is not a permutation", fn);
+    seen |= 1 << perm[k];
+    pm[k] = perm[k];
+    fl[k] = flip[k] != 0;
+  }
+  if (seen != 7) return fail(-1, "%s: perm is not a permutation", fn);
+  return 0;
+}
+
+// A caller's pointer must be device (or managed) memory of the engine's device: a host pointer would fault in a kernel.
+int check_device_ptr(const lm_engine* e, const char* fn, const char* what, const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(-1, "%s: %s is not a CUDA pointer", fn, what);
+  }
+  if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != e->device)
+    return fail(-1, "%s: %s is not device memory of the engine's device %d", fn, what, e->device);
+  return 0;
+}
+
+// The volume type inference_dev works in for an LM_DTYPE_* code: 0 int16, 1 float32, 2 float64.
+int vtype_of(int dtype) {
+  if (dtype == LM_DTYPE_F64) return 2;
+  return (dtype == LM_DTYPE_F32 || dtype == LM_DTYPE_F16 || dtype == LM_DTYPE_BF16) ? 1 : 0;
+}
+size_t dtype_bytes(int dtype) {
+  switch (dtype) {
+    case LM_DTYPE_U8: case LM_DTYPE_I8: return 1;
+    case LM_DTYPE_I16: case LM_DTYPE_F16: case LM_DTYPE_BF16: return 2;
+    case LM_DTYPE_F32: case LM_DTYPE_I32: return 4;
+    default: return 8;
+  }
+}
+
+// One volume of LMInferer._inference / LMInferer.apply on device memory: the volume in its native orientation in, the
+// mask (and the probabilities) in that orientation out.  lm_apply_dev runs it on the caller's pointers,
+// lm_apply_volume_oriented and lm_apply_volume_probs on the engine buffers they upload to.
+struct VolumeJob {
+  int slot, slot_fill;   // slot_fill >= 0: the fusion of mask.py:223-232
+  const void* d_vol;     // (n0,n1,n2), element type `dtype` (LM_DTYPE_*); never written
+  int dtype, flags;
+  int dn[3], perm[3], flip[3];   // native dims; lps = transpose(native, perm) flipped along every axis k with flip[k]
+  uint8_t* d_out;        // (n0,n1,n2)
+  float* d_probs;        // nullptr, or (K,n0,n1,n2); not with slot_fill >= 0
+};
+
+// Enqueues the whole volume on the engine stream; the caller records ev[0] before and ev[6] after it.
+int volume_enqueue(lm_engine* e, const VolumeJob& j) {
+  const int* pm = j.perm;
+  const int* fl = j.flip;
+  const bool lps = pm[0] == 0 && pm[1] == 1 && pm[2] == 2 && !fl[0] && !fl[1] && !fl[2];
+  const int dl[3] = {j.dn[pm[0]], j.dn[pm[1]], j.dn[pm[2]]};   // the LPS array: (slices, rows, columns) of the path
+  const size_t n = (size_t)j.dn[0] * j.dn[1] * j.dn[2];
+  const int vtype = vtype_of(j.dtype);
+  const bool path_dtype = j.dtype == LM_DTYPE_I16 || j.dtype == LM_DTYPE_F32 || j.dtype == LM_DTYPE_F64;
+  const void* d_lps_in = j.d_vol;   // an LPS volume of a path dtype is read in place
+  if (!lps || !path_dtype) {
+    // sitk.DICOMOrient(image, "LPS") (mask.py:163) and / or the dtype conversion of mask.py _to_engine_volume, one pass
+    void* stage = nullptr;
+    if (vtype == 0) { RC(e->d_vol.reserve(n)); stage = e->d_vol.p; }
+    else { RC(e->d_fvol.reserve(n * (vtype == 2 ? 8 : 4))); stage = e->d_fvol.p; }
+    RC(launch_orient_convert(j.d_vol, j.dtype, stage, dl, pm, fl, e->num_sms, e->st));
+    e->launches++;
+    d_lps_in = stage;
+  }
+  if (!lps) RC(e->d_lps_out.reserve(n));
+  if (j.slot_fill < 0) {
+    ProbOut po{nullptr, j.d_probs, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]}};
+    if (j.d_probs) {
+      RC(e->d_scores.reserve((size_t)dl[0] * e->slots[j.slot].K * R * R));
+      po.scores = e->d_scores.p;
+    }
+    RC(inference_dev(e, j.slot, d_lps_in, dl[0], dl[1], dl[2], j.flags, lps ? j.d_out : e->d_lps_out.p, vtype,
+                     j.d_probs ? &po : nullptr));
+    if (!lps) {   // the mask back to the native orientation, mask.py:204-208
+      RC(launch_orient_u8(e->d_lps_out.p, j.d_out, dl, pm, fl, 0, e->num_sms, e->st));
+      e->launches++;
+    }
+    return 0;
+  }
+  // both inner inferences honour volume_postprocessing (mask.py:191-194); the fusion post-processing does not.  Each
+  // _inference call re-orients its own result back, and the fusion and its post-processing work on the NATIVE-orientation
+  // results (mask.py:225-232).
+  const int inner = j.flags & LM_FLAG_NO_POSTPROCESS;
+  RC(e->d_native_l.reserve(n));
+  RC(e->d_native_r.reserve(n));
+  const int slots[2] = {j.slot, j.slot_fill};
+  uint8_t* const res[2] = {e->d_native_l.p, e->d_native_r.p};   // res_l, res_r (mask.py:225,227)
+  for (int m = 0; m < 2; ++m) {
+    RC(inference_dev(e, slots[m], d_lps_in, dl[0], dl[1], dl[2], inner, lps ? res[m] : e->d_lps_out.p, vtype));
+    if (!lps) {
+      RC(launch_orient_u8(e->d_lps_out.p, res[m], dl, pm, fl, 0, e->num_sms, e->st));
+      e->launches++;
+    }
+  }
+  RC(fuse_device(res[0], res[1], n, e->d_scratch.p, e->d_spare, e->num_sms, e->st));   // spare stays on the device
+  e->launches += 3;
+  // labels after the fusion are <= K_base (the spare value is max + 1 <= K_base): mask.py:232
+  RC(postprocess_device(e->post, res[0], j.dn[0], j.dn[1], j.dn[2], nullptr, 0, e->d_spare, 1, 3, e->slots[j.slot].K, j.d_out,
+                        e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -672,6 +784,7 @@ static int create_resources(lm_engine* e) {
   CU(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
   for (int i = 0; i < 8; ++i) CU(cudaEventCreate(&e->ev[i]));
   for (int i = 0; i < 2; ++i) CU(cudaEventCreate(&e->ev_conv[i]));
+  CU(cudaEventCreateWithFlags(&e->ev_in, cudaEventDisableTiming));
   for (int a = 0; a < NUM_ACT; ++a) {
     const int hw = R >> ACT[a].level;
     const size_t elems = (size_t)batch_capacity * hw * hw * ACT[a].C;
@@ -708,6 +821,7 @@ void lm_destroy(lm_engine* e) {
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
+  if (e->ev_in) cudaEventDestroy(e->ev_in);
   cudaStreamDestroy(e->st);
   delete e;
 }
@@ -950,43 +1064,24 @@ int lm_apply_volume_oriented(lm_engine* e, int slot, int slot_fill, const int16_
                              const int* flip, int flags, uint8_t* out) {
   if (!e || !vol || !out || !perm || !flip) return fail(-1, "lm_apply_volume_oriented: NULL argument");
   if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_volume_oriented: empty volume");
-  int seen = 0;
-  for (int k = 0; k < 3; ++k) { if (perm[k] < 0 || perm[k] > 2) return fail(-1, "lm_apply_volume_oriented: perm is not a permutation"); seen |= 1 << perm[k]; }
-  if (seen != 7) return fail(-1, "lm_apply_volume_oriented: perm is not a permutation");
+  int pm[3], fl[3];
+  RC(parse_orientation("lm_apply_volume_oriented", perm, flip, pm, fl));
   if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
   const bool fused = slot_fill >= 0;
   if (fused && (slot_fill >= LM_MAX_SLOTS || !e->slots[slot_fill].loaded)) return fail(-30, "weight slot %d not loaded", slot_fill);
   CU(cudaSetDevice(e->device));
-  const int dn[3] = {n0, n1, n2};
-  const int dl[3] = {dn[perm[0]], dn[perm[1]], dn[perm[2]]};   // the LPS array: (slices, rows, columns) of the path
-  const int fl[3] = {flip[0] != 0, flip[1] != 0, flip[2] != 0};
   const size_t n = (size_t)n0 * n1 * n2;
   RC(e->d_native.reserve(n));
-  RC(e->d_vol.reserve(n));
-  RC(e->d_lps_out.reserve(n));
-  RC(e->d_native_l.reserve(n));
-  if (fused) { RC(e->d_native_r.reserve(n)); RC(e->d_fused.reserve(n)); }
+  RC(e->d_out.reserve(n));
+  const VolumeJob job{slot, fused ? slot_fill : -1, e->d_native.p, LM_DTYPE_I16, flags, {n0, n1, n2},
+                      {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]}, e->d_out.p, nullptr};
   RC(run_checked(e, [&]() -> int {
     e->launches = 0;
     e->ev_used = 0;
     CU(cudaEventRecord(e->ev[0], e->st));
     CU(cudaMemcpyAsync(e->d_native.p, vol, n * sizeof(int16_t), cudaMemcpyHostToDevice, e->st));
-    RC(launch_orient_i16(e->d_native.p, e->d_vol.p, dl, perm, fl, 1, e->num_sms, e->st));            // sitk.DICOMOrient(image, "LPS"), mask.py:163
-    const int inner = fused ? (flags & LM_FLAG_NO_POSTPROCESS) : flags;
-    RC(inference_dev(e, slot, e->d_vol.p, dl[0], dl[1], dl[2], inner, e->d_lps_out.p));
-    RC(launch_orient_u8(e->d_lps_out.p, e->d_native_l.p, dl, perm, fl, 0, e->num_sms, e->st));       // back, mask.py:204-208
-    e->launches += 2;
-    const uint8_t* result = e->d_native_l.p;
-    if (fused) {   // the fusion and its post-processing work on the NATIVE-orientation results (mask.py:225-232)
-      RC(inference_dev(e, slot_fill, e->d_vol.p, dl[0], dl[1], dl[2], inner, e->d_lps_out.p));
-      RC(launch_orient_u8(e->d_lps_out.p, e->d_native_r.p, dl, perm, fl, 0, e->num_sms, e->st));
-      RC(fuse_device(e->d_native_l.p, e->d_native_r.p, n, e->d_scratch.p, e->d_spare, e->num_sms, e->st));
-      e->launches += 4;
-      RC(postprocess_device(e->post, e->d_native_l.p, n0, n1, n2, nullptr, 0, e->d_spare, 1, 3, e->slots[slot].K, e->d_fused.p,
-                            e->num_sms, e->st, &e->launches));
-      result = e->d_fused.p;
-    }
-    CU(cudaMemcpyAsync(out, result, n, cudaMemcpyDeviceToHost, e->st));
+    RC(volume_enqueue(e, job));
+    CU(cudaMemcpyAsync(out, e->d_out.p, n, cudaMemcpyDeviceToHost, e->st));
     CU(cudaEventRecord(e->ev[6], e->st));
     return 0;
   }));
@@ -1001,59 +1096,61 @@ int lm_apply_volume_probs(lm_engine* e, int slot, const void* vol, int dtype, in
   if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_volume_probs: empty volume");
   if (dtype != LM_DTYPE_I16 && dtype != LM_DTYPE_F32 && dtype != LM_DTYPE_F64)
     return fail(-1, "lm_apply_volume_probs: dtype %d is not LM_DTYPE_I16, LM_DTYPE_F32 or LM_DTYPE_F64", dtype);
-  int pm[3] = {0, 1, 2}, fl[3] = {0, 0, 0};
-  if (perm) {
-    int seen = 0;
-    for (int k = 0; k < 3; ++k) {
-      if (perm[k] < 0 || perm[k] > 2) return fail(-1, "lm_apply_volume_probs: perm is not a permutation");
-      seen |= 1 << perm[k];
-      pm[k] = perm[k];
-      fl[k] = flip[k] != 0;
-    }
-    if (seen != 7) return fail(-1, "lm_apply_volume_probs: perm is not a permutation");
-  }
+  int pm[3], fl[3];
+  RC(parse_orientation("lm_apply_volume_probs", perm, flip, pm, fl));
   if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
   CU(cudaSetDevice(e->device));
-  const bool lps = pm[0] == 0 && pm[1] == 1 && pm[2] == 2 && !fl[0] && !fl[1] && !fl[2];
-  const int dn[3] = {n0, n1, n2};
-  const int dl[3] = {dn[pm[0]], dn[pm[1]], dn[pm[2]]};   // the LPS array: (slices, rows, columns) of the path
   const int K = e->slots[slot].K;
-  const size_t n = (size_t)n0 * n1 * n2, esz = dtype == LM_DTYPE_I16 ? 2 : (dtype == LM_DTYPE_F32 ? 4 : 8);
-  const int vtype = dtype == LM_DTYPE_I16 ? 0 : (dtype == LM_DTYPE_F32 ? 1 : 2);
-  void* d_lps_in = nullptr;     // the LPS volume the path reads
-  void* d_native_in = nullptr;  // the upload target when the volume is not LPS
-  if (vtype == 0) {
-    RC(e->d_vol.reserve(n));
-    d_lps_in = e->d_vol.p;
-    if (!lps) { RC(e->d_native.reserve(n)); d_native_in = e->d_native.p; }
-  } else {
-    RC(e->d_fvol.reserve(n * esz));
-    d_lps_in = e->d_fvol.p;
-    if (!lps) { RC(e->d_fnative.reserve(n * esz)); d_native_in = e->d_fnative.p; }
-  }
+  const size_t n = (size_t)n0 * n1 * n2, esz = dtype_bytes(dtype);
+  void* d_native_in = nullptr;  // the upload target: the volume in its native orientation
+  if (dtype == LM_DTYPE_I16) { RC(e->d_native.reserve(n)); d_native_in = e->d_native.p; }
+  else { RC(e->d_fnative.reserve(n * esz)); d_native_in = e->d_fnative.p; }
   RC(e->d_out.reserve(n));
-  if (!lps) RC(e->d_lps_out.reserve(n));
-  RC(e->d_scores.reserve((size_t)dl[0] * K * R * R));
   RC(e->d_probs.reserve((size_t)K * n));
-  ProbOut po{e->d_scores.p, e->d_probs.p, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]}};
+  const VolumeJob job{slot, -1, d_native_in, dtype, flags, {n0, n1, n2}, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]},
+                      e->d_out.p, e->d_probs.p};
   RC(run_checked(e, [&]() -> int {
     e->launches = 0;
     e->ev_used = 0;
     CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaMemcpyAsync(lps ? d_lps_in : d_native_in, vol, n * esz, cudaMemcpyHostToDevice, e->st));
-    if (!lps) {   // sitk.DICOMOrient(image, "LPS"), mask.py:163
-      if (vtype == 0) RC(launch_orient_i16(static_cast<const int16_t*>(d_native_in), static_cast<int16_t*>(d_lps_in), dl, pm, fl, 1,
-                                           e->num_sms, e->st));
-      else RC(launch_orient_float(d_native_in, d_lps_in, vtype == 2, dl, pm, fl, 1, e->num_sms, e->st));
-      e->launches++;
-    }
-    RC(inference_dev(e, slot, d_lps_in, dl[0], dl[1], dl[2], flags, lps ? e->d_out.p : e->d_lps_out.p, vtype, &po));
-    if (!lps) {   // the mask back to the native orientation, mask.py:204-208
-      RC(launch_orient_u8(e->d_lps_out.p, e->d_out.p, dl, pm, fl, 0, e->num_sms, e->st));
-      e->launches++;
-    }
+    CU(cudaMemcpyAsync(d_native_in, vol, n * esz, cudaMemcpyHostToDevice, e->st));
+    RC(volume_enqueue(e, job));
     CU(cudaMemcpyAsync(out, e->d_out.p, n, cudaMemcpyDeviceToHost, e->st));
     CU(cudaMemcpyAsync(probs, e->d_probs.p, (size_t)K * n * sizeof(float), cudaMemcpyDeviceToHost, e->st));
+    CU(cudaEventRecord(e->ev[6], e->st));
+    return 0;
+  }));
+  collect_timings(e);
+  return 0;
+}
+
+int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol, int dtype, int n0, int n1, int n2, const int* perm,
+                 const int* flip, int flags, uint8_t* d_out, float* d_probs, void* stream) {
+  if (!e || !d_vol || !d_out) return fail(-1, "lm_apply_dev: NULL argument");
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_dev: empty volume (%d,%d,%d)", n0, n1, n2);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "lm_apply_dev: unknown dtype code %d", dtype);
+  int pm[3], fl[3];
+  RC(parse_orientation("lm_apply_dev", perm, flip, pm, fl));
+  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
+  const bool fused = slot_fill >= 0;
+  if (fused && d_probs)
+    return fail(-1, "lm_apply_dev: no probabilities for the fusion with a fill model (slot_fill %d): the reference's fusion "
+                    "defines none", slot_fill);
+  if (fused && (slot_fill >= LM_MAX_SLOTS || !e->slots[slot_fill].loaded)) return fail(-30, "weight slot %d not loaded", slot_fill);
+  CU(cudaSetDevice(e->device));
+  RC(check_device_ptr(e, "lm_apply_dev", "d_vol", d_vol));
+  RC(check_device_ptr(e, "lm_apply_dev", "d_out", d_out));
+  if (d_probs) RC(check_device_ptr(e, "lm_apply_dev", "d_probs", d_probs));
+  const VolumeJob job{slot, fused ? slot_fill : -1, d_vol, dtype, flags, {n0, n1, n2}, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]},
+                      d_out, d_probs};
+  // the engine stream (non-blocking) is ordered after everything the caller queued on its stream so far
+  CU(cudaEventRecord(e->ev_in, static_cast<cudaStream_t>(stream)));
+  RC(run_checked(e, [&]() -> int {
+    e->launches = 0;
+    e->ev_used = 0;
+    CU(cudaEventRecord(e->ev[0], e->st));
+    CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
+    RC(volume_enqueue(e, job));
     CU(cudaEventRecord(e->ev[6], e->st));
     return 0;
   }));

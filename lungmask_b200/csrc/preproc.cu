@@ -11,6 +11,10 @@
 // full-resolution mask is never materialised (it is written only when a caller asks for it).
 // resize_kernel: one thread per output pixel, float64 coordinates and accumulation order as scipy's zoom.
 #include <atomic>
+#include <type_traits>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include "../../include/lungmask_b200.h"
 #include "preproc.cuh"
 
 namespace lm {
@@ -339,11 +343,32 @@ resize_kernel(const VT* __restrict__ vol, int S, int H, int W, const int32_t* __
   }
 }
 
-// Native orientation <-> LPS (OrientMap, preproc.cuh).
+// Element conversion of orient_kernel.  Tin == Tout: the value itself.  Integer (and bool) elements into int16: clipped to
+// [-1024, 600] first, as mask.py _to_int16_volume does on the host (the reference clips to that range before resampling
+// and thresholds at -500 HU, so the clip changes no result).  Half-precision floats: widened to float32.
+template <typename Tin, typename Tout>
+struct Convert {
+  static __device__ __forceinline__ Tout f(Tin x) {
+    if constexpr (std::is_same<Tin, Tout>::value) {
+      return x;
+    } else if constexpr (std::is_same<Tout, int16_t>::value) {
+      const long long v = (long long)x;
+      return (int16_t)(v < -1024 ? -1024 : (v > 600 ? 600 : v));
+    } else if constexpr (std::is_same<Tin, __half>::value) {
+      return __half2float(x);
+    } else {
+      static_assert(std::is_same<Tin, __nv_bfloat16>::value && std::is_same<Tout, float>::value, "unsupported conversion");
+      return __bfloat162float(x);
+    }
+  }
+};
+
+// Native orientation <-> LPS (OrientMap, preproc.cuh), every element passed through Convert<Tin, Tout>.
 // to_lps != 0: threads walk the LPS array (coalesced writes) and gather; to_lps == 0: threads walk the native array
-// (coalesced writes) and gather from the LPS array - the inverse map, orient_lps_of_native.
-template <typename T>
-__global__ void __launch_bounds__(256) orient_kernel(const T* __restrict__ src, T* __restrict__ dst, OrientMap m, int to_lps) {
+// (coalesced writes) and gather from the LPS array - the inverse map, orient_lps_of_native.  With the identity map the
+// kernel is a plain conversion pass.
+template <typename Tin, typename Tout>
+__global__ void __launch_bounds__(256) orient_kernel(const Tin* __restrict__ src, Tout* __restrict__ dst, OrientMap m, int to_lps) {
   int dn[3];  // native dims: dn[perm[k]] = dl[k] (selects: a run-time index would put dn in local memory)
   for (int j = 0; j < 3; ++j) dn[j] = m.perm[0] == j ? m.dl[0] : (m.perm[1] == j ? m.dl[1] : m.dl[2]);
   const size_t n = (size_t)m.dl[0] * m.dl[1] * m.dl[2];
@@ -356,28 +381,46 @@ __global__ void __launch_bounds__(256) orient_kernel(const T* __restrict__ src, 
       int v[3], c[3];   // c[perm[k]] = v[k]
       for (int k = 0; k < 3; ++k) v[k] = m.flip[k] ? m.dl[k] - 1 - i[k] : i[k];
       for (int j = 0; j < 3; ++j) c[j] = m.perm[0] == j ? v[0] : (m.perm[1] == j ? v[1] : v[2]);
-      dst[t] = src[((size_t)c[0] * dn[1] + c[1]) * dn[2] + c[2]];
+      dst[t] = Convert<Tin, Tout>::f(src[((size_t)c[0] * dn[1] + c[1]) * dn[2] + c[2]]);
     } else {
       int i[3];
       orient_lps_of_native(m, dn, t, i);
-      dst[t] = src[((size_t)i[0] * m.dl[1] + i[1]) * m.dl[2] + i[2]];
+      dst[t] = Convert<Tin, Tout>::f(src[((size_t)i[0] * m.dl[1] + i[1]) * m.dl[2] + i[2]]);
     }
   }
 }
 
 }  // namespace
 
-template <typename T>
-static int launch_orient_t(const T* src, T* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps, int num_sms,
-                           cudaStream_t stream) {
+template <typename Tin, typename Tout = Tin>
+static int launch_orient_t(const Tin* src, Tout* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
+                           int num_sms, cudaStream_t stream) {
   OrientMap m;
   for (int k = 0; k < 3; ++k) { m.dl[k] = dims_lps[k]; m.perm[k] = perm[k]; m.flip[k] = flip[k]; }
   const size_t n = (size_t)dims_lps[0] * dims_lps[1] * dims_lps[2];
   size_t g = (n + 255) / 256;
   if (g > (size_t)num_sms * 16) g = (size_t)num_sms * 16;
   if (g < 1) g = 1;
-  orient_kernel<T><<<(int)g, 256, 0, stream>>>(src, dst, m, to_lps);
+  orient_kernel<Tin, Tout><<<(int)g, 256, 0, stream>>>(src, dst, m, to_lps);
   return (int)cudaGetLastError();
+}
+int launch_orient_convert(const void* src, int dtype, void* dst, const int dims_lps[3], const int perm[3], const int flip[3],
+                          int num_sms, cudaStream_t stream) {
+  int16_t* const d16 = static_cast<int16_t*>(dst);
+  float* const d32 = static_cast<float*>(dst);
+  switch (dtype) {
+    case LM_DTYPE_I16: return launch_orient_t(static_cast<const int16_t*>(src), d16, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_F32: return launch_orient_t(static_cast<const float*>(src), d32, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_F64:
+      return launch_orient_t(static_cast<const double*>(src), static_cast<double*>(dst), dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_U8: return launch_orient_t(static_cast<const uint8_t*>(src), d16, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_I8: return launch_orient_t(static_cast<const int8_t*>(src), d16, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_I32: return launch_orient_t(static_cast<const int32_t*>(src), d16, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_I64: return launch_orient_t(static_cast<const int64_t*>(src), d16, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_F16: return launch_orient_t(static_cast<const __half*>(src), d32, dims_lps, perm, flip, 1, num_sms, stream);
+    case LM_DTYPE_BF16: return launch_orient_t(static_cast<const __nv_bfloat16*>(src), d32, dims_lps, perm, flip, 1, num_sms, stream);
+    default: return -1;
+  }
 }
 int launch_orient_i16(const int16_t* src, int16_t* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
                       int num_sms, cudaStream_t stream) {

@@ -27,6 +27,11 @@ int launch_orient_u8(const uint8_t* src, uint8_t* dst, const int dims_lps[3], co
 // The same for float volumes: float64 with is_f64 != 0, else float32.
 int launch_orient_float(const void* src, void* dst, int is_f64, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
                         int num_sms, cudaStream_t stream);
+// Native -> LPS in one pass with the element conversion of lm_apply_dev: src of element type `dtype` (LM_DTYPE_*);
+// dst int16 for LM_DTYPE_I16 and the integer codes (clipped to [-1024, 600] unless already int16), float32 for
+// LM_DTYPE_F32 / F16 / BF16, float64 for LM_DTYPE_F64.  Returns -1 for an unknown code.
+int launch_orient_convert(const void* src, int dtype, void* dst, const int dims_lps[3], const int perm[3], const int flip[3],
+                          int num_sms, cudaStream_t stream);
 
 // Axis permutation + flips between an array in its native orientation and the LPS array the path works on
 // (sitk.DICOMOrient, mask.py:157-164,204-208; lungmask_b200/orient.py states the index map):

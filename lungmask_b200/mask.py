@@ -115,6 +115,24 @@ def _to_engine_volume(image: np.ndarray) -> np.ndarray:
     return _to_int16_volume(image)
 
 
+def _is_tensor(image) -> bool:
+    import torch
+    return isinstance(image, torch.Tensor)
+
+
+def _tensor_dtype_code(t) -> int:
+    """LM_DTYPE_* of lm_apply_dev for a tensor's dtype; TypeError for the dtypes the engine does not read."""
+    import torch
+    codes = {torch.bool: _native.DTYPE_U8, torch.uint8: _native.DTYPE_U8, torch.int8: _native.DTYPE_I8,
+             torch.int16: _native.DTYPE_I16, torch.int32: _native.DTYPE_I32, torch.int64: _native.DTYPE_I64,
+             torch.float16: _native.DTYPE_F16, torch.bfloat16: _native.DTYPE_BF16, torch.float32: _native.DTYPE_F32,
+             torch.float64: _native.DTYPE_F64}
+    if t.dtype not in codes:
+        raise TypeError("volume tensor dtype %s is not supported: use bool, uint8, a signed integer type, float16, bfloat16, "
+                        "float32 or float64" % t.dtype)
+    return codes[t.dtype]
+
+
 class LMInferer:
     def __init__(
         self,
@@ -178,20 +196,27 @@ class LMInferer:
         except Exception:
             return None
 
+    def _log_fusion(self):
+        logger.info(f"Apply: {self.modelname}")
+        logger.info(f"Apply: {self.fillmodel}")
+        logger.info("Fusing results... this may take up to several minutes!")
+
     def _run(self, volume: np.ndarray, code: str = "LPS") -> np.ndarray:
         vol = _to_engine_volume(volume)
         fused = self.fillmodel is not None
+        if vol.dtype != np.int16 and code != "LPS" and fused:
+            # the fusion runs in the native orientation (mask.py:225-232): the engine's device path does the re-orientation,
+            # so the volume goes through a CUDA tensor on the engine's device
+            import torch
+            src = torch.from_numpy(vol if vol.flags.writeable else vol.copy()).to(torch.device("cuda", self.engine.device))
+            return self._run_tensor(src, code).cpu().numpy()
         if fused:
-            logger.info(f"Apply: {self.modelname}")
-            logger.info(f"Apply: {self.fillmodel}")
-            logger.info("Fusing results... this may take up to several minutes!")
+            self._log_fusion()
         if vol.dtype != np.int16:   # float volume
             if code != "LPS":       # re-orient on the host (rare: float + non-LPS); the integer path does it on the device
-                res = self.engine.apply_volume_float(0, orient.to_lps(vol, code), slot_fill=-1 if not fused else 1,
+                res = self.engine.apply_volume_float(0, orient.to_lps(vol, code), slot_fill=-1,
                                                      postprocess=self.volume_postprocessing)
-                if not fused:
-                    return orient.from_lps(res, code)
-                raise NotImplementedError("fusion of a float volume in a non-LPS orientation: re-orient the image first")
+                return orient.from_lps(res, code)
             return self.engine.apply_volume_float(0, vol, slot_fill=1 if fused else -1, postprocess=self.volume_postprocessing)
         if code == "LPS":
             if not fused:
@@ -201,11 +226,53 @@ class LMInferer:
         return self.engine.apply_volume_oriented(0, vol, perm, flip, slot_fill=1 if fused else -1,
                                                  postprocess=self.volume_postprocessing)
 
-    def apply_oriented(self, array: np.ndarray, direction) -> np.ndarray:
+    def _run_tensor(self, t, code: str = "LPS", with_probs: bool = False):
+        """A torch.Tensor volume (slices, H, W).  A CUDA tensor on the engine's device is segmented where it lies
+        (lm_apply_dev, ordered after the work queued on the current stream): the uint8 mask (and the float32 probabilities)
+        come back as tensors on that device.  A CPU tensor takes the numpy path and gets CPU tensors back."""
+        import torch
+        if t.dim() != 3:
+            raise ValueError("expected a (slices, H, W) volume, got shape %s" % (tuple(t.shape),))
+        dtype_code = _tensor_dtype_code(t)
+        if t.device.type not in ("cpu", "cuda"):
+            raise ValueError("the volume tensor is on %s: give a CPU tensor or a CUDA tensor on cuda:%d" % (t.device, self.engine.device))
+        t = t.detach()
+        if not t.is_cuda:
+            if t.dtype == torch.bfloat16:   # numpy has no bfloat16: widen here, with the warning of the float16 path
+                logger.warning("volume dtype %s is computed as float32", t.dtype)
+                t = t.float()
+            a = t.numpy()
+            if with_probs:
+                mask, probs = self._probabilities(a, code)
+                return torch.from_numpy(mask), torch.from_numpy(probs)
+            return torch.from_numpy(self._run(a, code))
+        if t.device.index != self.engine.device:
+            raise ValueError("the volume tensor is on %s, the engine on cuda:%d" % (t.device, self.engine.device))
+        if t.dtype in (torch.float16, torch.bfloat16):
+            logger.warning("volume dtype %s is computed as float32", t.dtype)
+        if not t.is_contiguous():
+            t = t.contiguous()
+        fused = self.fillmodel is not None
+        if fused:
+            self._log_fusion()
+        perm, flip = (None, None) if code == "LPS" else orient.array_transform_to_lps(code)
+        out = torch.empty(t.shape, dtype=torch.uint8, device=t.device)
+        probs = None
+        if with_probs:
+            probs = torch.empty((self.engine.n_classes[0],) + tuple(t.shape), dtype=torch.float32, device=t.device)
+        self.engine.apply_dev(0, t.data_ptr(), dtype_code, t.shape, out.data_ptr(), perm, flip, slot_fill=1 if fused else -1,
+                              d_probs_ptr=probs.data_ptr() if probs is not None else None,
+                              postprocess=self.volume_postprocessing, stream=torch.cuda.current_stream(t.device).cuda_stream)
+        return (out, probs) if with_probs else out
+
+    def apply_oriented(self, array, direction):
         """What `apply(sitk_image)` does, for callers without SimpleITK: `array` = sitk.GetArrayFromImage(image)
-        (axes z, y, x), `direction` = image.GetDirection() (9 direction cosines).  The mask comes back in the array's
-        own orientation (mask.py:157-164,204-208)."""
-        return self._run(array, orient.orientation_from_direction(direction))
+        (axes z, y, x) as a numpy array or a torch.Tensor, `direction` = image.GetDirection() (9 direction cosines).  The
+        mask comes back in the array's own orientation (mask.py:157-164,204-208), as a tensor for a tensor (see `apply`)."""
+        code = orient.orientation_from_direction(direction)
+        if _is_tensor(array):
+            return self._run_tensor(array, code)
+        return self._run(array, code)
 
     def _array_and_orientation(self, image, caller: str = "apply"):
         """(array (z, y, x), orientation code) of what `apply` accepts: a numpy array is taken as LPS; a
@@ -220,10 +287,23 @@ class LMInferer:
             raise TypeError("%s() expects a numpy array, a SimpleITK image or a lungmask_b200.io.Volume" % caller)
         return sitk.GetArrayFromImage(image), orient.orientation_from_direction(image.GetDirection())
 
-    def apply(self, image) -> np.ndarray:
+    def apply(self, image):
         """Segments a volume: numpy (slices, H, W), sitk.Image or lungmask_b200.io.Volume -> uint8 labels of the same shape
-        (lungmask/mask.py:212-232).  The input is not modified."""
+        (lungmask/mask.py:212-232).  The input is not modified.
+
+        A torch.Tensor (slices, H, W) is taken as LPS, like a numpy array.  A CUDA tensor on the engine's device never
+        leaves the GPU: the engine waits for the work queued on the current stream, reads the tensor in place (int16,
+        float32, float64) or converts it on the device (bool and other integers are clipped to [-1024, 600], float16 /
+        bfloat16 are widened to float32), and returns a uint8 tensor on that device, complete when the call returns.  A CPU
+        tensor gives what its numpy array gives, as a CPU tensor."""
+        if _is_tensor(image):
+            return self._run_tensor(image)
         return self._run(*self._array_and_orientation(image))
+
+    def _probabilities(self, array, code):
+        vol = _to_engine_volume(array)
+        perm, flip = (None, None) if code == "LPS" else orient.array_transform_to_lps(code)
+        return self.engine.apply_volume_probs(0, vol, perm, flip, postprocess=self.volume_postprocessing)
 
     def apply_with_probabilities(self, image):
         """The mask and the per-class probabilities of the model from one forward pass: image as for `apply` ->
@@ -235,14 +315,16 @@ class LMInferer:
         that the mask's order-0 resampling (utils.reshape_mask) puts at that voxel.  Voxels outside the slice's body
         crop box are background with probability 1.  The probabilities are the network's output BEFORE
         post-processing; with volume_postprocessing=False, their argmax is the mask.  Needs K * mask.size * 4 bytes on
-        the device and on the host.  Not defined for a fill model (the reference's fusion has no probabilities)."""
+        the device and on the host.  Not defined for a fill model (the reference's fusion has no probabilities).
+
+        For a CUDA tensor on the engine's device (see `apply`) both come back as tensors on that device, bit-identical to
+        the numpy results, with no copy to the host."""
         if self.fillmodel is not None:
             raise ValueError("apply_with_probabilities: the fusion with a fill model (%s) has no class probabilities; "
                              "use an LMInferer without fillmodel" % self.fillmodel)
-        array, code = self._array_and_orientation(image, "apply_with_probabilities")
-        vol = _to_engine_volume(array)
-        perm, flip = (None, None) if code == "LPS" else orient.array_transform_to_lps(code)
-        return self.engine.apply_volume_probs(0, vol, perm, flip, postprocess=self.volume_postprocessing)
+        if _is_tensor(image):
+            return self._run_tensor(image, with_probs=True)
+        return self._probabilities(*self._array_and_orientation(image, "apply_with_probabilities"))
 
 
 def apply(image, model=None, force_cpu=False, batch_size=20, volume_postprocessing=True, tqdm_disable=False):
