@@ -174,14 +174,18 @@ struct lm_engine {
   int range_slot = -1;      // the slot of the last forward (lm_debug_read_activation unscales with its scales)
   int range_retries = 0;
   Slot slots[LM_MAX_SLOTS];
-  DevBuf<int16_t> d_vol, d_resized, d_native;
+  // Whole-volume calls (run_volume): a host volume is uploaded to d_upload; volume_enqueue stages a volume that needs
+  // re-orientation or conversion into d_vol / d_fvol, keeps the LPS mask in d_lps_out and the fusion's two masks in
+  // d_native_l / d_native_r; a host call's results come back from d_out.
+  DevBuf<uint8_t> d_upload;   // the host volume in its native orientation, raw bytes of any dtype
+  DevBuf<int16_t> d_vol, d_resized;   // d_vol: the int16 LPS volume; also the upload of the stage taps and the sharded call
+  DevBuf<uint8_t> d_fvol;     // the float32 / float64 LPS volume, raw bytes; also the upload of lm_preprocess_float
   DevBuf<uint8_t> d_lps_out, d_native_l, d_native_r;
   DevBuf<int32_t> d_boxes;
-  DevBuf<uint8_t> d_labels, d_post, d_out, d_out2, d_fused, d_mask;
-  DevBuf<float> d_scores, d_norm;   // d_scores: one wave of lm_forward's tap, or a whole volume of lm_apply_volume_probs
-  DevBuf<float> d_probs;            // lm_apply_volume_probs: (K, n0, n1, n2) probabilities (lm_apply_dev writes the caller's)
-  DevBuf<uint8_t> d_fvol;   // float volumes (float32 / float64), raw bytes; also volume_enqueue's converted / LPS float volume
-  DevBuf<uint8_t> d_fnative;  // lm_apply_volume_probs: the uploaded float volume in its native orientation, raw bytes
+  // d_out: the mask of a host call, followed (lm_apply_volume_probs) by the (K, n0, n1, n2) probabilities at a 256-byte
+  // aligned offset.  d_out and d_out2 are also the work buffers of the stage taps and d_out the sharded call's result.
+  DevBuf<uint8_t> d_labels, d_post, d_out, d_out2, d_mask;
+  DevBuf<float> d_scores, d_norm;   // d_scores: one wave of lm_forward's tap, or a whole volume of scores for the probabilities
   DevBuf<uint32_t> d_scratch;
   PostScratch post;
   cudaEvent_t ev[8] = {};
@@ -411,30 +415,42 @@ int forward_all(lm_engine* e, int slot, const void* d_in, int S, uint8_t* d_labe
 // given by perm / flip (identity: the volume is LPS).
 struct ProbOut { float* scores; float* probs; int perm[3]; int flip[3]; };
 
-// preprocess -> forward -> postprocess -> reshape, all device-resident. d_out: (S,H,W) uint8.
+// ev[1]; bodymask + resize of S slices (S, H, W) into the network input d_resized / d_norm; ev[2]; the forward; ev[3].
 // vtype: 0 = int16 HU volume, 1 = float32, 2 = float64 (float volumes keep their dtype through the reference's
-// pre-processing and normalisation; preproc.cu resize_kernel)
-int inference_dev(lm_engine* e, int slot, const void* d_vol, int S, int H, int W, int flags, uint8_t* d_out, int vtype = 0,
-                  const ProbOut* prob = nullptr) {
-  float* const d_vol_scores = prob ? prob->scores : nullptr;
+// pre-processing and normalisation; preproc.cu resize_kernel).  boxes (S, 4), labels (S, 256, 256) and scores (nullptr,
+// or (S, K, 256, 256)) are the caller's.  S == 0 (a rank without slices): the events alone.
+int forward_head(lm_engine* e, int slot, const void* d_vol, int vtype, int S, int H, int W, int32_t* boxes, uint8_t* labels,
+                 float* scores) {
+  const size_t nr = (size_t)S * R * R;
+  if (S > 0) RC(vtype == 0 ? e->d_resized.reserve(nr) : e->d_norm.reserve(nr));
+  CU(cudaEventRecord(e->ev[1], e->st));
+  if (S > 0) {
+    if (vtype == 0) {
+      RC(launch_bodymask(static_cast<const int16_t*>(d_vol), S, H, W, boxes, nullptr, e->num_sms, e->st));
+      RC(launch_resize(static_cast<const int16_t*>(d_vol), S, H, W, boxes, e->d_resized.p, R, R, 1, e->num_sms, e->st));
+    } else {
+      RC(launch_bodymask_float(d_vol, vtype == 2, S, H, W, boxes, nullptr, e->num_sms, e->st));
+      RC(launch_resize_float(d_vol, vtype == 2, S, H, W, boxes, e->d_norm.p, R, R, e->num_sms, e->st));
+    }
+    e->launches += 2;
+  }
+  CU(cudaEventRecord(e->ev[2], e->st));
+  if (S > 0) {
+    const void* net_in = vtype == 0 ? static_cast<const void*>(e->d_resized.p) : e->d_norm.p;
+    RC(forward_all(e, slot, net_in, S, labels, nullptr, nullptr, vtype != 0, scores));
+  }
+  CU(cudaEventRecord(e->ev[3], e->st));
+  return 0;
+}
+
+// preprocess -> forward -> postprocess -> reshape of an LPS volume, all device-resident. d_out: (S,H,W) uint8.
+int inference_dev(lm_engine* e, int slot, const void* d_vol, int vtype, int S, int H, int W, int flags, uint8_t* d_out,
+                  const ProbOut* prob) {
   const size_t nr = (size_t)S * R * R;
   RC(e->d_boxes.reserve((size_t)S * 4));
-  if (vtype == 0) RC(e->d_resized.reserve(nr)); else RC(e->d_norm.reserve(nr));
   RC(e->d_labels.reserve(nr));
   RC(e->d_post.reserve(nr));
-  CU(cudaEventRecord(e->ev[1], e->st));
-  if (vtype == 0) {
-    RC(launch_bodymask(static_cast<const int16_t*>(d_vol), S, H, W, e->d_boxes.p, nullptr, e->num_sms, e->st));
-    RC(launch_resize(static_cast<const int16_t*>(d_vol), S, H, W, e->d_boxes.p, e->d_resized.p, R, R, 1, e->num_sms, e->st));
-  } else {
-    RC(launch_bodymask_float(d_vol, vtype == 2, S, H, W, e->d_boxes.p, nullptr, e->num_sms, e->st));
-    RC(launch_resize_float(d_vol, vtype == 2, S, H, W, e->d_boxes.p, e->d_norm.p, R, R, e->num_sms, e->st));
-  }
-  e->launches += 2;
-  CU(cudaEventRecord(e->ev[2], e->st));
-  if (vtype == 0) RC(forward_all(e, slot, e->d_resized.p, S, e->d_labels.p, nullptr, nullptr, false, d_vol_scores));
-  else RC(forward_all(e, slot, e->d_norm.p, S, e->d_labels.p, nullptr, nullptr, true, d_vol_scores));
-  CU(cudaEventRecord(e->ev[3], e->st));
+  RC(forward_head(e, slot, d_vol, vtype, S, H, W, e->d_boxes.p, e->d_labels.p, prob ? prob->scores : nullptr));
   const uint8_t* masks = e->d_labels.p;
   if (!(flags & LM_FLAG_NO_POSTPROCESS)) {
     // labels out of the argmax are < K: the post-processing needs no host round trip to learn which occur
@@ -535,16 +551,8 @@ int sharded_dev(lm_engine* e, int slot, const int16_t* d_vol, int S, int H, int 
   int32_t* boxes_full = reinterpret_cast<int32_t*>(v.block[v.rank] + shard_boxes_offset());
   const uint32_t epoch = ++e->shard_epoch;
   const int ns = hi - lo;
-  CU(cudaEventRecord(e->ev[1], e->st));
-  if (ns > 0) {
-    RC(e->d_resized.reserve((size_t)ns * rr));
-    RC(launch_bodymask(d_vol + (size_t)lo * plane, ns, H, W, boxes_full + 4 * (size_t)lo, nullptr, e->num_sms, e->st));
-    RC(launch_resize(d_vol + (size_t)lo * plane, ns, H, W, boxes_full + 4 * (size_t)lo, e->d_resized.p, R, R, 1, e->num_sms, e->st));
-    e->launches += 2;
-  }
-  CU(cudaEventRecord(e->ev[2], e->st));
-  if (ns > 0) RC(forward_all(e, slot, e->d_resized.p, ns, labels_full + (size_t)lo * rr, nullptr, nullptr));
-  CU(cudaEventRecord(e->ev[3], e->st));
+  RC(forward_head(e, slot, d_vol + (size_t)lo * plane, 0, ns, H, W, boxes_full + 4 * (size_t)lo, labels_full + (size_t)lo * rr,
+                  nullptr));
   // slab-sharded 3-D labelling (SURVEY 8f-1): this rank labels its own slices (26-connected, neighbours outside the slab
   // ignored) and ships the union-find parents with the labels; after the gather every rank only links the slab
   // boundaries and flattens
@@ -659,8 +667,8 @@ size_t dtype_bytes(int dtype) {
 }
 
 // One volume of LMInferer._inference / LMInferer.apply on device memory: the volume in its native orientation in, the
-// mask (and the probabilities) in that orientation out.  lm_apply_dev runs it on the caller's pointers,
-// lm_apply_volume_oriented and lm_apply_volume_probs on the engine buffers they upload to.
+// mask (and the probabilities) in that orientation out.  Every whole-volume entry point runs one through run_volume,
+// the _dev ones on the caller's pointers, the host ones on the engine buffers run_volume copies through.
 struct VolumeJob {
   int slot, slot_fill;   // slot_fill >= 0: the fusion of mask.py:223-232
   const void* d_vol;     // (n0,n1,n2), element type `dtype` (LM_DTYPE_*); never written
@@ -696,7 +704,7 @@ int volume_enqueue(lm_engine* e, const VolumeJob& j) {
       RC(e->d_scores.reserve((size_t)dl[0] * e->slots[j.slot].K * R * R));
       po.scores = e->d_scores.p;
     }
-    RC(inference_dev(e, j.slot, d_lps_in, dl[0], dl[1], dl[2], j.flags, lps ? j.d_out : e->d_lps_out.p, vtype,
+    RC(inference_dev(e, j.slot, d_lps_in, vtype, dl[0], dl[1], dl[2], j.flags, lps ? j.d_out : e->d_lps_out.p,
                      j.d_probs ? &po : nullptr));
     if (!lps) {   // the mask back to the native orientation, mask.py:204-208
       RC(launch_orient_u8(e->d_lps_out.p, j.d_out, dl, pm, fl, 0, e->num_sms, e->st));
@@ -713,7 +721,7 @@ int volume_enqueue(lm_engine* e, const VolumeJob& j) {
   const int slots[2] = {j.slot, j.slot_fill};
   uint8_t* const res[2] = {e->d_native_l.p, e->d_native_r.p};   // res_l, res_r (mask.py:225,227)
   for (int m = 0; m < 2; ++m) {
-    RC(inference_dev(e, slots[m], d_lps_in, dl[0], dl[1], dl[2], inner, lps ? res[m] : e->d_lps_out.p, vtype));
+    RC(inference_dev(e, slots[m], d_lps_in, vtype, dl[0], dl[1], dl[2], inner, lps ? res[m] : e->d_lps_out.p, nullptr));
     if (!lps) {
       RC(launch_orient_u8(e->d_lps_out.p, res[m], dl, pm, fl, 0, e->num_sms, e->st));
       e->launches++;
@@ -724,6 +732,55 @@ int volume_enqueue(lm_engine* e, const VolumeJob& j) {
   // labels after the fusion are <= K_base (the spare value is max + 1 <= K_base): mask.py:232
   RC(postprocess_device(e->post, res[0], j.dn[0], j.dn[1], j.dn[2], nullptr, 0, e->d_spare, 1, 3, e->slots[j.slot].K, j.d_out,
                         e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+// The argument checks of the whole-volume entry points, with fn's name in the messages: -1 for a NULL pointer (ptrs_ok
+// false) or an empty volume, -30 for a weight slot that is not loaded.  slot_fill < 0 means "no fill model", unless
+// fill_required (lm_apply_fused*): there it is an unloaded slot as well.
+int check_volume_call(const lm_engine* e, const char* fn, bool ptrs_ok, int n0, int n1, int n2, int slot, int slot_fill,
+                      bool fill_required = false) {
+  if (!e || !ptrs_ok) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "%s: weight slot %d not loaded", fn, slot);
+  if ((slot_fill >= 0 || fill_required) && (slot_fill < 0 || slot_fill >= LM_MAX_SLOTS || !e->slots[slot_fill].loaded))
+    return fail(-30, "%s: weight slot %d not loaded", fn, slot_fill);
+  return 0;
+}
+
+// Runs one VolumeJob as a whole call: volume_enqueue between ev[0] and ev[6] under run_checked, then the timings.
+//   h_vol    NULL (j.d_vol is device memory), or a host volume of j.dtype: uploaded to d_upload, which becomes j.d_vol.
+//   h_out    NULL (j.d_out is device memory), or the host mask: copied back from d_out, which becomes j.d_out.
+//   h_probs  NULL, or the host (K, n0, n1, n2) probabilities (needs h_out): copied back from d_out behind the mask.
+//   caller   NULL, or the caller's stream: the engine stream waits for the work queued on it (lm_apply_dev).
+int run_volume(lm_engine* e, VolumeJob j, const void* h_vol, uint8_t* h_out, float* h_probs, const cudaStream_t* caller = nullptr) {
+  CU(cudaSetDevice(e->device));
+  const size_t n = (size_t)j.dn[0] * j.dn[1] * j.dn[2], in_bytes = n * dtype_bytes(j.dtype);
+  const size_t probs_at = (n + 255) & ~(size_t)255;
+  const size_t probs_bytes = h_probs ? (size_t)e->slots[j.slot].K * n * sizeof(float) : 0;
+  if (h_vol) {
+    RC(e->d_upload.reserve(in_bytes));
+    j.d_vol = e->d_upload.p;
+  }
+  if (h_out) {
+    RC(e->d_out.reserve(h_probs ? probs_at + probs_bytes : n));
+    j.d_out = e->d_out.p;
+    if (h_probs) j.d_probs = reinterpret_cast<float*>(e->d_out.p + probs_at);
+  }
+  if (caller) CU(cudaEventRecord(e->ev_in, *caller));
+  RC(run_checked(e, [&]() -> int {
+    e->launches = 0;
+    e->ev_used = 0;
+    CU(cudaEventRecord(e->ev[0], e->st));
+    if (caller) CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
+    if (h_vol) CU(cudaMemcpyAsync(e->d_upload.p, h_vol, in_bytes, cudaMemcpyHostToDevice, e->st));
+    RC(volume_enqueue(e, j));
+    if (h_out) CU(cudaMemcpyAsync(h_out, j.d_out, n, cudaMemcpyDeviceToHost, e->st));
+    if (h_probs) CU(cudaMemcpyAsync(h_probs, j.d_probs, probs_bytes, cudaMemcpyDeviceToHost, e->st));
+    CU(cudaEventRecord(e->ev[6], e->st));
+    return 0;
+  }));
+  collect_timings(e);
   return 0;
 }
 
@@ -813,10 +870,10 @@ void lm_destroy(lm_engine* e) {
     cudaFree(s.stem_w); cudaFree(s.stem_bias); cudaFree(s.stem_scale); cudaFree(s.stem_shift); cudaFree(s.head_w); cudaFree(s.head_b);
     for (auto& l : s.lw) { cudaFree(l.w); cudaFree(l.bias); cudaFree(l.scale); cudaFree(l.shift); }
   }
-  e->d_norm.release(); e->d_fvol.release(); e->d_fnative.release(); e->d_probs.release();
-  e->d_native.release(); e->d_lps_out.release(); e->d_native_l.release(); e->d_native_r.release();
+  e->d_norm.release(); e->d_fvol.release(); e->d_upload.release();
+  e->d_lps_out.release(); e->d_native_l.release(); e->d_native_r.release();
   e->d_vol.release(); e->d_resized.release(); e->d_boxes.release(); e->d_labels.release(); e->d_post.release();
-  e->d_out.release(); e->d_out2.release(); e->d_fused.release(); e->d_mask.release(); e->d_scores.release(); e->d_scratch.release();
+  e->d_out.release(); e->d_out2.release(); e->d_mask.release(); e->d_scores.release(); e->d_scratch.release();
   e->post.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
@@ -918,129 +975,35 @@ int lm_load_weights(lm_engine* e, int slot, const float* blob, size_t n_floats, 
 }
 
 int lm_apply_volume_dev(lm_engine* e, int slot, const int16_t* d_vol, int S, int H, int W, int flags, uint8_t* d_out) {
-  if (!e || !d_vol || !d_out) return fail(-1, "lm_apply_volume_dev: NULL argument");
-  if (S < 1 || H < 1 || W < 1) return fail(-1, "lm_apply_volume_dev: empty volume (%d,%d,%d)", S, H, W);
-  CU(cudaSetDevice(e->device));
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    RC(inference_dev(e, slot, d_vol, S, H, W, flags, d_out));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  RC(check_volume_call(e, "lm_apply_volume_dev", d_vol && d_out, S, H, W, slot, -1));
+  return run_volume(e, {slot, -1, d_vol, LM_DTYPE_I16, flags, {S, H, W}, {0, 1, 2}, {0, 0, 0}, d_out, nullptr}, nullptr, nullptr,
+                    nullptr);
 }
 
 int lm_apply_volume(lm_engine* e, int slot, const int16_t* vol, int S, int H, int W, int flags, uint8_t* out) {
-  if (!e || !vol || !out) return fail(-1, "lm_apply_volume: NULL argument");
-  if (S < 1 || H < 1 || W < 1) return fail(-1, "lm_apply_volume: empty volume (%d,%d,%d)", S, H, W);
-  CU(cudaSetDevice(e->device));
-  const size_t n = (size_t)S * H * W;
-  RC(e->d_vol.reserve(n));
-  RC(e->d_out.reserve(n));
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaMemcpyAsync(e->d_vol.p, vol, n * sizeof(int16_t), cudaMemcpyHostToDevice, e->st));
-    RC(inference_dev(e, slot, e->d_vol.p, S, H, W, flags, e->d_out.p));
-    CU(cudaMemcpyAsync(out, e->d_out.p, n, cudaMemcpyDeviceToHost, e->st));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
-}
-
-// LMInferer.apply with a fill model on a device-resident volume: res_l / res_r in engine buffers, result to d_final
-static int fused_enqueue(lm_engine* e, int slot_base, int slot_fill, const void* d_vol, int S, int H, int W, int flags,
-                         uint8_t* d_final, int vtype = 0) {
-  // both inner inferences honour volume_postprocessing (mask.py:191-194); the fusion post-processing below does not
-  const int inner = flags & LM_FLAG_NO_POSTPROCESS;
-  const size_t n = (size_t)S * H * W;
-  RC(inference_dev(e, slot_base, d_vol, S, H, W, inner, e->d_out.p, vtype));   // res_l (mask.py:225)
-  RC(inference_dev(e, slot_fill, d_vol, S, H, W, inner, e->d_out2.p, vtype));  // res_r (mask.py:227)
-  RC(fuse_device(e->d_out.p, e->d_out2.p, n, e->d_scratch.p, e->d_spare, e->num_sms, e->st));  // spare stays on the device
-  e->launches += 3;
-  // labels after the fusion are <= K_base (the spare value is max + 1 <= K_base): mask.py:232
-  RC(postprocess_device(e->post, e->d_out.p, S, H, W, nullptr, 0, e->d_spare, 1, 3, e->slots[slot_base].K, d_final, e->num_sms, e->st,
-                        &e->launches));
-  return 0;
+  RC(check_volume_call(e, "lm_apply_volume", vol && out, S, H, W, slot, -1));
+  return run_volume(e, {slot, -1, nullptr, LM_DTYPE_I16, flags, {S, H, W}, {0, 1, 2}, {0, 0, 0}, nullptr, nullptr}, vol, out,
+                    nullptr);
 }
 
 int lm_apply_fused(lm_engine* e, int slot_base, int slot_fill, const int16_t* vol, int S, int H, int W, int flags, uint8_t* out) {
-  if (!e || !vol || !out) return fail(-1, "lm_apply_fused: NULL argument");
-  if (S < 1 || H < 1 || W < 1) return fail(-1, "lm_apply_fused: empty volume");
-  if (slot_base < 0 || slot_base >= LM_MAX_SLOTS || !e->slots[slot_base].loaded) return fail(-30, "weight slot %d not loaded", slot_base);
-  CU(cudaSetDevice(e->device));
-  const size_t n = (size_t)S * H * W;
-  RC(e->d_vol.reserve(n));
-  RC(e->d_out.reserve(n));
-  RC(e->d_out2.reserve(n));
-  RC(e->d_fused.reserve(n));
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaMemcpyAsync(e->d_vol.p, vol, n * sizeof(int16_t), cudaMemcpyHostToDevice, e->st));
-    RC(fused_enqueue(e, slot_base, slot_fill, e->d_vol.p, S, H, W, flags, e->d_fused.p));
-    CU(cudaMemcpyAsync(out, e->d_fused.p, n, cudaMemcpyDeviceToHost, e->st));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  RC(check_volume_call(e, "lm_apply_fused", vol && out, S, H, W, slot_base, slot_fill, true));
+  return run_volume(e, {slot_base, slot_fill, nullptr, LM_DTYPE_I16, flags, {S, H, W}, {0, 1, 2}, {0, 0, 0}, nullptr, nullptr},
+                    vol, out, nullptr);
 }
 
 int lm_apply_fused_dev(lm_engine* e, int slot_base, int slot_fill, const int16_t* d_vol, int S, int H, int W, int flags, uint8_t* d_out) {
-  if (!e || !d_vol || !d_out) return fail(-1, "lm_apply_fused_dev: NULL argument");
-  if (S < 1 || H < 1 || W < 1) return fail(-1, "lm_apply_fused_dev: empty volume");
-  if (slot_base < 0 || slot_base >= LM_MAX_SLOTS || !e->slots[slot_base].loaded) return fail(-30, "weight slot %d not loaded", slot_base);
-  CU(cudaSetDevice(e->device));
-  const size_t n = (size_t)S * H * W;
-  RC(e->d_out.reserve(n));
-  RC(e->d_out2.reserve(n));
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    RC(fused_enqueue(e, slot_base, slot_fill, d_vol, S, H, W, flags, d_out));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  RC(check_volume_call(e, "lm_apply_fused_dev", d_vol && d_out, S, H, W, slot_base, slot_fill, true));
+  return run_volume(e, {slot_base, slot_fill, d_vol, LM_DTYPE_I16, flags, {S, H, W}, {0, 1, 2}, {0, 0, 0}, d_out, nullptr},
+                    nullptr, nullptr, nullptr);
 }
 
 int lm_apply_volume_float(lm_engine* e, int slot, int slot_fill, const void* vol, int is_f64, int S, int H, int W, int flags,
                           uint8_t* out) {
-  if (!e || !vol || !out) return fail(-1, "lm_apply_volume_float: NULL argument");
-  if (S < 1 || H < 1 || W < 1) return fail(-1, "lm_apply_volume_float: empty volume");
-  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
-  const bool fused = slot_fill >= 0;
-  if (fused && (slot_fill >= LM_MAX_SLOTS || !e->slots[slot_fill].loaded)) return fail(-30, "weight slot %d not loaded", slot_fill);
-  CU(cudaSetDevice(e->device));
-  const size_t n = (size_t)S * H * W, esz = is_f64 ? 8 : 4;
-  RC(e->d_fvol.reserve(n * esz));
-  RC(e->d_out.reserve(n));
-  if (fused) { RC(e->d_out2.reserve(n)); RC(e->d_fused.reserve(n)); }
-  const int vtype = is_f64 ? 2 : 1;
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaMemcpyAsync(e->d_fvol.p, vol, n * esz, cudaMemcpyHostToDevice, e->st));
-    const uint8_t* result = e->d_out.p;
-    if (fused) { RC(fused_enqueue(e, slot, slot_fill, e->d_fvol.p, S, H, W, flags, e->d_fused.p, vtype)); result = e->d_fused.p; }
-    else RC(inference_dev(e, slot, e->d_fvol.p, S, H, W, flags, e->d_out.p, vtype));
-    CU(cudaMemcpyAsync(out, result, n, cudaMemcpyDeviceToHost, e->st));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  RC(check_volume_call(e, "lm_apply_volume_float", vol && out, S, H, W, slot, slot_fill));
+  const int dtype = is_f64 ? LM_DTYPE_F64 : LM_DTYPE_F32;
+  return run_volume(e, {slot, slot_fill, nullptr, dtype, flags, {S, H, W}, {0, 1, 2}, {0, 0, 0}, nullptr, nullptr}, vol, out,
+                    nullptr);
 }
 
 int lm_preprocess_float(lm_engine* e, const void* vol, int is_f64, int S, int H, int W, float* normalised, int32_t* boxes) {
@@ -1062,100 +1025,37 @@ int lm_preprocess_float(lm_engine* e, const void* vol, int is_f64, int S, int H,
 
 int lm_apply_volume_oriented(lm_engine* e, int slot, int slot_fill, const int16_t* vol, int n0, int n1, int n2, const int* perm,
                              const int* flip, int flags, uint8_t* out) {
-  if (!e || !vol || !out || !perm || !flip) return fail(-1, "lm_apply_volume_oriented: NULL argument");
-  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_volume_oriented: empty volume");
-  int pm[3], fl[3];
-  RC(parse_orientation("lm_apply_volume_oriented", perm, flip, pm, fl));
-  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
-  const bool fused = slot_fill >= 0;
-  if (fused && (slot_fill >= LM_MAX_SLOTS || !e->slots[slot_fill].loaded)) return fail(-30, "weight slot %d not loaded", slot_fill);
-  CU(cudaSetDevice(e->device));
-  const size_t n = (size_t)n0 * n1 * n2;
-  RC(e->d_native.reserve(n));
-  RC(e->d_out.reserve(n));
-  const VolumeJob job{slot, fused ? slot_fill : -1, e->d_native.p, LM_DTYPE_I16, flags, {n0, n1, n2},
-                      {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]}, e->d_out.p, nullptr};
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaMemcpyAsync(e->d_native.p, vol, n * sizeof(int16_t), cudaMemcpyHostToDevice, e->st));
-    RC(volume_enqueue(e, job));
-    CU(cudaMemcpyAsync(out, e->d_out.p, n, cudaMemcpyDeviceToHost, e->st));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  RC(check_volume_call(e, "lm_apply_volume_oriented", vol && out && perm && flip, n0, n1, n2, slot, slot_fill));
+  VolumeJob j{slot, slot_fill, nullptr, LM_DTYPE_I16, flags, {n0, n1, n2}, {}, {}, nullptr, nullptr};
+  RC(parse_orientation("lm_apply_volume_oriented", perm, flip, j.perm, j.flip));
+  return run_volume(e, j, vol, out, nullptr);
 }
 
 int lm_apply_volume_probs(lm_engine* e, int slot, const void* vol, int dtype, int n0, int n1, int n2, const int* perm,
                           const int* flip, int flags, uint8_t* out, float* probs) {
-  if (!e || !vol || !out || !probs) return fail(-1, "lm_apply_volume_probs: NULL argument");
-  if ((perm == nullptr) != (flip == nullptr)) return fail(-1, "lm_apply_volume_probs: perm and flip must both be given or both be NULL");
-  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_volume_probs: empty volume");
+  RC(check_volume_call(e, "lm_apply_volume_probs", vol && out && probs, n0, n1, n2, slot, -1));
   if (dtype != LM_DTYPE_I16 && dtype != LM_DTYPE_F32 && dtype != LM_DTYPE_F64)
     return fail(-1, "lm_apply_volume_probs: dtype %d is not LM_DTYPE_I16, LM_DTYPE_F32 or LM_DTYPE_F64", dtype);
-  int pm[3], fl[3];
-  RC(parse_orientation("lm_apply_volume_probs", perm, flip, pm, fl));
-  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
-  CU(cudaSetDevice(e->device));
-  const int K = e->slots[slot].K;
-  const size_t n = (size_t)n0 * n1 * n2, esz = dtype_bytes(dtype);
-  void* d_native_in = nullptr;  // the upload target: the volume in its native orientation
-  if (dtype == LM_DTYPE_I16) { RC(e->d_native.reserve(n)); d_native_in = e->d_native.p; }
-  else { RC(e->d_fnative.reserve(n * esz)); d_native_in = e->d_fnative.p; }
-  RC(e->d_out.reserve(n));
-  RC(e->d_probs.reserve((size_t)K * n));
-  const VolumeJob job{slot, -1, d_native_in, dtype, flags, {n0, n1, n2}, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]},
-                      e->d_out.p, e->d_probs.p};
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaMemcpyAsync(d_native_in, vol, n * esz, cudaMemcpyHostToDevice, e->st));
-    RC(volume_enqueue(e, job));
-    CU(cudaMemcpyAsync(out, e->d_out.p, n, cudaMemcpyDeviceToHost, e->st));
-    CU(cudaMemcpyAsync(probs, e->d_probs.p, (size_t)K * n * sizeof(float), cudaMemcpyDeviceToHost, e->st));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  VolumeJob j{slot, -1, nullptr, dtype, flags, {n0, n1, n2}, {}, {}, nullptr, nullptr};
+  RC(parse_orientation("lm_apply_volume_probs", perm, flip, j.perm, j.flip));
+  return run_volume(e, j, vol, out, probs);
 }
 
 int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol, int dtype, int n0, int n1, int n2, const int* perm,
                  const int* flip, int flags, uint8_t* d_out, float* d_probs, void* stream) {
-  if (!e || !d_vol || !d_out) return fail(-1, "lm_apply_dev: NULL argument");
-  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "lm_apply_dev: empty volume (%d,%d,%d)", n0, n1, n2);
+  RC(check_volume_call(e, "lm_apply_dev", d_vol && d_out, n0, n1, n2, slot, slot_fill));
   if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "lm_apply_dev: unknown dtype code %d", dtype);
-  int pm[3], fl[3];
-  RC(parse_orientation("lm_apply_dev", perm, flip, pm, fl));
-  if (slot < 0 || slot >= LM_MAX_SLOTS || !e->slots[slot].loaded) return fail(-30, "weight slot %d not loaded", slot);
-  const bool fused = slot_fill >= 0;
-  if (fused && d_probs)
+  VolumeJob j{slot, slot_fill, d_vol, dtype, flags, {n0, n1, n2}, {}, {}, d_out, d_probs};
+  RC(parse_orientation("lm_apply_dev", perm, flip, j.perm, j.flip));
+  if (slot_fill >= 0 && d_probs)
     return fail(-1, "lm_apply_dev: no probabilities for the fusion with a fill model (slot_fill %d): the reference's fusion "
                     "defines none", slot_fill);
-  if (fused && (slot_fill >= LM_MAX_SLOTS || !e->slots[slot_fill].loaded)) return fail(-30, "weight slot %d not loaded", slot_fill);
   CU(cudaSetDevice(e->device));
   RC(check_device_ptr(e, "lm_apply_dev", "d_vol", d_vol));
   RC(check_device_ptr(e, "lm_apply_dev", "d_out", d_out));
   if (d_probs) RC(check_device_ptr(e, "lm_apply_dev", "d_probs", d_probs));
-  const VolumeJob job{slot, fused ? slot_fill : -1, d_vol, dtype, flags, {n0, n1, n2}, {pm[0], pm[1], pm[2]}, {fl[0], fl[1], fl[2]},
-                      d_out, d_probs};
-  // the engine stream (non-blocking) is ordered after everything the caller queued on its stream so far
-  CU(cudaEventRecord(e->ev_in, static_cast<cudaStream_t>(stream)));
-  RC(run_checked(e, [&]() -> int {
-    e->launches = 0;
-    e->ev_used = 0;
-    CU(cudaEventRecord(e->ev[0], e->st));
-    CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
-    RC(volume_enqueue(e, job));
-    CU(cudaEventRecord(e->ev[6], e->st));
-    return 0;
-  }));
-  collect_timings(e);
-  return 0;
+  const cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  return run_volume(e, j, nullptr, nullptr, nullptr, &caller);
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

@@ -516,14 +516,6 @@ static int launch_stem_t(const IT* in, void* out, const float* w, const float* b
   return (int)cudaGetLastError();
 }
 
-int launch_stem(const int16_t* in, void* out, const float* w, const float* bias, const float* scale,
-                const float* shift, int N, int H, int W, int* range_flag, float out_scale, int num_sms, cudaStream_t stream) {
-  return launch_stem_t<int16_t>(in, out, w, bias, scale, shift, N, H, W, range_flag, out_scale, 0, num_sms, stream);
-}
-int launch_stem_v2(const int16_t* in, void* out, const float* w, const float* bias, const float* scale,
-                   const float* shift, int N, int H, int W, int* range_flag, float out_scale, int num_sms, cudaStream_t stream) {
-  return launch_stem_t<int16_t>(in, out, w, bias, scale, shift, N, H, W, range_flag, out_scale, 1, num_sms, stream);
-}
 int launch_stem_any(const int16_t* in, void* out, const float* w, const float* bias, const float* scale, const float* shift, int N, int H,
                     int W, int* range_flag, float out_scale, int version, int num_sms, cudaStream_t stream) {
   return launch_stem_t<int16_t>(in, out, w, bias, scale, shift, N, H, W, range_flag, out_scale, version, num_sms, stream);

@@ -7,12 +7,8 @@
 namespace lm {
 // resized HU slices int16 [N][H][W] -> split planes [N][2][H][W][64]
 // (range_flag: device int set to 1 when a value leaves the operand format's range; may be nullptr)
-int launch_stem(const int16_t* in, void* out, const float* w, const float* bias, const float* scale,
-                const float* shift, int N, int H, int W, int* range_flag, float out_scale, int num_sms, cudaStream_t stream);
-// same result from a different work assignment (weights in registers, 4-pixel quads); opt-in, see forward_misc.cu
-int launch_stem_v2(const int16_t* in, void* out, const float* w, const float* bias, const float* scale,
-                   const float* shift, int N, int H, int W, int* range_flag, float out_scale, int num_sms, cudaStream_t stream);
-// version: 0 = stem_kernel, 1 = stem_kernel_v2, 2 = stem_kernel_v3 (shared input tile + shared weights; the default)
+// version: 0 = stem_kernel, 1 = stem_kernel_v2 (weights in registers, 4-pixel quads), 2 = stem_kernel_v3 (shared input
+// tile + shared weights), 3 = stem_kernel_v3 with the next tile's samples fetched ahead (the default)
 int launch_stem_any(const int16_t* in, void* out, const float* w, const float* bias, const float* scale, const float* shift, int N, int H,
                     int W, int* range_flag, float out_scale, int version, int num_sms, cudaStream_t stream);
 // the same convolution on an already normalised fp32 input [N][H][W] (float volumes, preproc.cuh launch_resize_float)

@@ -422,20 +422,9 @@ int launch_orient_convert(const void* src, int dtype, void* dst, const int dims_
     default: return -1;
   }
 }
-int launch_orient_i16(const int16_t* src, int16_t* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
-                      int num_sms, cudaStream_t stream) {
-  return launch_orient_t<int16_t>(src, dst, dims_lps, perm, flip, to_lps, num_sms, stream);
-}
 int launch_orient_u8(const uint8_t* src, uint8_t* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
                      int num_sms, cudaStream_t stream) {
   return launch_orient_t<uint8_t>(src, dst, dims_lps, perm, flip, to_lps, num_sms, stream);
-}
-int launch_orient_float(const void* src, void* dst, int is_f64, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
-                        int num_sms, cudaStream_t stream) {
-  return is_f64 ? launch_orient_t<double>(static_cast<const double*>(src), static_cast<double*>(dst), dims_lps, perm, flip, to_lps,
-                                          num_sms, stream)
-                : launch_orient_t<float>(static_cast<const float*>(src), static_cast<float*>(dst), dims_lps, perm, flip, to_lps,
-                                         num_sms, stream);
 }
 
 int preproc_smem_bytes() { return (int)sizeof(Smem); }

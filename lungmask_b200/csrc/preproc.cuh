@@ -20,13 +20,8 @@ int launch_resize_float(const void* vol, int is_f64, int S, int H, int W, const 
                         int num_sms, cudaStream_t stream);
 // Native orientation <-> LPS (axis permutation + flips, see preproc.cu orient_kernel): dims_lps = shape of the LPS array,
 // lps = transpose(native, perm) flipped along every axis k with flip[k].  to_lps = 1: native -> LPS; 0: LPS -> native.
-int launch_orient_i16(const int16_t* src, int16_t* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
-                      int num_sms, cudaStream_t stream);
 int launch_orient_u8(const uint8_t* src, uint8_t* dst, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
                      int num_sms, cudaStream_t stream);
-// The same for float volumes: float64 with is_f64 != 0, else float32.
-int launch_orient_float(const void* src, void* dst, int is_f64, const int dims_lps[3], const int perm[3], const int flip[3], int to_lps,
-                        int num_sms, cudaStream_t stream);
 // Native -> LPS in one pass with the element conversion of lm_apply_dev: src of element type `dtype` (LM_DTYPE_*);
 // dst int16 for LM_DTYPE_I16 and the integer codes (clipped to [-1024, 600] unless already int16), float32 for
 // LM_DTYPE_F32 / F16 / BF16, float64 for LM_DTYPE_F64.  Returns -1 for an unknown code.
