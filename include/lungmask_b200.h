@@ -151,6 +151,31 @@ LM_API int lm_apply_volume_probs(lm_engine* e, int slot, const void* vol, int dt
 LM_API int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol, int dtype, int n0, int n1, int n2,
                         const int* perm, const int* flip, int flags, uint8_t* d_out, float* d_probs, void* stream);
 
+/* Per-label volume and HU statistics of a volume and its label mask (no counterpart in the reference; DESIGN §4.6): what
+ * lung-CT tools report from a lungmask result - each lung's or lobe's voxel count, mean / std / min / max HU, percentiles
+ * (Perc15) and the fraction of voxels below thresholds (LAA-950).
+ *   vol      (n0,n1,n2) of element type `dtype` (every LM_DTYPE_* code; bool as LM_DTYPE_U8).  Values are read as they
+ *            are: not clipped; float16 / bfloat16 are widened to float32, every value statistic is computed in float64.
+ *   mask     (n0,n1,n2) uint8, voxel i paired with voxel i of vol (orientation does not matter).
+ *   percentiles  n_q values q in [0, 100]; thresholds  n_t integers t in [-1024, 3072].
+ * Results: 257 rows, row l = the voxels with mask == l (row 0: voxels only), row 256 = the union mask > 0.  NaN values
+ * are counted in nan_voxels and excluded from everything else; n = voxels - nan_voxels.
+ *   voxels [257], nan_voxels [257]   int64 counts
+ *   moments [257][4]       mean, std (population), min, max of the row's values; NaN when n = 0
+ *   percentile [257][n_q]  bit-identical to numpy.percentile(values.astype(float64), q) (method "linear"); NaN when n = 0
+ *   below_count [257][n_t] count(value < t); 0 when n = 0
+ * lm_label_stats takes host arrays (uploaded into engine buffers); lm_label_stats_dev takes device memory of the engine's
+ * device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev.  Both return after the engine's stream
+ * has synchronised; the inputs are never written. */
+#define LM_STATS_MAX_PERCENTILES 64
+#define LM_STATS_MAX_THRESHOLDS 4097
+LM_API int lm_label_stats(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2,
+                          const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
+                          int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count);
+LM_API int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                              const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
+                              int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

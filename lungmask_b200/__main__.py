@@ -2,13 +2,15 @@
 
 Inputs are read by lungmask_b200/io.py (DICOM series directory, NIfTI, MetaImage, .npy - no SimpleITK needed); the
 mask is written with the input's geometry as .nii / .nii.gz / .mha / .npy.  `--probabilities PATH` also writes the
-model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_with_probabilities).
+model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_with_probabilities), and `--statistics PATH`
+the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950).
 """
 import argparse
 import os
 import sys
 
-from .io import check_probabilities_path, load_input_image, save_mask, save_probabilities
+from .io import (check_probabilities_path, check_statistics_path, load_input_image, save_mask, save_probabilities,
+                 save_statistics)
 from .logger import logger
 from .mask import LMInferer
 
@@ -37,6 +39,9 @@ def build_parser():
     p.add_argument("--probabilities", metavar="PATH", type=str, default=None,
                    help="Also write the model's per-class probabilities (before post-processing) with the mask's geometry: "
                         ".npy, or a 4-D .nii / .nii.gz with the classes as 4th dimension. Not for LTRCLobes_R231")
+    p.add_argument("--statistics", metavar="PATH", type=str, default=None,
+                   help="Also write per-label volume (mL) and HU statistics of the input under the mask - mean, std, min, "
+                        "max, Perc15 and LAA-950 - for every label and the whole lung: .json or .csv")
     return p
 
 
@@ -46,6 +51,8 @@ def main(argv=None):
         if args.modelname == "LTRCLobes_R231":
             sys.exit("--probabilities: the LTRCLobes_R231 fusion has no class probabilities; use LTRCLobes or R231")
         check_probabilities_path(args.probabilities)
+    if args.statistics is not None:
+        check_statistics_path(args.statistics)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -68,6 +75,9 @@ def main(argv=None):
     if probs is not None:
         logger.info(f"Save probabilities to: {args.probabilities}")
         save_probabilities(args.probabilities, probs, image)
+    if args.statistics is not None:
+        logger.info(f"Save statistics to: {args.statistics}")
+        save_statistics(args.statistics, inferer.statistics(image, result))
 
 
 if __name__ == "__main__":

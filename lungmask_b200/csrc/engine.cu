@@ -16,6 +16,7 @@
 #include "postproc.cuh"
 #include "preproc.cuh"
 #include "shard.cuh"
+#include "stats.cuh"
 
 using namespace lm;
 
@@ -188,6 +189,7 @@ struct lm_engine {
   DevBuf<float> d_scores, d_norm;   // d_scores: one wave of lm_forward's tap, or a whole volume of scores for the probabilities
   DevBuf<uint32_t> d_scratch;
   PostScratch post;
+  LabelStatsWork stats;   // lm_label_stats*: counts, histograms and selection state (a host call's volume and mask go to d_upload)
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -784,6 +786,41 @@ int run_volume(lm_engine* e, VolumeJob j, const void* h_vol, uint8_t* h_out, flo
   return 0;
 }
 
+// lm_label_stats / lm_label_stats_dev: every argument is checked before any kernel runs.  h_vol / h_mask NULL: d_vol /
+// d_mask are the caller's device memory (and `caller` its stream); otherwise both are uploaded into d_upload.
+int label_stats_call(lm_engine* e, const char* fn, const void* vol, int dtype, const uint8_t* mask, bool host, int n0, int n1,
+                     int n2, const double* q, int n_q, const int* t, int n_t, int64_t* voxels, int64_t* nan_voxels,
+                     double* moments, double* percentile, int64_t* below, const cudaStream_t* caller) {
+  if (!e || !vol || !mask || !voxels || !nan_voxels || !moments || (n_q > 0 && (!q || !percentile)) || (n_t > 0 && (!t || !below)))
+    return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (n_q < 0 || n_q > LM_STATS_MAX_PERCENTILES) return fail(-1, "%s: n_q %d not in [0,%d]", fn, n_q, LM_STATS_MAX_PERCENTILES);
+  if (n_t < 0 || n_t > LM_STATS_MAX_THRESHOLDS) return fail(-1, "%s: n_t %d not in [0,%d]", fn, n_t, LM_STATS_MAX_THRESHOLDS);
+  for (int k = 0; k < n_q; ++k)
+    if (!(q[k] >= 0.0 && q[k] <= 100.0)) return fail(-1, "%s: percentile %g not in [0,100]", fn, q[k]);
+  for (int k = 0; k < n_t; ++k)
+    if (t[k] < -1024 || t[k] > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, t[k]);
+  CU(cudaSetDevice(e->device));
+  const size_t n = (size_t)n0 * n1 * n2, vol_bytes = n * dtype_bytes(dtype), mask_at = (vol_bytes + 255) & ~(size_t)255;
+  if (host) {
+    RC(e->d_upload.reserve(mask_at + n));
+    CU(cudaMemcpyAsync(e->d_upload.p, vol, vol_bytes, cudaMemcpyHostToDevice, e->st));
+    CU(cudaMemcpyAsync(e->d_upload.p + mask_at, mask, n, cudaMemcpyHostToDevice, e->st));
+    vol = e->d_upload.p;
+    mask = e->d_upload.p + mask_at;
+  } else {
+    RC(check_device_ptr(e, fn, "d_vol", vol));
+    RC(check_device_ptr(e, fn, "d_mask", mask));
+    CU(cudaEventRecord(e->ev_in, *caller));
+    CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
+  }
+  e->launches = 0;
+  const LabelStatsOut out{voxels, nan_voxels, moments, percentile, below};
+  RC(label_stats(e->stats, vol, dtype, mask, n, q, n_q, t, n_t, out, e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -875,6 +912,7 @@ void lm_destroy(lm_engine* e) {
   e->d_vol.release(); e->d_resized.release(); e->d_boxes.release(); e->d_labels.release(); e->d_post.release();
   e->d_out.release(); e->d_out2.release(); e->d_mask.release(); e->d_scores.release(); e->d_scratch.release();
   e->post.release();
+  e->stats.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1056,6 +1094,21 @@ int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol, int d
   if (d_probs) RC(check_device_ptr(e, "lm_apply_dev", "d_probs", d_probs));
   const cudaStream_t caller = static_cast<cudaStream_t>(stream);
   return run_volume(e, j, nullptr, nullptr, nullptr, &caller);
+}
+
+int lm_label_stats(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2,
+                   const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels, int64_t* nan_voxels,
+                   double* moments, double* percentile, int64_t* below_count) {
+  return label_stats_call(e, "lm_label_stats", vol, dtype, mask, true, n0, n1, n2, percentiles, n_q, thresholds, n_t, voxels,
+                          nan_voxels, moments, percentile, below_count, nullptr);
+}
+
+int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                       const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
+                       int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count, void* stream) {
+  const cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  return label_stats_call(e, "lm_label_stats_dev", d_vol, dtype, d_mask, false, n0, n1, n2, percentiles, n_q, thresholds, n_t,
+                          voxels, nan_voxels, moments, percentile, below_count, &caller);
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

@@ -405,3 +405,40 @@ def save_probabilities(path, probs, like=None):
         np.save(path, probs)
     else:
         _write_nifti(path, probs, like)
+
+
+def check_statistics_path(path):
+    """Refuses, before any work is done, an output path save_statistics cannot write."""
+    if not path.lower().endswith((".json", ".csv")):
+        raise SystemExit("unsupported statistics output format (use .json or .csv): %s" % path)
+
+
+def _csv_cell(v):
+    if v is None:
+        return ""
+    if isinstance(v, float):
+        return repr(v)
+    s = str(v)
+    return '"%s"' % s.replace('"', '""') if any(c in s for c in ',"\n') else s
+
+
+def save_statistics(path, stats):
+    """Writes the LabelStatistics of LMInferer.statistics: .json (spacing, percentiles, thresholds and one object per row,
+    NaN as null) or .csv (a header, then one line per row: label, name, voxels, nan_voxels, volume_ml, mean_hu, std_hu,
+    min_hu, max_hu, percentile_<q>..., fraction_below_<t>...; an unknown volume is an empty cell, NaN is "nan")."""
+    check_statistics_path(path)
+    if path.lower().endswith(".json"):
+        import json
+        with open(path, "w") as f:
+            json.dump(stats.to_dict(), f, indent=1, allow_nan=False)
+            f.write("\n")
+        return
+    base = ["label", "name", "voxels", "nan_voxels", "volume_ml", "mean_hu", "std_hu", "min_hu", "max_hu"]
+    header = base + ["percentile_%g" % q for q in stats.percentiles] + ["fraction_below_%d" % t for t in stats.thresholds]
+    lines = [",".join(header)]
+    for r in stats.rows:
+        cells = [getattr(r, k) for k in base] + [r.percentile_hu[q] for q in stats.percentiles] + \
+                [r.fraction_below[t] for t in stats.thresholds]
+        lines.append(",".join(_csv_cell(v) for v in cells))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")

@@ -326,6 +326,71 @@ class LMInferer:
             return self._run_tensor(image, with_probs=True)
         return self._probabilities(*self._array_and_orientation(image, "apply_with_probabilities"))
 
+    def statistics(self, image, mask, spacing=None, percentiles=(15.0,), thresholds=(-950,)):
+        """Per-label volume and HU statistics of `image` under `mask` (e.g. the mask `apply(image)` returned) ->
+        lungmask_b200.statistics.LabelStatistics: a row for every label value in the mask and every label 1..K-1 of the
+        model (absent ones with 0 voxels), then "lung", the union of all labels.  Each row holds the voxel count, the
+        volume in mL (when a spacing is known), the NaN count, mean / std / min / max HU, numpy.percentile of the values
+        for each of `percentiles` (bit-identical) and the fraction of the values below each integer HU of `thresholds`.
+        The defaults are Perc15 and LAA-950.
+
+        `image`: what `apply` accepts, with `mask` (uint8 or bool) of the same shape in the same array orientation; the
+        values are taken as they are (not clipped).  A Volume or SimpleITK image supplies its spacing (x, y, z) in mm
+        unless `spacing` is given.  A CUDA tensor with a CUDA mask tensor on the engine's device is read in place, ordered
+        after the work queued on the current stream; numpy arrays and CPU tensors are uploaded.  Both inputs are left
+        unchanged."""
+        from . import statistics as st
+        q, t = st.check_arguments(percentiles, thresholds)
+        if _is_tensor(image) and image.is_cuda or _is_tensor(mask) and mask.is_cuda:
+            res = self._statistics_tensor(image, mask, q, t)
+        else:
+            if _is_tensor(image):
+                image = image.detach()
+                image = (image.float() if str(image.dtype) == "torch.bfloat16" else image).numpy()
+            if _is_tensor(mask):
+                mask = mask.detach().numpy()
+            if isinstance(image, np.ndarray):
+                array = image
+            else:
+                array, _ = self._array_and_orientation(image, "statistics")
+                if spacing is None:
+                    spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
+            array, mask = np.asarray(array), np.asarray(mask)
+            self._check_statistics_inputs(array.shape, mask.shape, mask.dtype == np.uint8 or mask.dtype == bool, mask.dtype)
+            res = self.engine.label_stats(array, mask, q, t)
+        if spacing is not None:
+            spacing = tuple(float(s) for s in spacing)
+            if len(spacing) != 3:
+                raise ValueError("spacing must be (x, y, z), got %s" % (spacing,))
+        labels = set(np.nonzero(res["voxels"][1:256])[0] + 1) | set(range(1, self.engine.n_classes[0]))
+        return st.from_native(res, labels, self.modelname, spacing, q, t)
+
+    @staticmethod
+    def _check_statistics_inputs(shape, mask_shape, mask_ok, mask_dtype):
+        if len(shape) != 3:
+            raise ValueError("statistics: expected a (slices, H, W) volume, got shape %s" % (tuple(shape),))
+        if not mask_ok:
+            raise TypeError("statistics: the mask must be uint8 or bool, got %s" % mask_dtype)
+        if tuple(mask_shape) != tuple(shape):
+            raise ValueError("statistics: the mask's shape %s differs from the volume's %s" % (tuple(mask_shape), tuple(shape)))
+
+    def _statistics_tensor(self, image, mask, q, t):
+        import torch
+        if not (_is_tensor(image) and _is_tensor(mask) and image.is_cuda and mask.is_cuda):
+            raise ValueError("statistics: a CUDA tensor needs a CUDA tensor as partner (volume on %s, mask on %s)"
+                             % (getattr(image, "device", "host"), getattr(mask, "device", "host")))
+        for what, x in (("volume", image), ("mask", mask)):
+            if x.device.index != self.engine.device:
+                raise ValueError("statistics: the %s tensor is on %s, the engine on cuda:%d" % (what, x.device, self.engine.device))
+        self._check_statistics_inputs(image.shape, mask.shape, mask.dtype in (torch.uint8, torch.bool), mask.dtype)
+        code = _tensor_dtype_code(image)
+        image = image.detach().contiguous()
+        mask = mask.detach().contiguous()
+        if mask.dtype == torch.bool:
+            mask = mask.view(torch.uint8)
+        return self.engine.label_stats_dev(image.data_ptr(), code, mask.data_ptr(), image.shape, q, t,
+                                           stream=torch.cuda.current_stream(image.device).cuda_stream)
+
 
 def apply(image, model=None, force_cpu=False, batch_size=20, volume_postprocessing=True, tqdm_disable=False):
     """Deprecated wrapper (lungmask/mask.py:235-255)."""
