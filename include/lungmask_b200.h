@@ -176,6 +176,29 @@ LM_API int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const 
                               const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
                               int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count, void* stream);
 
+/* Size distributions of the connected clusters of low-attenuation (LAA) voxels per label (no counterpart in the reference;
+ * DESIGN §4.7): whether a lobe's LAA-950 is many small holes or a few large bullae (the power-law exponent D of
+ * Mishima et al., PNAS 1999, is computed from these pairs by LMInferer.laa_clusters).
+ *   vol, mask     as lm_label_stats; a voxel is LAA when mask > 0 and value < threshold, compared in the volume's type
+ *                 (integers unclipped, float16 / bfloat16 widened to float32; NaN is never LAA).
+ *   threshold     integer HU in [-1024, 3072];  connectivity  4 (faces within a slice, per-slice 2-D clusters), 6 (faces)
+ *                 or 26 (full).  Fewer than 2^32 voxels.
+ * Results: 257 rows.  Row l (1..255): the components of the LAA voxels with mask == l (a cluster never crosses a label
+ * boundary); row 256: the components of all LAA voxels (a cluster may span labels); row 0 is all zero.
+ *   laa_voxels [257], n_clusters [257]  int64
+ *   n_pairs [257]       the number of distinct cluster sizes of the row
+ *   sizes, counts       the (size, count) pairs, ascending by size within a row, rows concatenated in row order
+ *                       (sum of n_pairs entries).  max_pairs >= lm_laa_max_pairs(n0*n1*n2), which bounds that sum
+ *                       (a row of V LAA voxels has at most sqrt(2V) distinct sizes, the rows hold at most 2n voxels).
+ * lm_laa_clusters takes host arrays, lm_laa_clusters_dev device memory and the caller's stream, as lm_label_stats*. */
+LM_API size_t lm_laa_max_pairs(size_t n_voxels);   /* 32 * ceil(sqrt(n_voxels)) + 256 */
+LM_API int lm_laa_clusters(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2, int threshold,
+                           int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs, int64_t* sizes,
+                           int64_t* counts, size_t max_pairs);
+LM_API int lm_laa_clusters_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                               int threshold, int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs,
+                               int64_t* sizes, int64_t* counts, size_t max_pairs, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -3,14 +3,16 @@
 Inputs are read by lungmask_b200/io.py (DICOM series directory, NIfTI, MetaImage, .npy - no SimpleITK needed); the
 mask is written with the input's geometry as .nii / .nii.gz / .mha / .npy.  `--probabilities PATH` also writes the
 model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_with_probabilities), and `--statistics PATH`
-the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950).
+the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950),
+and `--clusters PATH` the size distributions of the low-attenuation clusters with their exponent D (.json / .csv,
+LMInferer.laa_clusters).
 """
 import argparse
 import os
 import sys
 
-from .io import (check_probabilities_path, check_statistics_path, load_input_image, save_mask, save_probabilities,
-                 save_statistics)
+from .io import (check_clusters_path, check_probabilities_path, check_statistics_path, load_input_image, save_clusters,
+                 save_mask, save_probabilities, save_statistics)
 from .logger import logger
 from .mask import LMInferer
 
@@ -42,6 +44,14 @@ def build_parser():
     p.add_argument("--statistics", metavar="PATH", type=str, default=None,
                    help="Also write per-label volume (mL) and HU statistics of the input under the mask - mean, std, min, "
                         "max, Perc15 and LAA-950 - for every label and the whole lung: .json or .csv")
+    p.add_argument("--clusters", metavar="PATH", type=str, default=None,
+                   help="Also write the size distributions of the connected clusters of low-attenuation voxels (below "
+                        "--clusters-threshold HU) for every label and the whole lung, with the power-law exponent D: "
+                        ".json (with the (size, count) pairs) or .csv (the summary)")
+    p.add_argument("--clusters-threshold", metavar="HU", type=int, default=-950,
+                   help="Low-attenuation threshold of --clusters, an integer HU in [-1024, 3072] (default -950)")
+    p.add_argument("--clusters-connectivity", type=int, choices=[4, 6, 26], default=6,
+                   help="Cluster connectivity of --clusters: 6 faces (default), 26 full, 4 faces within a slice")
     return p
 
 
@@ -53,6 +63,13 @@ def main(argv=None):
         check_probabilities_path(args.probabilities)
     if args.statistics is not None:
         check_statistics_path(args.statistics)
+    if args.clusters is not None:
+        check_clusters_path(args.clusters)
+        from .clusters import check_arguments
+        try:
+            check_arguments(args.clusters_threshold, args.clusters_connectivity, 1)
+        except ValueError as ex:
+            sys.exit("--clusters-threshold: %s" % ex)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -78,6 +95,10 @@ def main(argv=None):
     if args.statistics is not None:
         logger.info(f"Save statistics to: {args.statistics}")
         save_statistics(args.statistics, inferer.statistics(image, result))
+    if args.clusters is not None:
+        logger.info(f"Save clusters to: {args.clusters}")
+        save_clusters(args.clusters, inferer.laa_clusters(image, result, threshold=args.clusters_threshold,
+                                                          connectivity=args.clusters_connectivity))
 
 
 if __name__ == "__main__":

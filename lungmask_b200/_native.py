@@ -54,6 +54,9 @@ def lib():
         "lm_apply_dev": ([vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, i32, u8p, f32p, vp], i32),
         "lm_label_stats": ([vp, vp, i32, u8p, i32, i32, i32, vp, i32, vp, i32, vp, vp, vp, vp, vp], i32),
         "lm_label_stats_dev": ([vp, vp, i32, u8p, i32, i32, i32, vp, i32, vp, i32, vp, vp, vp, vp, vp, vp], i32),
+        "lm_laa_max_pairs": ([C.c_size_t], C.c_size_t),
+        "lm_laa_clusters": ([vp, vp, i32, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t], i32),
+        "lm_laa_clusters_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -83,7 +86,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats", "lm_label_stats_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters", "lm_laa_clusters_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -120,6 +123,24 @@ def _as(a, dtype, ndim=None):
     if ndim is not None and a.ndim != ndim:
         raise ValueError("expected %d-d array, got shape %s" % (ndim, a.shape))
     return a
+
+
+def _host_pair(vol, mask, fn):
+    """The (volume, LM_DTYPE_* code, mask) of a per-label call on host arrays: C-contiguous, bool viewed as uint8,
+    uint16 / uint32 volumes widened to int32 / int64 without loss."""
+    vol = np.asarray(vol)
+    if vol.dtype in (np.uint16, np.uint32):
+        vol = vol.astype(np.int32 if vol.dtype == np.uint16 else np.int64)
+    if vol.dtype not in _HOST_DTYPE_CODES:
+        raise TypeError("%s: volume dtype %s is not supported" % (fn, vol.dtype))
+    code = _HOST_DTYPE_CODES[vol.dtype]
+    vol = np.ascontiguousarray(vol.view(np.uint8) if vol.dtype == bool else vol)
+    mask = np.ascontiguousarray(np.asarray(mask).view(np.uint8) if np.asarray(mask).dtype == bool else mask)
+    if mask.dtype != np.uint8:
+        raise TypeError("%s: the mask must be uint8 or bool, got %s" % (fn, mask.dtype))
+    if vol.ndim != 3 or mask.shape != vol.shape:
+        raise ValueError("%s: expected (S,H,W) volume and mask of one shape, got %s and %s" % (fn, vol.shape, mask.shape))
+    return vol, code, mask
 
 
 class Engine:
@@ -264,18 +285,7 @@ class Engine:
         """lm_label_stats on host arrays: `vol` (S,H,W) of any dtype with an LM_DTYPE_* code (bool, uint8, int8, int16,
         int32, int64, float16, float32, float64; uint16 / uint32 are widened to int32 / int64 without loss), `mask` (S,H,W)
         uint8 or bool.  -> dict of the 257-row arrays (see label_stats_dev)."""
-        vol = np.asarray(vol)
-        if vol.dtype in (np.uint16, np.uint32):
-            vol = vol.astype(np.int32 if vol.dtype == np.uint16 else np.int64)
-        if vol.dtype not in _HOST_DTYPE_CODES:
-            raise TypeError("label_stats: volume dtype %s is not supported" % vol.dtype)
-        code = _HOST_DTYPE_CODES[vol.dtype]
-        vol = np.ascontiguousarray(vol.view(np.uint8) if vol.dtype == bool else vol)
-        mask = np.ascontiguousarray(np.asarray(mask).view(np.uint8) if np.asarray(mask).dtype == bool else mask)
-        if mask.dtype != np.uint8:
-            raise TypeError("label_stats: the mask must be uint8 or bool, got %s" % mask.dtype)
-        if vol.ndim != 3 or mask.shape != vol.shape:
-            raise ValueError("label_stats: expected (S,H,W) volume and mask of one shape, got %s and %s" % (vol.shape, mask.shape))
+        vol, code, mask = _host_pair(vol, mask, "label_stats")
         return self._label_stats(lambda *a: lib().lm_label_stats(self._h, _ptr(vol), code, _ptr(mask), *vol.shape, *a),
                                  percentiles, thresholds)
 
@@ -300,6 +310,35 @@ class Engine:
                     _ptr(res["percentile"]), _ptr(res["below_count"])))
         res["percentile"] = res["percentile"][:, :q.size]
         res["below_count"] = res["below_count"][:, :t.size]
+        return res
+
+    # ---- LAA cluster size distributions (lm_laa_clusters*)
+    def laa_clusters(self, vol, mask, threshold=-950, connectivity=6):
+        """lm_laa_clusters on host arrays (`vol` and `mask` as for label_stats) -> dict (see laa_clusters_dev)."""
+        vol, code, mask = _host_pair(vol, mask, "laa_clusters")
+        return self._laa_clusters(lambda *a: lib().lm_laa_clusters(self._h, _ptr(vol), code, _ptr(mask), *vol.shape, *a),
+                                  vol.size, threshold, connectivity)
+
+    def laa_clusters_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, threshold=-950, connectivity=6, stream=0):
+        """lm_laa_clusters_dev on device memory of this engine's device (`stream` as for apply_dev) -> dict over 257 rows
+        (row l = label l, row 256 = all LAA voxels): "laa_voxels", "n_clusters", "n_pairs" (int64 [257]) and "sizes",
+        "counts" (int64, the rows' (size, count) pairs concatenated; row r's are [offsets[r], offsets[r + 1])), "offsets"."""
+        n0, n1, n2 = (int(x) for x in shape)
+        return self._laa_clusters(lambda *a: lib().lm_laa_clusters_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code),
+                                                                       C.c_void_p(d_mask_ptr), n0, n1, n2, *a,
+                                                                       C.c_void_p(int(stream)) if stream else None),
+                                  max(n0, 0) * max(n1, 0) * max(n2, 0), threshold, connectivity)
+
+    @staticmethod
+    def _laa_clusters(call, n_voxels, threshold, connectivity):
+        cap = int(lib().lm_laa_max_pairs(n_voxels))
+        res = {k: np.zeros(257, np.int64) for k in ("laa_voxels", "n_clusters", "n_pairs")}
+        sizes, counts = np.zeros(cap, np.int64), np.zeros(cap, np.int64)
+        _check(call(int(threshold), int(connectivity), _ptr(res["laa_voxels"]), _ptr(res["n_clusters"]), _ptr(res["n_pairs"]),
+                    _ptr(sizes), _ptr(counts), cap))
+        res["offsets"] = np.concatenate([[0], np.cumsum(res["n_pairs"])])
+        total = int(res["offsets"][-1])
+        res["sizes"], res["counts"] = sizes[:total].copy(), counts[:total].copy()
         return res
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)

@@ -17,6 +17,7 @@
 #include "preproc.cuh"
 #include "shard.cuh"
 #include "stats.cuh"
+#include "clusters.cuh"
 
 using namespace lm;
 
@@ -190,6 +191,7 @@ struct lm_engine {
   DevBuf<uint32_t> d_scratch;
   PostScratch post;
   LabelStatsWork stats;   // lm_label_stats*: counts, histograms and selection state (a host call's volume and mask go to d_upload)
+  ClusterWork clusters;   // lm_laa_clusters*: LAA maps, union-find parents, cluster sizes, size histogram (inputs as for stats)
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -786,8 +788,30 @@ int run_volume(lm_engine* e, VolumeJob j, const void* h_vol, uint8_t* h_out, flo
   return 0;
 }
 
-// lm_label_stats / lm_label_stats_dev: every argument is checked before any kernel runs.  h_vol / h_mask NULL: d_vol /
-// d_mask are the caller's device memory (and `caller` its stream); otherwise both are uploaded into d_upload.
+// The (volume, mask) pair of a per-label call on the engine's stream.  host: *vol and *mask are host arrays, uploaded into
+// d_upload (the pointers then point there); otherwise they are the caller's device memory, checked, and the engine's
+// stream waits for the work queued on *caller.
+int volume_mask_inputs(lm_engine* e, const char* fn, const void** vol, int dtype, const uint8_t** mask, bool host, size_t n,
+                       const cudaStream_t* caller) {
+  CU(cudaSetDevice(e->device));
+  const size_t vol_bytes = n * dtype_bytes(dtype), mask_at = (vol_bytes + 255) & ~(size_t)255;
+  if (host) {
+    RC(e->d_upload.reserve(mask_at + n));
+    CU(cudaMemcpyAsync(e->d_upload.p, *vol, vol_bytes, cudaMemcpyHostToDevice, e->st));
+    CU(cudaMemcpyAsync(e->d_upload.p + mask_at, *mask, n, cudaMemcpyHostToDevice, e->st));
+    *vol = e->d_upload.p;
+    *mask = e->d_upload.p + mask_at;
+  } else {
+    RC(check_device_ptr(e, fn, "d_vol", *vol));
+    RC(check_device_ptr(e, fn, "d_mask", *mask));
+    CU(cudaEventRecord(e->ev_in, *caller));
+    CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
+  }
+  return 0;
+}
+
+// lm_label_stats / lm_label_stats_dev: every argument is checked before any kernel runs.  host false: vol / mask are the
+// caller's device memory (and `caller` its stream); otherwise both are uploaded into d_upload.
 int label_stats_call(lm_engine* e, const char* fn, const void* vol, int dtype, const uint8_t* mask, bool host, int n0, int n1,
                      int n2, const double* q, int n_q, const int* t, int n_t, int64_t* voxels, int64_t* nan_voxels,
                      double* moments, double* percentile, int64_t* below, const cudaStream_t* caller) {
@@ -801,23 +825,32 @@ int label_stats_call(lm_engine* e, const char* fn, const void* vol, int dtype, c
     if (!(q[k] >= 0.0 && q[k] <= 100.0)) return fail(-1, "%s: percentile %g not in [0,100]", fn, q[k]);
   for (int k = 0; k < n_t; ++k)
     if (t[k] < -1024 || t[k] > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, t[k]);
-  CU(cudaSetDevice(e->device));
-  const size_t n = (size_t)n0 * n1 * n2, vol_bytes = n * dtype_bytes(dtype), mask_at = (vol_bytes + 255) & ~(size_t)255;
-  if (host) {
-    RC(e->d_upload.reserve(mask_at + n));
-    CU(cudaMemcpyAsync(e->d_upload.p, vol, vol_bytes, cudaMemcpyHostToDevice, e->st));
-    CU(cudaMemcpyAsync(e->d_upload.p + mask_at, mask, n, cudaMemcpyHostToDevice, e->st));
-    vol = e->d_upload.p;
-    mask = e->d_upload.p + mask_at;
-  } else {
-    RC(check_device_ptr(e, fn, "d_vol", vol));
-    RC(check_device_ptr(e, fn, "d_mask", mask));
-    CU(cudaEventRecord(e->ev_in, *caller));
-    CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
-  }
+  const size_t n = (size_t)n0 * n1 * n2;
+  RC(volume_mask_inputs(e, fn, &vol, dtype, &mask, host, n, caller));
   e->launches = 0;
   const LabelStatsOut out{voxels, nan_voxels, moments, percentile, below};
   RC(label_stats(e->stats, vol, dtype, mask, n, q, n_q, t, n_t, out, e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+// lm_laa_clusters / lm_laa_clusters_dev: every argument is checked before any kernel runs; the inputs as label_stats_call.
+int laa_clusters_call(lm_engine* e, const char* fn, const void* vol, int dtype, const uint8_t* mask, bool host, int n0, int n1,
+                      int n2, int threshold, int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs,
+                      int64_t* sizes, int64_t* counts, size_t max_pairs, const cudaStream_t* caller) {
+  if (!e || !vol || !mask || !laa_voxels || !n_clusters || !n_pairs || !sizes || !counts) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the labelling takes fewer than 2^32", fn, n);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (threshold < -1024 || threshold > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, threshold);
+  if (connectivity != 4 && connectivity != 6 && connectivity != 26)
+    return fail(-1, "%s: connectivity %d is not 4, 6 or 26", fn, connectivity);
+  if (max_pairs < laa_max_pairs(n))
+    return fail(-1, "%s: max_pairs %zu below lm_laa_max_pairs(%zu) = %zu", fn, max_pairs, n, laa_max_pairs(n));
+  RC(volume_mask_inputs(e, fn, &vol, dtype, &mask, host, n, caller));
+  e->launches = 0;
+  const LaaClustersOut out{laa_voxels, n_clusters, n_pairs, sizes, counts, max_pairs};
+  RC(laa_clusters(e->clusters, vol, dtype, mask, n0, n1, n2, threshold, connectivity, out, e->num_sms, e->st, &e->launches));
   return 0;
 }
 
@@ -913,6 +946,7 @@ void lm_destroy(lm_engine* e) {
   e->d_out.release(); e->d_out2.release(); e->d_mask.release(); e->d_scores.release(); e->d_scratch.release();
   e->post.release();
   e->stats.release();
+  e->clusters.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1109,6 +1143,23 @@ int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t
   const cudaStream_t caller = static_cast<cudaStream_t>(stream);
   return label_stats_call(e, "lm_label_stats_dev", d_vol, dtype, d_mask, false, n0, n1, n2, percentiles, n_q, thresholds, n_t,
                           voxels, nan_voxels, moments, percentile, below_count, &caller);
+}
+
+size_t lm_laa_max_pairs(size_t n_voxels) { return laa_max_pairs(n_voxels); }
+
+int lm_laa_clusters(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2, int threshold,
+                    int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs, int64_t* sizes, int64_t* counts,
+                    size_t max_pairs) {
+  return laa_clusters_call(e, "lm_laa_clusters", vol, dtype, mask, true, n0, n1, n2, threshold, connectivity, laa_voxels, n_clusters,
+                           n_pairs, sizes, counts, max_pairs, nullptr);
+}
+
+int lm_laa_clusters_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2, int threshold,
+                        int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs, int64_t* sizes,
+                        int64_t* counts, size_t max_pairs, void* stream) {
+  const cudaStream_t caller = static_cast<cudaStream_t>(stream);
+  return laa_clusters_call(e, "lm_laa_clusters_dev", d_vol, dtype, d_mask, false, n0, n1, n2, threshold, connectivity, laa_voxels,
+                           n_clusters, n_pairs, sizes, counts, max_pairs, &caller);
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

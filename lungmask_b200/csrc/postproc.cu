@@ -1162,6 +1162,19 @@ int ccl_slab_device(const uint8_t* d_labels, uint32_t* d_parent, int S, int H, i
   return (int)cudaGetLastError();
 }
 
+int ccl_volume_device(const uint8_t* d_vals, uint32_t* d_parent, int S, int H, int W, int conn, int num_sms, cudaStream_t st,
+                      int64_t* launches) {
+  const Dim d{S, H, W};
+  const BoxSrc full = fixed_box(Box{0, S, 0, H, 0, W});
+  const size_t n = (size_t)S * H * W;
+  switch (conn) {
+    case 4: return run_ccl<4>(d_vals, d_parent, d, full, n, num_sms, st, launches);
+    case 6: return run_ccl<6>(d_vals, d_parent, d, full, n, num_sms, st, launches);
+    case 26: return run_ccl<26>(d_vals, d_parent, d, full, n, num_sms, st, launches);
+    default: return -1;
+  }
+}
+
 int ccl_join_slabs_device(const uint8_t* d_labels, uint32_t* d_parent, int S, int H, int W, const int* first_slices, int n_bounds,
                           int num_sms, cudaStream_t st, int64_t* launches) {
   const Dim d{S, H, W};

@@ -23,13 +23,13 @@
 #include <vector>
 
 #include "../../include/lungmask_b200.h"
+#include "mask_chunk.cuh"
 #include "stats.cuh"
 
 namespace lm {
 namespace {
 
 constexpr int kThreads = 512;
-constexpr int kChunk = 16;          // voxels per thread and step: one 16-byte mask vector
 constexpr int kSmemSlots = 12;      // labels whose histograms are privatised in shared memory: 12 x 4098 x 4 B = 192 KB
 constexpr int kSmemTargets = 96;    // selection targets whose digit histograms fit shared memory: 96 x 256 x 4 B = 96 KB
 constexpr int kMaxSlots = 255;      // labels 1..255
@@ -107,21 +107,6 @@ template <typename T> __device__ __forceinline__ int bin_of(T x) {
     const double d = to_f64(x);
     return d < -1024.0 ? 0 : (d >= 3072.0 ? kStatsBins - 1 : (int)floor(d) + 1025);
   }
-}
-
-// The 16 labels of a chunk as one vector (a 16-byte load where the mask allows it; 0 past the end).
-__device__ __forceinline__ uint4 load_labels(const uint8_t* __restrict__ m, size_t base, size_t n) {
-  if (base + kChunk <= n && (reinterpret_cast<uintptr_t>(m) & 15) == 0) return __ldg(reinterpret_cast<const uint4*>(m + base));
-  unsigned w[4] = {0, 0, 0, 0};
-#pragma unroll
-  for (int k = 0; k < kChunk; ++k)
-    if (base + k < n) w[k >> 2] |= (unsigned)m[base + k] << (8 * (k & 3));
-  return make_uint4(w[0], w[1], w[2], w[3]);
-}
-// Label k of the chunk, with selects rather than an indexed array (no local memory when the loop is not unrolled).
-__device__ __forceinline__ int label_at(const uint4& u, int k) {
-  const unsigned w = k < 8 ? (k < 4 ? u.x : u.y) : (k < 12 ? u.z : u.w);
-  return (int)((w >> (8 * (k & 3))) & 255u);
 }
 
 // 128-bit modular add from two 64-bit atomics: the carry of the low word goes into the high word, so the sum is exact

@@ -442,3 +442,29 @@ def save_statistics(path, stats):
         lines.append(",".join(_csv_cell(v) for v in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")
+
+
+def check_clusters_path(path):
+    """Refuses, before any work is done, an output path save_clusters cannot write."""
+    if not path.lower().endswith((".json", ".csv")):
+        raise SystemExit("unsupported clusters output format (use .json or .csv): %s" % path)
+
+
+def save_clusters(path, clusters):
+    """Writes the LaaClusters of LMInferer.laa_clusters: .json (spacing, threshold, connectivity, min_cluster_voxels and
+    one object per row with its sizes / counts pairs, NaN as null) or .csv (a header, then one summary line per row:
+    label, name, laa_voxels, laa_volume_ml, clusters, largest_voxels, largest_ml, d; an unknown volume is an empty cell,
+    NaN is "nan")."""
+    check_clusters_path(path)
+    if path.lower().endswith(".json"):
+        import json
+        with open(path, "w") as f:
+            json.dump(clusters.to_dict(), f, indent=1, allow_nan=False)
+            f.write("\n")
+        return
+    from .clusters import ClusterRow
+    lines = [",".join(ClusterRow.SUMMARY)]
+    for r in clusters.rows:
+        lines.append(",".join(_csv_cell(getattr(r, k)) for k in ClusterRow.SUMMARY))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")

@@ -341,8 +341,62 @@ class LMInferer:
         unchanged."""
         from . import statistics as st
         q, t = st.check_arguments(percentiles, thresholds)
+        res, spacing = self._per_label_call(
+            "statistics", image, mask, spacing, lambda vol, m: self.engine.label_stats(vol, m, q, t),
+            lambda v, code, m, stream: self.engine.label_stats_dev(v.data_ptr(), code, m.data_ptr(), v.shape, q, t,
+                                                                   stream=stream))
+        labels = set(np.nonzero(res["voxels"][1:256])[0] + 1) | set(range(1, self.engine.n_classes[0]))
+        return st.from_native(res, labels, self.modelname, spacing, q, t)
+
+    def laa_clusters(self, image, mask, threshold=-950, connectivity=6, spacing=None, min_cluster_voxels=1):
+        """Size distributions of the connected clusters of low-attenuation voxels (mask > 0 and value < `threshold` HU)
+        per label and for the whole lung -> lungmask_b200.clusters.LaaClusters, with the rows of `statistics`: every
+        label value in the mask and every label 1..K-1 of the model, then "lung".  A label's clusters never cross its
+        boundary; the "lung" row labels all LAA voxels together, so a cluster there may span two lobes.
+
+        Each row holds the LAA voxel count and volume (mL, when a spacing is known), the number of clusters, the largest
+        cluster (voxels and mL), the exact distribution as `sizes` / `counts` arrays (ascending sizes, int64), and D,
+        the exponent of the power law of the cumulative size distribution (Mishima et al., PNAS 1999): minus the
+        least-squares slope of log10 Y(s) on log10 s, one point per distinct size s >= `min_cluster_voxels`, Y(s) = the
+        number of clusters of s voxels or more; NaN with fewer than two points.  That is one convention among several
+        (binning, size cut-offs, fit ranges differ between studies); the raw pairs are there for the others.
+
+        `connectivity`: 6 (faces, scipy.ndimage.label's default), 26 (full, as the post-processing) or 4 (faces within a
+        slice: per-slice 2-D clusters as in the original 2-D analysis).  `threshold`: an integer HU in [-1024, 3072],
+        compared in the volume's dtype (not clipped; NaN is never LAA).  `image`, `mask` and `spacing` as for
+        `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the spacing), CPU tensors, or CUDA tensors
+        on the engine's device read in place after the work queued on the current stream."""
+        from . import clusters as cl
+        threshold, connectivity, min_cluster_voxels = cl.check_arguments(threshold, connectivity, min_cluster_voxels)
+        import torch
+        device = torch.device("cuda", self.engine.device)
+
+        def host_call(vol, m):
+            res = self.engine.laa_clusters(vol, m, threshold, connectivity)
+            m = torch.from_numpy(np.ascontiguousarray(m).view(np.uint8)).to(device)
+            return dict(res, labels=self._mask_labels(m, torch.cuda.current_stream(device).cuda_stream))
+
+        def dev_call(v, code, m, stream):
+            res = self.engine.laa_clusters_dev(v.data_ptr(), code, m.data_ptr(), v.shape, threshold, connectivity, stream=stream)
+            return dict(res, labels=self._mask_labels(m, stream))
+
+        res, spacing = self._per_label_call("laa_clusters", image, mask, spacing, host_call, dev_call)
+        return cl.from_native(res, res["labels"] | set(range(1, self.engine.n_classes[0])), self.modelname, spacing, threshold,
+                              connectivity, min_cluster_voxels)
+
+    def _mask_labels(self, mask, stream):
+        """The non-zero label values of a (S,H,W) uint8 CUDA mask tensor.  lm_label_stats_dev with the mask as its own uint8
+        volume and no percentiles or thresholds: its count and histogram passes over the mask bytes."""
+        voxels = self.engine.label_stats_dev(mask.data_ptr(), _native.DTYPE_U8, mask.data_ptr(), mask.shape, (), (),
+                                             stream=stream)["voxels"]
+        return set(int(x) for x in np.nonzero(voxels[1:256])[0] + 1)
+
+    def _per_label_call(self, what, image, mask, spacing, host_call, dev_call):
+        """The input handling of `statistics` and `laa_clusters` -> (the engine's result, spacing).  CUDA tensors go to
+        dev_call(volume tensor, dtype code, uint8 mask tensor, stream), both contiguous; everything else to
+        host_call(volume array, mask array)."""
         if _is_tensor(image) and image.is_cuda or _is_tensor(mask) and mask.is_cuda:
-            res = self._statistics_tensor(image, mask, q, t)
+            res = self._per_label_tensor(what, image, mask, dev_call)
         else:
             if _is_tensor(image):
                 image = image.detach()
@@ -352,44 +406,42 @@ class LMInferer:
             if isinstance(image, np.ndarray):
                 array = image
             else:
-                array, _ = self._array_and_orientation(image, "statistics")
+                array, _ = self._array_and_orientation(image, what)
                 if spacing is None:
                     spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
             array, mask = np.asarray(array), np.asarray(mask)
-            self._check_statistics_inputs(array.shape, mask.shape, mask.dtype == np.uint8 or mask.dtype == bool, mask.dtype)
-            res = self.engine.label_stats(array, mask, q, t)
+            self._check_per_label_inputs(what, array.shape, mask.shape, mask.dtype == np.uint8 or mask.dtype == bool, mask.dtype)
+            res = host_call(array, mask)
         if spacing is not None:
             spacing = tuple(float(s) for s in spacing)
             if len(spacing) != 3:
                 raise ValueError("spacing must be (x, y, z), got %s" % (spacing,))
-        labels = set(np.nonzero(res["voxels"][1:256])[0] + 1) | set(range(1, self.engine.n_classes[0]))
-        return st.from_native(res, labels, self.modelname, spacing, q, t)
+        return res, spacing
 
     @staticmethod
-    def _check_statistics_inputs(shape, mask_shape, mask_ok, mask_dtype):
+    def _check_per_label_inputs(what, shape, mask_shape, mask_ok, mask_dtype):
         if len(shape) != 3:
-            raise ValueError("statistics: expected a (slices, H, W) volume, got shape %s" % (tuple(shape),))
+            raise ValueError("%s: expected a (slices, H, W) volume, got shape %s" % (what, tuple(shape)))
         if not mask_ok:
-            raise TypeError("statistics: the mask must be uint8 or bool, got %s" % mask_dtype)
+            raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, mask_dtype))
         if tuple(mask_shape) != tuple(shape):
-            raise ValueError("statistics: the mask's shape %s differs from the volume's %s" % (tuple(mask_shape), tuple(shape)))
+            raise ValueError("%s: the mask's shape %s differs from the volume's %s" % (what, tuple(mask_shape), tuple(shape)))
 
-    def _statistics_tensor(self, image, mask, q, t):
+    def _per_label_tensor(self, what, image, mask, dev_call):
         import torch
         if not (_is_tensor(image) and _is_tensor(mask) and image.is_cuda and mask.is_cuda):
-            raise ValueError("statistics: a CUDA tensor needs a CUDA tensor as partner (volume on %s, mask on %s)"
-                             % (getattr(image, "device", "host"), getattr(mask, "device", "host")))
-        for what, x in (("volume", image), ("mask", mask)):
+            raise ValueError("%s: a CUDA tensor needs a CUDA tensor as partner (volume on %s, mask on %s)"
+                             % (what, getattr(image, "device", "host"), getattr(mask, "device", "host")))
+        for name, x in (("volume", image), ("mask", mask)):
             if x.device.index != self.engine.device:
-                raise ValueError("statistics: the %s tensor is on %s, the engine on cuda:%d" % (what, x.device, self.engine.device))
-        self._check_statistics_inputs(image.shape, mask.shape, mask.dtype in (torch.uint8, torch.bool), mask.dtype)
+                raise ValueError("%s: the %s tensor is on %s, the engine on cuda:%d" % (what, name, x.device, self.engine.device))
+        self._check_per_label_inputs(what, image.shape, mask.shape, mask.dtype in (torch.uint8, torch.bool), mask.dtype)
         code = _tensor_dtype_code(image)
         image = image.detach().contiguous()
         mask = mask.detach().contiguous()
         if mask.dtype == torch.bool:
             mask = mask.view(torch.uint8)
-        return self.engine.label_stats_dev(image.data_ptr(), code, mask.data_ptr(), image.shape, q, t,
-                                           stream=torch.cuda.current_stream(image.device).cuda_stream)
+        return dev_call(image, code, mask, torch.cuda.current_stream(image.device).cuda_stream)
 
 
 def apply(image, model=None, force_cpu=False, batch_size=20, volume_postprocessing=True, tqdm_disable=False):
