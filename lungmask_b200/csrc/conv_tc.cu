@@ -27,7 +27,9 @@
 //     the tensor core for the whole tile.
 //   * persistent CTAs (one per SM), warp-specialised: warp 0 is the TMA producer, warpgroups 1 and 2 are consumers
 //     that each own 64 rows of the tile (image rows 0-7 / 8-15 of the patch): they issue the wgmmas, drain the
-//     chunks and run the epilogue of their rows straight from the accumulator registers.
+//     chunks and run the epilogue of their rows from the accumulator registers.  Split-plane outputs (fp16 build) are
+//     staged in the tile's last activation buffer and written by warp 1, the storer, with TMA stores, so that the
+//     consumers go back to the wgmmas instead of waiting for scattered global stores to drain.
 //   * the 3x3 layers with 64 output channels run conv_cm64_kernel (below) unless ConvParams::conv64_cm is 0: the same
 //     scheme with the GEMM roles swapped (M = output channels, N = pixels), bit-identical results.
 #include <atomic>
@@ -49,6 +51,12 @@ constexpr int NUM_THREADS = 384;
 constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int MAX_CLASSES = 8;
 constexpr int REGS_PRODUCER = 40, REGS_CONSUMER = 232;   // 128 x 40 + 256 x 232 <= 65536
+// Split-plane output staging (fp16 build): one 64-channel half of a tile in the tile's last activation buffer, laid out
+// as the store boxes (ConvMaps::out / pool, 128B-swizzled): 16 x 8 pixels x 2 planes, then the 8 x 4 pooled pixels.
+constexpr int ST_PLANE = TILE_H * TILE_W * ROW_BYTES;                 // 16 KB
+constexpr int ST_POOL = 2 * ST_PLANE;
+constexpr int ST_POOL_PLANE = (TILE_H / 2) * (TILE_W / 2) * ROW_BYTES;  // 4 KB
+static_assert(ST_POOL + 2 * ST_POOL_PLANE <= A_BUF_BYTES, "a tile's output half fits one activation buffer");
 
 template <int BN>
 struct Cfg {
@@ -56,7 +64,8 @@ struct Cfg {
   static constexpr int STAGE_BYTES = 2 * B_PLANE_BYTES;      // one weight tile (hi + lo planes) per k-block
   static constexpr int STAGES = (BN == 64) ? 6 : 4;
   // dynamic shared memory only (1024-aligned for the swizzled tiles): activation patches | weight ring | mbarriers | head
-  static constexpr int NUM_BARS = 2 * STAGES + 2 * NUM_A_BUFS;
+  // mbarriers: full / empty per weight stage, full / empty / staged per activation buffer, and the staging area's "free"
+  static constexpr int NUM_BARS = 2 * STAGES + 3 * NUM_A_BUFS + 1;
   static constexpr int OFF_B = NUM_A_BUFS * A_BUF_BYTES;
   static constexpr int OFF_BARS = OFF_B + STAGES * STAGE_BYTES;
   static constexpr int OFF_HEAD = OFF_BARS + NUM_BARS * 8;                         // BN = 64 only: head weights + bias
@@ -100,24 +109,24 @@ struct WorkItems {
   }
 };
 
+#if !LM_OPERAND_F16
 // the hi / lo operand planes of two adjacent channels (c even) of one pixel
 __device__ __forceinline__ void store_split_pair(op_t* dst, size_t plane_stride, float a, float b) {
-#if LM_OPERAND_F16
-  uint32_t hi, lo;
-  split_f16x2(a, b, hi, lo);
-  *reinterpret_cast<uint32_t*>(dst) = hi;
-  *reinterpret_cast<uint32_t*>(dst + plane_stride) = lo;
-#else
   float ha, la, hb, lb;
   split_tf32(a, ha, la);
   split_tf32(b, hb, lb);
   *reinterpret_cast<float2*>(dst) = make_float2(ha, hb);
   *reinterpret_cast<float2*>(dst + plane_stride) = make_float2(la, lb);
-#endif
 }
+#endif
 
 __device__ __forceinline__ float2 ldg2_or_zero(const float* p, int c) {
   return p ? __ldg(reinterpret_cast<const float2*>(p + c)) : make_float2(0.f, 0.f);
+}
+
+// Modes whose outputs are split planes that the consumers stage in shared memory and the storer warp writes with TMA.
+__device__ __forceinline__ bool staged_stores(const ConvParams& p) {
+  return LM_OPERAND_F16 && (p.mode == kModeReluBn || p.mode == kModeReluBnPool);
 }
 
 // One consumer warpgroup: the wgmma loop over every tile of the CTA for its 64 rows, then the tile's epilogue.
@@ -125,8 +134,8 @@ __device__ __forceinline__ float2 ldg2_or_zero(const float* p, int c) {
 // (pairs c, c + 1 at c = n0 + 8 j + 2 (lane % 4)).
 template <int BN, int TAPS, int MC>
 __device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem_a, uint32_t smem_b, uint32_t full0,
-                                              uint32_t empty0, uint32_t afull0, uint32_t aempty0, const float* s_head_w,
-                                              const float* s_head_b) {
+                                              uint32_t empty0, uint32_t afull0, uint32_t aempty0, uint32_t staged0,
+                                              uint32_t sfree, const float* s_head_w, const float* s_head_b) {
   using C = Cfg<BN>;
   constexpr int NA = BN / 2;  // accumulator registers per thread for BN columns
   constexpr int STAGES = C::STAGES;
@@ -142,10 +151,12 @@ __device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem
   const int num_cb = (p.C0 + p.C1) / BK;
   const int num_kb = num_cb * TAPS, chunk_kb = p.chunk_kb;
   const uint32_t a_half = (uint32_t)(8 * half * PATCH_W * ROW_BYTES);
+  const bool staged = staged_stores(p);   // the storer, not the consumers, frees each tile's last activation buffer
 
   const WorkItems<MC> items(total_tiles, n_tiles);
   float S[NA], P[NA], Q[NA];   // round-to-nearest sum of hi*hi | open chunk of hi*hi | corrections (x 2^11 for fp16)
   uint32_t s = 0, ph = 0, ab = 0, aph = 0;
+  [[maybe_unused]] uint32_t fph = 0;   // parity of the staging area's "free" barrier (fp16 build)
   auto release = [&](uint32_t st, int a) {   // a weight stage (and an activation buffer, a >= 0) may be refilled
     __syncwarp();
     if (lane == 0) {
@@ -192,7 +203,8 @@ __device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem
           release(pend_s, pend_a);
         }
         pend_s = s;
-        pend_a = (tap == TAPS - 1) ? (int)ab : -1;   // a channel block's last tap frees its activation buffer
+        // a channel block's last tap frees its activation buffer, except the tile's last one when it stages the outputs
+        pend_a = (tap == TAPS - 1 && !(staged && kb == num_kb - 1)) ? (int)ab : -1;
         if (++s == STAGES) { s = 0; ph ^= 1u; }
         if (tap == TAPS - 1 && ++ab == NUM_A_BUFS) { ab = 0; aph ^= 1u; }
       }
@@ -295,7 +307,61 @@ __device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem
       for (int i = 0; i < NA; ++i) ovf |= !(fabsf(S[i]) <= kOpMax);
       if (__any_sync(0xffffffffu, ovf) && lane == 0 && p.range_flag) *p.range_flag = 1;
     }
-#endif
+    // Split planes (and their 2x2 average) staged in the tile's last activation buffer, one 64-channel half at a time, in
+    // the layout of the store boxes: box row (x, y) holds 128 B of channels, its 16-byte chunk k at chunk k ^ (row % 8)
+    // (128B swizzle).  The eight lanes of a chunk column hold eight consecutive box rows, so every store is conflict-free.
+    // The storer warp hands each staged half to TMA.
+    {
+      const uint32_t buf = smem_a + (ab ^ 1u) * (uint32_t)A_BUF_BYTES;   // ab has moved past the tile's last channel block
+      named_bar_sync(1, 256);   // both warpgroups' wgmmas have read the buffer (each reads halo rows of the other)
+#pragma unroll
+      for (int hc = 0; hc < BN / 64; ++hc) {
+        if (hc > 0) {   // the storer's TMA has read the previous half
+          mbar_spin(sfree, fph);
+          fph ^= 1u;
+        }
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = 8 * hc + jj;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            uint32_t hi, lo;
+            split_f16x2(S[4 * j + 2 * r], S[4 * j + 2 * r + 1], hi, lo);
+            const uint32_t row = (uint32_t)((8 * half + 2 * wq + r) * TILE_W + g);
+            const uint32_t a = buf + row * ROW_BYTES + (uint32_t)(((jj ^ g) << 4) + 4 * qd);
+            st_shared_u32(a, hi);
+            st_shared_u32(a + ST_PLANE, lo);
+          }
+        }
+        if (p.mode == kModeReluBnPool) {
+          // 2x2 average (resunet.py:64): a thread holds rows y and y + 1 of column x, lane ^ 4 holds column x ^ 1;
+          // (top-left + top-right) + (bottom-left + bottom-right), staged by the even-x lane
+          const uint32_t prow = (uint32_t)((4 * half + wq) * (TILE_W / 2) + (g >> 1));
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * hc + jj;
+            float pv[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float top = S[4 * j + e] + __shfl_xor_sync(0xffffffffu, S[4 * j + e], 4);
+              const float bot = S[4 * j + 2 + e] + __shfl_xor_sync(0xffffffffu, S[4 * j + 2 + e], 4);
+              pv[e] = (top + bot) * 0.25f;
+            }
+            if ((g & 1) == 0) {
+              uint32_t hi, lo;
+              split_f16x2(pv[0], pv[1], hi, lo);
+              const uint32_t a = buf + ST_POOL + prow * ROW_BYTES + ((((uint32_t)jj ^ (prow & 7u)) << 4) + 4 * qd);
+              st_shared_u32(a, hi);
+              st_shared_u32(a + ST_POOL_PLANE, lo);
+            }
+          }
+        }
+        fence_proxy_async_smem();   // the staged half is visible to the TMA store that reads it
+        __syncwarp();
+        if (lane == 0) mbar_arrive(staged0 + 8 * (ab ^ 1u));
+      }
+    }
+#else
     {
       const size_t plane = (size_t)p.H * p.W * p.Cout;
       op_t* img = static_cast<op_t*>(p.out) + (size_t)t.n * 2 * plane;
@@ -323,6 +389,7 @@ __device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem
         if ((g & 1) == 0) store_split_pair(img + 8 * j, plane, pv[0], pv[1]);
       }
     }
+#endif
   }
 }
 
@@ -334,7 +401,8 @@ __device__ __forceinline__ void conv_consumer(const ConvParams& p, uint32_t smem
 template <int BN, int MC>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBX, const ConvParams p) {
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBX,
+               const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmPool, const ConvParams p) {
   using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ __align__(1024) uint8_t smem[];   // layout: Cfg<BN>; no static shared memory
@@ -343,14 +411,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   float* s_head_b = s_head_w + MAX_CLASSES * 64;
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = full0 + 8 * STAGES;
   const uint32_t afull0 = full0 + 16 * STAGES, aempty0 = afull0 + 8 * NUM_A_BUFS;
+  const uint32_t staged0 = aempty0 + 8 * NUM_A_BUFS, sfree = staged0 + 8 * NUM_A_BUFS;
   const uint32_t smem_a = smem_u32(smem), smem_b = smem_a + C::OFF_B;
-  const int warp = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool staged = staged_stores(p);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, MC * NUM_CONSUMER_WARPS); }
-    for (int s = 0; s < NUM_A_BUFS; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, NUM_CONSUMER_WARPS); }
+    for (int s = 0; s < NUM_A_BUFS; ++s) {
+      mbar_init(afull0 + 8 * s, 1);
+      mbar_init(aempty0 + 8 * s, NUM_CONSUMER_WARPS);
+      mbar_init(staged0 + 8 * s, NUM_CONSUMER_WARPS);
+    }
+    mbar_init(sfree, 1);
     fence_mbar_init();
     tma_prefetch_desc(&tmA0); tma_prefetch_desc(&tmA1); tma_prefetch_desc(MC > 1 ? &tmBX : &tmB);
+    if (staged) {
+      tma_prefetch_desc(&tmOut);
+      if (p.mode == kModeReluBnPool) tma_prefetch_desc(&tmPool);
+    }
   }
   if (BN == 64 && p.mode == kModeHead) {
     for (int i = threadIdx.x; i < p.K * 64; i += NUM_THREADS) s_head_w[i] = p.head_w[i];
@@ -361,8 +440,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
 
   if (warp >= 4) {
     setmaxnreg_inc<REGS_CONSUMER>();
-    if (p.taps == 9) conv_consumer<BN, 9, MC>(p, smem_a, smem_b, full0, empty0, afull0, aempty0, s_head_w, s_head_b);
-    else conv_consumer<BN, 1, MC>(p, smem_a, smem_b, full0, empty0, afull0, aempty0, s_head_w, s_head_b);
+    if (p.taps == 9) conv_consumer<BN, 9, MC>(p, smem_a, smem_b, full0, empty0, afull0, aempty0, staged0, sfree, s_head_w, s_head_b);
+    else conv_consumer<BN, 1, MC>(p, smem_a, smem_b, full0, empty0, afull0, aempty0, staged0, sfree, s_head_w, s_head_b);
   } else {
     setmaxnreg_dec<REGS_PRODUCER>();
     if (warp == 0) {
@@ -403,6 +482,34 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
           }
         }
       }
+    } else if (warp == 1 && staged) {
+      // ------------------------------------------- storer (warp 1, lane 0 issues): the staged output halves to global
+      const int tiles_x = p.W / TILE_W, tiles_img = tiles_x * (p.H / TILE_H);
+      const int n_tiles = p.Cout / BN;
+      const WorkItems<MC> items(p.N * tiles_img * n_tiles, n_tiles);
+      const int num_cb = (p.C0 + p.C1) / BK;
+      uint32_t nb = 0, sph = 0;   // activation buffers the producer has filled so far | staged parity, one bit per buffer
+      for (int item = items.first; item < items.total; item += items.step) {
+        const TileCoord t = decode_tile(items.tile(item), n_tiles, tiles_x, tiles_img, BN);
+        const uint32_t b = (nb + (uint32_t)num_cb - 1u) % NUM_A_BUFS;   // the tile's last activation buffer
+        nb += (uint32_t)num_cb;
+#pragma unroll
+        for (int hc = 0; hc < BN / 64; ++hc) {
+          mbar_wait_inline(staged0 + 8 * b, (sph >> b) & 1u);
+          sph ^= 1u << b;
+          if (lane == 0) {
+            const uint32_t src = smem_a + b * (uint32_t)A_BUF_BYTES;
+            tma_store_5d(&tmOut, src, t.n0 + 64 * hc, t.x0, t.y0, 0, t.n);
+            if (p.mode == kModeReluBnPool) tma_store_5d(&tmPool, src + ST_POOL, t.n0 + 64 * hc, t.x0 / 2, t.y0 / 2, 0, t.n);
+            bulk_commit();
+            bulk_wait_read<0>();
+            if (hc + 1 < BN / 64) mbar_arrive(sfree);                       // the consumers may stage the next half
+            else mbar_arrive_cnt(aempty0 + 8 * b, NUM_CONSUMER_WARPS);    // the producer may refill the buffer
+          }
+          __syncwarp();
+        }
+      }
+      if (lane == 0) bulk_wait<0>();   // the outputs are in global memory before the CTA (and its cluster) finishes
     }
   }
   // MC = 2: no CTA leaves while its peer may still multicast into its shared memory or arrive on its barriers
@@ -429,14 +536,19 @@ constexpr int CM_A_PLANE = CM_HALO * CM_HALO * ROW_BYTES;  // 324 rows x 128 B =
 constexpr int CM_A_BUF = 2 * CM_A_PLANE;                   // 82944 B (both planes), 1024-aligned
 constexpr int CM_STAGES = 3;
 constexpr int CM_STAGE_BYTES = Cfg<64>::STAGE_BYTES;       // 16 KB: 64 cout x 64 cin, hi + lo planes
-constexpr int CM_NUM_BARS = 2 * CM_STAGES + 2 * NUM_A_BUFS;
+constexpr int CM_NUM_BARS = 2 * CM_STAGES + 3 * NUM_A_BUFS;   // full / empty per stage, full / empty / staged per buffer
 constexpr int CM_OFF_B = NUM_A_BUFS * CM_A_BUF;
 constexpr int CM_OFF_BARS = CM_OFF_B + CM_STAGES * CM_STAGE_BYTES;
 constexpr int CM_OFF_HEAD = CM_OFF_BARS + CM_NUM_BARS * 8;
-constexpr int CM_DYN_SMEM = CM_OFF_HEAD + (MAX_CLASSES * 64 + MAX_CLASSES) * 4;   // 217200 B
+constexpr int CM_DYN_SMEM = CM_OFF_HEAD + (MAX_CLASSES * 64 + MAX_CLASSES) * 4;   // 217216 B
 static_assert(CM_DYN_SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
 constexpr int CM_Y_STRIDE = 65;   // head: the tile's fp32 y staged [pixel][channel], padded against bank conflicts
 static_assert(CM_TILE * CM_TILE * CM_Y_STRIDE * 4 <= CM_A_BUF, "the head's staging fits one activation buffer");
+// split-plane staging: the tile's 16 x 16 pixels x 2 planes, then its 8 x 8 pooled pixels, as the store boxes lay them out
+constexpr int CM_ST_PLANE = CM_TILE * CM_TILE * ROW_BYTES;                 // 32 KB
+constexpr int CM_ST_POOL = 2 * CM_ST_PLANE;
+constexpr int CM_ST_POOL_PLANE = (CM_TILE / 2) * (CM_TILE / 2) * ROW_BYTES;  // 8 KB
+static_assert(CM_ST_POOL + 2 * CM_ST_POOL_PLANE <= CM_A_BUF, "a tile's outputs fit one activation buffer");
 
 #if LM_OPERAND_F16
 struct CmTile {
@@ -454,7 +566,7 @@ __device__ __forceinline__ CmTile cm_tile(int tile, int tiles_x, int tiles_img) 
 
 __device__ __forceinline__ void cm64_consumer(const ConvParams& p, uint8_t* smem, uint32_t smem_a, uint32_t smem_b,
                                               uint32_t full0, uint32_t empty0, uint32_t afull0, uint32_t aempty0,
-                                              const float* s_head_w, const float* s_head_b) {
+                                              uint32_t staged0, const float* s_head_w, const float* s_head_b) {
   constexpr uint32_t SBO_X = CM_HALO * ROW_BYTES;
   const int tid = threadIdx.x - 128;
   const int half = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
@@ -479,8 +591,8 @@ __device__ __forceinline__ void cm64_consumer(const ConvParams& p, uint8_t* smem
     const CmTile t = cm_tile(tile, tiles_x, tiles_img);
 #pragma unroll
     for (int i = 0; i < 64; ++i) { S[i] = 0.f; Q[i] = 0.f; }
-    // the k loop of conv_consumer (chunks, wait discipline, releases); the head keeps the tile's last activation buffer
-    // until its epilogue has staged y through it
+    // the k loop of conv_consumer (chunks, wait discipline, releases); the tile's last activation buffer stays taken until
+    // the epilogue has staged y (head) or the outputs (the storer frees it) through it
     for (int kb0 = 0; kb0 < num_kb; kb0 += chunk_kb) {
       const int kb1 = min(kb0 + chunk_kb, num_kb);
       uint32_t pend_s = 0;
@@ -506,7 +618,7 @@ __device__ __forceinline__ void cm64_consumer(const ConvParams& p, uint8_t* smem
           release(pend_s, pend_a);
         }
         pend_s = s;
-        pend_a = (tap == 8 && !(head && kb == num_kb - 1)) ? (int)ab : -1;
+        pend_a = (tap == 8 && kb != num_kb - 1) ? (int)ab : -1;
         if (++s == CM_STAGES) { s = 0; ph ^= 1u; }
         if (tap == 8 && ++ab == NUM_A_BUFS) { ab = 0; aph ^= 1u; }
       }
@@ -593,31 +705,27 @@ __device__ __forceinline__ void cm64_consumer(const ConvParams& p, uint8_t* smem
       for (int i = 0; i < 64; ++i) ovf |= !(fabsf(S[i]) <= kOpMax);
       if (__any_sync(0xffffffffu, ovf) && lane == 0 && p.range_flag) *p.range_flag = 1;
     }
-    // Split planes.  Per image row j and channel octet u the warp holds an 8 x 8 matrix (channel g, pixel column 2qd + e)
-    // in the movmatrix fragment layout; its transpose gives lane (g, qd) channels 16w + 8u + 2qd, +1 of column 8h + g,
-    // stored as one hi and one lo pair like conv_consumer's.
-    {
-      const size_t plane = (size_t)p.H * p.W * 64;
-      op_t* dst = static_cast<op_t*>(p.out) + (size_t)t.n * 2 * plane + ((size_t)t.y0 * p.W + t.x0 + 8 * half + g) * 64 + 16 * wq + 2 * qd;
+    // Split planes, staged in the tile's last activation buffer in the layout of the store boxes (conv_consumer's:
+    // 128-byte box rows of channels, 16-byte chunk k at chunk k ^ (row % 8)) for the storer warp's TMA stores.  Per image
+    // row j and channel octet u the warp holds an 8 x 8 matrix (channel g, pixel column 2qd + e) in the movmatrix
+    // fragment layout; its transpose gives lane (g, qd) channels 16w + 8u + 2qd, +1 of column 8h + g: the eight lanes of
+    // a chunk column hold eight consecutive box rows.
+    const uint32_t buf = smem_a + (ab ^ 1u) * (uint32_t)CM_A_BUF;   // ab has moved past the tile's last channel block
+    named_bar_sync(1, 256);   // both warpgroups' wgmmas have read the buffer (each reads halo rows of the other)
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
+    for (int j = 0; j < 16; ++j)
 #pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          uint32_t hi, lo;
-          split_f16x2(S[4 * j + 2 * u], S[4 * j + 2 * u + 1], hi, lo);
-          op_t* d = dst + (size_t)j * p.W * 64 + 8 * u;
-          *reinterpret_cast<uint32_t*>(d) = movmatrix_trans(hi);
-          *reinterpret_cast<uint32_t*>(d + plane) = movmatrix_trans(lo);
-        }
-    }
+      for (int u = 0; u < 2; ++u) {
+        uint32_t hi, lo;
+        split_f16x2(S[4 * j + 2 * u], S[4 * j + 2 * u + 1], hi, lo);
+        const uint32_t a = buf + (uint32_t)((16 * j + 8 * half + g) * ROW_BYTES + (((2 * wq + u) ^ g) << 4) + 4 * qd);
+        st_shared_u32(a, movmatrix_trans(hi));
+        st_shared_u32(a + CM_ST_PLANE, movmatrix_trans(lo));
+      }
     if (p.mode == kModeReluBnPool) {
       // 2x2 average, ((top-left + top-right) + (bottom-left + bottom-right)) * 0.25, inside the thread: pooled pixel (row i,
       // column 4h + qd).  Pooled rows 2m and 2m + 1 pack into one matrix (channel g, column 2qd + r); after the transpose
       // lane (g, qd) holds channels 16w + 8u + 2qd, +1 of pooled pixel (row 2m + g % 2, column 4h + g / 2).
-      const int Wp = p.W / 2;
-      const size_t plane = (size_t)(p.H / 2) * Wp * 64;
-      op_t* dst = static_cast<op_t*>(p.out_pool) + (size_t)t.n * 2 * plane +
-                  ((size_t)(t.y0 / 2 + (g & 1)) * Wp + t.x0 / 2 + 4 * half + (g >> 1)) * 64 + 16 * wq + 2 * qd;
 #pragma unroll
       for (int m = 0; m < 4; ++m)
 #pragma unroll
@@ -632,32 +740,45 @@ __device__ __forceinline__ void cm64_consumer(const ConvParams& p, uint8_t* smem
           }
           uint32_t hi, lo;
           split_f16x2(pv[0], pv[1], hi, lo);
-          op_t* d = dst + (size_t)(2 * m) * Wp * 64 + 8 * u;
-          *reinterpret_cast<uint32_t*>(d) = movmatrix_trans(hi);
-          *reinterpret_cast<uint32_t*>(d + plane) = movmatrix_trans(lo);
+          const int prow = (2 * m + (g & 1)) * (CM_TILE / 2) + 4 * half + (g >> 1);
+          const uint32_t a = buf + CM_ST_POOL + (uint32_t)(prow * ROW_BYTES + (((2 * wq + u) ^ (prow & 7)) << 4) + 4 * qd);
+          st_shared_u32(a, movmatrix_trans(hi));
+          st_shared_u32(a + CM_ST_POOL_PLANE, movmatrix_trans(lo));
         }
     }
+    fence_proxy_async_smem();   // the staged tile is visible to the TMA stores that read it
+    __syncwarp();
+    if (lane == 0) mbar_arrive(staged0 + 8 * (ab ^ 1u));
   }
 }
 
 // conv_tc_kernel's warp roles and mbarrier protocol (MC = 1) with the channel-major consumer; 3 weight stages.
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_cm64_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
-                 const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
+                 const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+                 const __grid_constant__ CUtensorMap tmPool, const ConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];   // activation buffers | weight ring | mbarriers | head
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + CM_OFF_BARS);
   float* s_head_w = reinterpret_cast<float*>(smem + CM_OFF_HEAD);
   float* s_head_b = s_head_w + MAX_CLASSES * 64;
   const uint32_t full0 = smem_u32(&bars[0]), empty0 = full0 + 8 * CM_STAGES;
-  const uint32_t afull0 = full0 + 16 * CM_STAGES, aempty0 = afull0 + 8 * NUM_A_BUFS;
+  const uint32_t afull0 = full0 + 16 * CM_STAGES, aempty0 = afull0 + 8 * NUM_A_BUFS, staged0 = aempty0 + 8 * NUM_A_BUFS;
   const uint32_t smem_a = smem_u32(smem), smem_b = smem_a + CM_OFF_B;
-  const int warp = threadIdx.x >> 5;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < CM_STAGES; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, NUM_CONSUMER_WARPS); }
-    for (int s = 0; s < NUM_A_BUFS; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, NUM_CONSUMER_WARPS); }
+    for (int s = 0; s < NUM_A_BUFS; ++s) {
+      mbar_init(afull0 + 8 * s, 1);
+      mbar_init(aempty0 + 8 * s, NUM_CONSUMER_WARPS);
+      mbar_init(staged0 + 8 * s, NUM_CONSUMER_WARPS);
+    }
     fence_mbar_init();
     tma_prefetch_desc(&tmA0); tma_prefetch_desc(&tmA1); tma_prefetch_desc(&tmB);
+    if (p.mode != kModeHead) {
+      tma_prefetch_desc(&tmOut);
+      if (p.mode == kModeReluBnPool) tma_prefetch_desc(&tmPool);
+    }
   }
   if (p.mode == kModeHead) {
     for (int i = threadIdx.x; i < p.K * 64; i += NUM_THREADS) s_head_w[i] = p.head_w[i];
@@ -667,7 +788,7 @@ conv_cm64_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
 
   if (warp >= 4) {
     setmaxnreg_inc<REGS_CONSUMER>();
-    cm64_consumer(p, smem, smem_a, smem_b, full0, empty0, afull0, aempty0, s_head_w, s_head_b);
+    cm64_consumer(p, smem, smem_a, smem_b, full0, empty0, afull0, aempty0, staged0, s_head_w, s_head_b);
   } else {
     setmaxnreg_dec<REGS_PRODUCER>();
     if (warp == 0) {
@@ -699,6 +820,28 @@ conv_cm64_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant
           }
         }
       }
+    } else if (warp == 1 && p.mode != kModeHead) {
+      // ------------------------------------------------- storer (warp 1, lane 0 issues): conv_tc_kernel's, one pass per tile
+      const int tiles_x = p.W / CM_TILE, tiles_img = tiles_x * (p.H / CM_TILE);
+      const int num_cb = (p.C0 + p.C1) / BK;
+      uint32_t nb = 0, sph = 0;
+      for (int tile = blockIdx.x; tile < p.N * tiles_img; tile += gridDim.x) {
+        const CmTile t = cm_tile(tile, tiles_x, tiles_img);
+        const uint32_t b = (nb + (uint32_t)num_cb - 1u) % NUM_A_BUFS;
+        nb += (uint32_t)num_cb;
+        mbar_wait_inline(staged0 + 8 * b, (sph >> b) & 1u);
+        sph ^= 1u << b;
+        if (lane == 0) {
+          const uint32_t src = smem_a + b * (uint32_t)CM_A_BUF;
+          tma_store_5d(&tmOut, src, 0, t.x0, t.y0, 0, t.n);
+          if (p.mode == kModeReluBnPool) tma_store_5d(&tmPool, src + CM_ST_POOL, 0, t.x0 / 2, t.y0 / 2, 0, t.n);
+          bulk_commit();
+          bulk_wait_read<0>();
+          mbar_arrive_cnt(aempty0 + 8 * b, NUM_CONSUMER_WARPS);
+        }
+        __syncwarp();
+      }
+      if (lane == 0) bulk_wait<0>();
     }
   }
 }
@@ -737,7 +880,8 @@ int encode(CUtensorMap* m, CUtensorMapDataType dtype, const void* base, int rank
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
-// activation boxes of box_w x box_h pixels (tile + halo), BK channels, both planes, one image
+// split-plane boxes of box_w x box_h pixels, BK channels, both planes, one image: activation loads (tile + halo) and
+// output stores
 int make_act_map(CUtensorMap* m, const void* base, int n_cap, int H, int W, int Cch, int box_w, int box_h) {
   const cuuint64_t E = kOpBytes;
   cuuint64_t dims[5] = {(cuuint64_t)Cch, (cuuint64_t)W, (cuuint64_t)H, 2, (cuuint64_t)n_cap};
@@ -769,6 +913,17 @@ int make_conv_maps(ConvMaps* maps, const void* src0, const void* src1, const voi
     r = make_act_map(&maps->a1cm, s1, n_capacity, p.H, p.W, c1, CM_HALO, CM_HALO);
     if (r) return r;
   }
+#if LM_OPERAND_F16
+  if (p.mode == kModeReluBn || p.mode == kModeReluBnPool) {
+    const bool pool = p.mode == kModeReluBnPool, cm = conv_cm64_fits(p);
+    const int Hp = p.H / 2, Wp = p.W / 2;
+    r = make_act_map(&maps->out, p.out, n_capacity, p.H, p.W, p.Cout, TILE_W, TILE_H);
+    if (!r && pool) r = make_act_map(&maps->pool, p.out_pool, n_capacity, Hp, Wp, p.Cout, TILE_W / 2, TILE_H / 2);
+    if (!r && cm) r = make_act_map(&maps->outcm, p.out, n_capacity, p.H, p.W, p.Cout, CM_TILE, CM_TILE);
+    if (!r && cm && pool) r = make_act_map(&maps->poolcm, p.out_pool, n_capacity, Hp, Wp, p.Cout, CM_TILE / 2, CM_TILE / 2);
+    if (r) return r;
+  }
+#endif
   const int Cin = p.C0 + p.C1;
   cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)p.Cout, (cuuint64_t)p.taps, 2};
   cuuint64_t strides[3] = {(cuuint64_t)Cin * E, (cuuint64_t)p.Cout * Cin * E, (cuuint64_t)p.taps * p.Cout * Cin * E};
@@ -801,7 +956,7 @@ static int launch_impl(const ConvMaps& maps, const ConvParams& p, int num_sms, c
   attr[0].val.clusterDim.x = MC; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, MC>, maps.a0, maps.a1, maps.b, maps.bx, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, MC>, maps.a0, maps.a1, maps.b, maps.bx, maps.out, maps.pool, p);
   return (int)(e != cudaSuccess ? e : cudaGetLastError());
 }
 
@@ -824,7 +979,8 @@ int launch_conv_tc(const ConvMaps& maps, const ConvParams& p, int num_sms, cudaS
 #if LM_OPERAND_F16
   if (p.conv64_cm && conv_cm64_fits(p)) {   // conv_tc_prepare has set the kernel's shared-memory opt-in
     const int total = p.N * (p.H / CM_TILE) * (p.W / CM_TILE);
-    conv_cm64_kernel<<<total < num_sms ? total : num_sms, NUM_THREADS, CM_DYN_SMEM, stream>>>(maps.a0cm, maps.a1cm, maps.b, p);
+    conv_cm64_kernel<<<total < num_sms ? total : num_sms, NUM_THREADS, CM_DYN_SMEM, stream>>>(maps.a0cm, maps.a1cm, maps.b, maps.outcm,
+                                                                                          maps.poolcm, p);
     return (int)cudaGetLastError();
   }
 #endif

@@ -81,6 +81,9 @@ struct ConvMaps {
   CUtensorMap a0, a1, b;
   CUtensorMap bx;  // weights, one plane per box: the per-CTA half of a multicast weight stage (weight_mcast = 2)
   CUtensorMap a0cm, a1cm;  // activations in 16x16-pixel boxes (+ halo) for conv_cm64_kernel; built when conv_cm64_fits
+  // split-plane outputs (fp16 build, modes 0 / 1), one 64-channel half of a tile per box, both planes: p.out in 16x8 /
+  // p.out_pool in 8x4 pixels for conv_tc_kernel, 16x16 / 8x8 for conv_cm64_kernel (built when conv_cm64_fits)
+  CUtensorMap out, pool, outcm, poolcm;
 };
 
 // Layers the channel-major kernel serves: 3x3, 64 output channels, 16x16 tiles, fp16-pair operands, a split-plane

@@ -35,6 +35,10 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// `count` arrivals at once (one thread standing in for several warps)
+__device__ __forceinline__ void mbar_arrive_cnt(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -96,6 +100,21 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* m, 
       "l"(m), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
+// shared memory -> global through a tensor map, tracked by the issuing thread's bulk async-groups (the shared-memory
+// writes it reads must be made visible to the async proxy first: fence_proxy_async_smem by every writing thread)
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(m),
+      "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of the thread's bulk groups still read their shared-memory source (the source may be overwritten)
+template <int N> __device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of the thread's bulk groups are incomplete (their global writes are done)
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // ---------------------------------------------------------------- clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -120,8 +139,11 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank)
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
-// generic-proxy shared-memory accesses before it are ordered before later async-proxy (TMA) writes to the same memory
+// generic-proxy shared-memory accesses before it are ordered before later async-proxy (TMA) accesses to the same memory
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 // 8x8 matrix of 16-bit elements held one row per lane quad (lane l: row l / 4, columns 2 (l % 4), +1 packed low / high)
 // -> its transpose in the same layout
 __device__ __forceinline__ uint32_t movmatrix_trans(uint32_t x) {

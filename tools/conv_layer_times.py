@@ -8,6 +8,11 @@ waves of 33 slices), profiles whole-volume forwards with torch.profiler (CUDA ac
 convolution kernel record, in start-time order, to its LAYERS index (engine.cu: 21 per wave).  Each entry of --values is
 one profiled round with the engine option --option set to it; alternating the settings in one process gives a before /
 after that shares the GPU's state.  Prints a table per setting and writes DIR/conv_layer_times.json.
+
+Per kernel it also fits  time = a * tiles + c * k-blocks  over that kernel's 3x3 layers, both counts those of the busiest
+CTA (the LAYERS shapes, waves of 33 slices over 132 SMs): c is the mainloop's cost per k-block, a the cost per output tile
+that does not overlap it (epilogue, pipeline fill).  The fit is printed for the mean and for every round, whose spread
+shows how far a and c can be trusted.
 """
 import argparse
 import json
@@ -50,6 +55,8 @@ FULL_RES_64 = (0, 19, 20)                                         # the 3x3 laye
 LEVEL_1_2_3X3 = [i for i, l in enumerate(LAYERS) if l[1] in (1, 2) and l[5] == 9]
 CONV_KERNELS = ("conv_tc_kernel", "conv_cm64_kernel")
 RES, SLICES, WAVE = 256, 300, 33
+WAVES = [min(WAVE, SLICES - s) for s in range(0, SLICES, WAVE)]   # slices per forward batch
+SMS = 132
 
 
 def layer_gflop(i):
@@ -113,6 +120,44 @@ def table(ms, names):
                      "gflop_per_slice": layer_gflop(i), "ms_per_volume": float(ms[i]),
                      "tflops": gf / (ms[i] * 1e-3) / 1e3, "kernel": names[i]})
     return rows
+
+
+def launch_work(i, kernel):
+    """(tiles, k-blocks) of the busiest CTA of layer i, summed over one volume's waves: conv_tc_kernel<BN, MC> tiles are
+    16x8 pixels x BN channels, conv_cm64_kernel tiles 16x16 pixels x 64 channels; a launch spreads its tiles over SMS CTAs"""
+    _, level, c0, c1, cout, taps = LAYERS[i]
+    hw = RES >> level
+    if "cm64" in kernel:
+        tiles_per_image = (hw // 16) ** 2
+    else:
+        bn = int(re.search(r"<\s*(\d+)", kernel).group(1))
+        tiles_per_image = (hw // 16) * (hw // 8) * (cout // bn)
+    kb_per_tile = (c0 + c1) // 64 * taps
+    tiles = sum(-(-n * tiles_per_image // SMS) for n in WAVES)
+    return tiles, tiles * kb_per_tile
+
+
+def tile_fit(ms, names):
+    """per kernel, the least-squares fit  us per volume = a * tiles per CTA + c * k-blocks per CTA  over its 3x3 layers"""
+    fits = {}
+    for kernel in sorted(set(names)):
+        idx = [i for i in range(len(LAYERS)) if names[i] == kernel and LAYERS[i][5] == 9]
+        if len(idx) < 2:
+            continue
+        X = np.array([launch_work(i, kernel) for i in idx], dtype=float)
+        y = np.array([ms[i] * 1e3 for i in idx])
+        (a, c), *_ = np.linalg.lstsq(X, y, rcond=None)
+        fits[kernel] = {"layers": idx, "a_us_per_tile": float(a), "c_us_per_kblock": float(c),
+                        "per_tile_share": float(a * X[:, 0].sum() / y.sum())}
+    return fits
+
+
+def print_fit(fits, per_round):
+    for kernel, f in fits.items():
+        rounds = [r[kernel] for r in per_round if kernel in r]
+        print("%-24s a = %6.2f us/tile (rounds %s), c = %6.3f us/k-block (rounds %s); per-tile term %.1f %% of its time"
+              % (kernel, f["a_us_per_tile"], ", ".join("%.2f" % r["a_us_per_tile"] for r in rounds), f["c_us_per_kblock"],
+                 ", ".join("%.3f" % r["c_us_per_kblock"] for r in rounds), 100 * f["per_tile_share"]))
 
 
 def summary(rows):
@@ -194,7 +239,10 @@ def main():
         summ["full_res_64_ms_per_round"] = [float(sum(r["ms"][i] for i in FULL_RES_64)) for r in mine]
         label = "defaults" if v is None else "%s = %d" % (args.option, v)
         print_table(label, rows, summ)
-        result["settings"][label] = {"layers": rows, "summary": summ}
+        fits = tile_fit(ms, mine[0]["names"])
+        per_round = [tile_fit(r["ms"], r["names"]) for r in mine]
+        print_fit(fits, per_round)
+        result["settings"][label] = {"layers": rows, "summary": summ, "tile_fit": fits, "tile_fit_per_round": per_round}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "conv_layer_times.json"), "w") as f:
         json.dump(result, f, indent=1)
