@@ -199,6 +199,34 @@ LM_API int lm_laa_clusters_dev(lm_engine* e, const void* d_vol, int dtype, const
                                int threshold, int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs,
                                int64_t* sizes, int64_t* counts, size_t max_pairs, void* stream);
 
+/* Regional statistics support (no counterpart in the reference; DESIGN §4.8): craniocaudal zones and depth shells below the
+ * lung surface.  LMInferer.regional_statistics turns a zone or shell assignment into a uint8 region map and runs
+ * lm_label_stats_dev on it.  All three take device memory of the engine's device and the caller's cudaStream_t with the
+ * event-wait rule of lm_apply_dev, check every argument before any kernel runs and return after the engine's stream has
+ * synchronised; the inputs are never written.  mask  (n0,n1,n2) uint8.
+ * lm_plane_label_counts_dev: the voxels of every label in every plane along array axis `axis` (0, 1 or 2):
+ *   counts [n_axis][257] int64 (host), counts[p][l] = the voxels with mask == l in plane p, counts[p][256] = mask > 0.
+ * lm_surface_distance_dev: the Euclidean distance in mm from every voxel with mask > 0 to the nearest voxel with
+ * mask == 0 (the outside of the union of all labels; fissures between labels are interior), axis k weighted by
+ * spacing[k] (3 finite positive doubles, per ARRAY axis).  d_out (n0,n1,n2) float32: the float64 distance rounded once;
+ * 0 where mask == 0; +inf when the mask has no zero voxel.  Voxels outside the array are not background (as
+ * scipy.ndimage.distance_transform_edt): a lung cut by the first or last slice has no surface there.  Equal to
+ * np.float32(scipy.ndimage.distance_transform_edt(mask > 0, sampling=spacing)) bit for bit when every (delta * s_k)^2 and
+ * their sums are exact in float64 (dyadic spacings such as 0.703125 or 1.25), else within 1 float32 ulp.  Work area:
+ * 20 bytes per voxel, kept by the engine.
+ * lm_region_map_dev: d_map[v] = lut[bucket(v) * 256 + mask[v]] (n0,n1,n2 uint8).  d_dist NULL: bucket = the plane index
+ * of v along `axis` (0, 1 or 2), n_bounds 0, n_axis buckets.  Otherwise bucket = the number of the n_bounds float32
+ * `bounds` (finite, positive, strictly increasing, at most 254; host memory) that are <= d_dist[v] (float32 (n0,n1,n2),
+ * e.g. from lm_surface_distance_dev), n_bounds + 1 buckets; `axis` is ignored.  lut (host): buckets * 256 codes
+ * (lut_size), lut[b * 256 + 0] == 0 for every b. */
+LM_API int lm_plane_label_counts_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int axis, int64_t* counts,
+                                     void* stream);
+LM_API int lm_surface_distance_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, const double* spacing,
+                                   float* d_out, void* stream);
+LM_API int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, int n0, int n1, int n2, int axis,
+                             const float* bounds, int n_bounds, const uint8_t* lut, size_t lut_size, uint8_t* d_map,
+                             void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -4,15 +4,16 @@ Inputs are read by lungmask_b200/io.py (DICOM series directory, NIfTI, MetaImage
 mask is written with the input's geometry as .nii / .nii.gz / .mha / .npy.  `--probabilities PATH` also writes the
 model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_with_probabilities), and `--statistics PATH`
 the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950),
-and `--clusters PATH` the size distributions of the low-attenuation clusters with their exponent D (.json / .csv,
-LMInferer.laa_clusters).
+`--clusters PATH` the size distributions of the low-attenuation clusters with their exponent D (.json / .csv,
+LMInferer.laa_clusters), and `--regions PATH` the statistics of every label by upper / middle / lower zone and by depth
+below the lung surface (.json / .csv, LMInferer.regional_statistics).
 """
 import argparse
 import os
 import sys
 
-from .io import (check_clusters_path, check_probabilities_path, check_statistics_path, load_input_image, save_clusters,
-                 save_mask, save_probabilities, save_statistics)
+from .io import (check_clusters_path, check_probabilities_path, check_regions_path, check_statistics_path, load_input_image,
+                 save_clusters, save_mask, save_probabilities, save_regional_statistics, save_statistics)
 from .logger import logger
 from .mask import LMInferer
 
@@ -52,6 +53,10 @@ def build_parser():
                    help="Low-attenuation threshold of --clusters, an integer HU in [-1024, 3072] (default -950)")
     p.add_argument("--clusters-connectivity", type=int, choices=[4, 6, 26], default=6,
                    help="Cluster connectivity of --clusters: 6 faces (default), 26 full, 4 faces within a slice")
+    p.add_argument("--regions", metavar="PATH", type=str, default=None,
+                   help="Also write the statistics of --statistics for every label and the whole lung by craniocaudal "
+                        "zone (upper / middle / lower thirds of each row's volume) and by depth below the lung surface "
+                        "(rind < 10 mm, core): .json (with the per-plane volume profile) or .csv")
     return p
 
 
@@ -70,6 +75,8 @@ def main(argv=None):
             check_arguments(args.clusters_threshold, args.clusters_connectivity, 1)
         except ValueError as ex:
             sys.exit("--clusters-threshold: %s" % ex)
+    if args.regions is not None:
+        check_regions_path(args.regions)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -99,6 +106,9 @@ def main(argv=None):
         logger.info(f"Save clusters to: {args.clusters}")
         save_clusters(args.clusters, inferer.laa_clusters(image, result, threshold=args.clusters_threshold,
                                                           connectivity=args.clusters_connectivity))
+    if args.regions is not None:
+        logger.info(f"Save regional statistics to: {args.regions}")
+        save_regional_statistics(args.regions, inferer.regional_statistics(image, result))
 
 
 if __name__ == "__main__":

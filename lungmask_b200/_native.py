@@ -57,6 +57,9 @@ def lib():
         "lm_laa_max_pairs": ([C.c_size_t], C.c_size_t),
         "lm_laa_clusters": ([vp, vp, i32, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t], i32),
         "lm_laa_clusters_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t, vp], i32),
+        "lm_plane_label_counts_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
+        "lm_surface_distance_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp], i32),
+        "lm_region_map_dev": ([vp, u8p, vp, i32, i32, i32, i32, vp, i32, vp, C.c_size_t, vp, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -86,7 +89,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters", "lm_laa_clusters_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -340,6 +343,37 @@ class Engine:
         total = int(res["offsets"][-1])
         res["sizes"], res["counts"] = sizes[:total].copy(), counts[:total].copy()
         return res
+
+    # ---- regional statistics support (lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev)
+    def plane_label_counts_dev(self, d_mask_ptr, shape, axis, stream=0):
+        """Voxels per label in every plane along array `axis` of a (n0,n1,n2) uint8 device mask (`stream` as for apply_dev)
+        -> int64 (n_axis, 257): [p, l] = voxels with mask == l in plane p, [p, 256] = mask > 0."""
+        n0, n1, n2 = (int(x) for x in shape)
+        n_axis = (n0, n1, n2)[axis] if axis in (0, 1, 2) else 0
+        counts = np.zeros((max(n_axis, 1), 257), np.int64)
+        _check(lib().lm_plane_label_counts_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, int(axis), _ptr(counts),
+                                               C.c_void_p(int(stream)) if stream else None))
+        return counts[:n_axis]
+
+    def surface_distance_dev(self, d_mask_ptr, shape, spacing, d_out_ptr, stream=0):
+        """Writes the float32 distance (mm) of every mask > 0 voxel to the nearest mask == 0 voxel to `d_out_ptr`;
+        `spacing` per array axis (s0, s1, s2)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        sp = np.ascontiguousarray(spacing, dtype=np.float64).reshape(-1)
+        if sp.size != 3:
+            raise ValueError("surface_distance_dev: spacing needs 3 values, got %d" % sp.size)
+        _check(lib().lm_surface_distance_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, _ptr(sp), C.c_void_p(d_out_ptr),
+                                             C.c_void_p(int(stream)) if stream else None))
+
+    def region_map_dev(self, d_mask_ptr, shape, lut, d_map_ptr, axis=None, d_dist_ptr=None, bounds=(), stream=0):
+        """Writes d_map[v] = lut[bucket(v), mask[v]]: bucket = the plane index along `axis` (d_dist_ptr None) or the
+        number of the float32 `bounds` <= d_dist[v].  `lut`: uint8 (buckets, 256) with lut[:, 0] == 0."""
+        n0, n1, n2 = (int(x) for x in shape)
+        lut = np.ascontiguousarray(lut, dtype=np.uint8)
+        b = np.ascontiguousarray(bounds, dtype=np.float32).reshape(-1)
+        _check(lib().lm_region_map_dev(self._h, C.c_void_p(d_mask_ptr), C.c_void_p(d_dist_ptr) if d_dist_ptr else None,
+                                       n0, n1, n2, -1 if axis is None else int(axis), _ptr(b) if b.size else None, int(b.size),
+                                       _ptr(lut), lut.size, C.c_void_p(d_map_ptr), C.c_void_p(int(stream)) if stream else None))
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

@@ -18,6 +18,7 @@
 #include "shard.cuh"
 #include "stats.cuh"
 #include "clusters.cuh"
+#include "regions.cuh"
 
 using namespace lm;
 
@@ -192,6 +193,7 @@ struct lm_engine {
   PostScratch post;
   LabelStatsWork stats;   // lm_label_stats*: counts, histograms and selection state (a host call's volume and mask go to d_upload)
   ClusterWork clusters;   // lm_laa_clusters*: LAA maps, union-find parents, cluster sizes, size histogram (inputs as for stats)
+  RegionWork regions;     // lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev: EDT stacks, counts, LUT
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -854,6 +856,22 @@ int laa_clusters_call(lm_engine* e, const char* fn, const void* vol, int dtype, 
   return 0;
 }
 
+// The region calls (lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev): the common checks, then the
+// engine's stream waits for the work queued on the caller's.
+int region_inputs(lm_engine* e, const char* fn, const uint8_t* d_mask, int n0, int n1, int n2) {
+  if (!e || !d_mask) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  CU(cudaSetDevice(e->device));
+  RC(check_device_ptr(e, fn, "d_mask", d_mask));
+  return 0;
+}
+int region_wait(lm_engine* e, void* stream) {
+  CU(cudaEventRecord(e->ev_in, static_cast<cudaStream_t>(stream)));
+  CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
+  e->launches = 0;
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -947,6 +965,7 @@ void lm_destroy(lm_engine* e) {
   e->post.release();
   e->stats.release();
   e->clusters.release();
+  e->regions.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1160,6 +1179,60 @@ int lm_laa_clusters_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_
   const cudaStream_t caller = static_cast<cudaStream_t>(stream);
   return laa_clusters_call(e, "lm_laa_clusters_dev", d_vol, dtype, d_mask, false, n0, n1, n2, threshold, connectivity, laa_voxels,
                            n_clusters, n_pairs, sizes, counts, max_pairs, &caller);
+}
+
+int lm_plane_label_counts_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int axis, int64_t* counts, void* stream) {
+  static const char* fn = "lm_plane_label_counts_dev";
+  RC(region_inputs(e, fn, d_mask, n0, n1, n2));
+  if (!counts) return fail(-1, "%s: NULL argument", fn);
+  if (axis < 0 || axis > 2) return fail(-1, "%s: axis %d is not 0, 1 or 2", fn, axis);
+  RC(region_wait(e, stream));
+  RC(plane_label_counts(e->regions, d_mask, n0, n1, n2, axis, counts, e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+int lm_surface_distance_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, const double* spacing, float* d_out,
+                            void* stream) {
+  static const char* fn = "lm_surface_distance_dev";
+  RC(region_inputs(e, fn, d_mask, n0, n1, n2));
+  if (!spacing || !d_out) return fail(-1, "%s: NULL argument", fn);
+  for (int k = 0; k < 3; ++k)
+    if (!(spacing[k] > 0.0 && spacing[k] < INFINITY)) return fail(-1, "%s: spacing[%d] = %g is not finite and positive", fn, k, spacing[k]);
+  if (n0 >= (1 << 30) || n1 >= (1 << 30) || n2 >= (1 << 30)) return fail(-1, "%s: (%d,%d,%d): an axis of 2^30 or more", fn, n0, n1, n2);
+  RC(check_device_ptr(e, fn, "d_out", d_out));
+  RC(region_wait(e, stream));
+  RC(surface_distance(e->regions, d_mask, n0, n1, n2, spacing, d_out, e->num_sms, e->st, &e->launches));
+  CU(cudaStreamSynchronize(e->st));
+  return 0;
+}
+
+int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, int n0, int n1, int n2, int axis,
+                      const float* bounds, int n_bounds, const uint8_t* lut, size_t lut_size, uint8_t* d_map, void* stream) {
+  static const char* fn = "lm_region_map_dev";
+  RC(region_inputs(e, fn, d_mask, n0, n1, n2));
+  if (!lut || !d_map || (d_dist && n_bounds > 0 && !bounds)) return fail(-1, "%s: NULL argument", fn);
+  size_t buckets;
+  if (d_dist) {
+    if (n_bounds < 0 || n_bounds > 254) return fail(-1, "%s: n_bounds %d not in [0,254]", fn, n_bounds);
+    for (int k = 0; k < n_bounds; ++k) {
+      if (!(bounds[k] > 0.0f && bounds[k] < INFINITY)) return fail(-1, "%s: bound %g is not finite and positive", fn, bounds[k]);
+      if (k > 0 && !(bounds[k] > bounds[k - 1])) return fail(-1, "%s: bounds are not strictly increasing", fn);
+    }
+    buckets = (size_t)n_bounds + 1;
+    RC(check_device_ptr(e, fn, "d_dist", d_dist));
+  } else {
+    if (axis < 0 || axis > 2) return fail(-1, "%s: axis %d is not 0, 1 or 2", fn, axis);
+    if (n_bounds != 0) return fail(-1, "%s: shell bounds without d_dist", fn);
+    buckets = (size_t)(axis == 0 ? n0 : (axis == 1 ? n1 : n2));
+  }
+  if (lut_size != buckets * 256) return fail(-1, "%s: lut_size %zu, expected %zu buckets x 256 = %zu", fn, lut_size, buckets, buckets * 256);
+  for (size_t b = 0; b < buckets; ++b)
+    if (lut[b * 256]) return fail(-1, "%s: lut[%zu][0] = %d, label 0 must map to 0", fn, b, (int)lut[b * 256]);
+  RC(check_device_ptr(e, fn, "d_map", d_map));
+  RC(region_wait(e, stream));
+  RC(region_map(e->regions, d_mask, d_dist, n0, n1, n2, d_dist ? -1 : axis, bounds, d_dist ? n_bounds : 0, lut, lut_size, d_map,
+                e->num_sms, e->st, &e->launches));
+  return 0;
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

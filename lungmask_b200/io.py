@@ -468,3 +468,37 @@ def save_clusters(path, clusters):
         lines.append(",".join(_csv_cell(getattr(r, k)) for k in ClusterRow.SUMMARY))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")
+
+
+def check_regions_path(path):
+    """Refuses, before any work is done, an output path save_regional_statistics cannot write."""
+    if not path.lower().endswith((".json", ".csv")):
+        raise SystemExit("unsupported regions output format (use .json or .csv): %s" % path)
+
+
+def save_regional_statistics(path, regions):
+    """Writes the RegionalStatistics of LMInferer.regional_statistics: .json (the parameters, one object per zone / shell
+    row with its statistics, and the per-plane profile of every row; NaN as null) or .csv (a header, then one line per
+    zone / shell row: label, name, region, index, region_name, first_plane, last_plane, depth_min_mm, depth_max_mm, then
+    the statistics columns of save_statistics; an empty cell where a value does not apply or is unknown)."""
+    check_regions_path(path)
+    if path.lower().endswith(".json"):
+        import json
+        with open(path, "w") as f:
+            json.dump(regions.to_dict(), f, indent=1, allow_nan=False)
+            f.write("\n")
+        return
+    stat = ["voxels", "nan_voxels", "volume_ml", "mean_hu", "std_hu", "min_hu", "max_hu"]
+    header = ["label", "name", "region", "index", "region_name", "first_plane", "last_plane", "depth_min_mm",
+              "depth_max_mm"] + stat + ["percentile_%g" % q for q in regions.percentiles] + \
+        ["fraction_below_%d" % t for t in regions.thresholds]
+    lines = [",".join(header)]
+    for r in regions.rows:
+        planes = r.planes if r.planes is not None else (None, None)
+        depth = r.depth_mm if r.depth_mm is not None else (None, None)
+        cells = [r.label, r.name, r.region, r.index, r.region_name, planes[0], planes[1], depth[0], depth[1]] + \
+            [getattr(r.stats, k) for k in stat] + [r.stats.percentile_hu[q] for q in regions.percentiles] + \
+            [r.stats.fraction_below[t] for t in regions.thresholds]
+        lines.append(",".join(_csv_cell(v) for v in cells))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")

@@ -384,6 +384,139 @@ class LMInferer:
         return cl.from_native(res, res["labels"] | set(range(1, self.engine.n_classes[0])), self.modelname, spacing, threshold,
                               connectivity, min_cluster_voxels)
 
+    def surface_distance(self, mask, spacing):
+        """The distance in mm from every voxel with mask > 0 to the nearest voxel with mask == 0 -> float32 of the mask's
+        shape: 0 outside the mask, +inf when the mask has no zero voxel.  The surface is that of the union of all labels,
+        so fissures between lobes are interior.  Voxels outside the array are not background (as in
+        scipy.ndimage.distance_transform_edt): a lung cut off by the first or last slice has no surface there.
+
+        `spacing`: the voxel size along each ARRAY axis, (s0, s1, s2) in mm, as scipy's `sampling` - for a Volume or
+        SimpleITK image that is GetSpacing()[::-1].  The exact Euclidean distance is computed in float64 on the GPU and
+        rounded once: np.float32(scipy.ndimage.distance_transform_edt(mask > 0, sampling=spacing)) bit for bit when the
+        squared distances are exact in float64 (dyadic spacings such as 0.703125 or 1.25), else within 1 float32 ulp.
+
+        `mask`: (S, H, W) uint8 or bool, numpy or a torch tensor.  A CUDA tensor on the engine's device is read in place
+        after the work queued on the current stream and the result is a float32 CUDA tensor there; a CPU tensor gives a
+        CPU tensor.  The mask is left unchanged."""
+        import torch
+        sp = tuple(float(s) for s in np.asarray(spacing, dtype=np.float64).reshape(-1))
+        if len(sp) != 3 or not all(np.isfinite(s) and s > 0 for s in sp):
+            raise ValueError("surface_distance: spacing must be 3 finite positive sizes (s0, s1, s2) in mm, got %s" % (spacing,))
+        m, back = self._region_mask(mask, "surface_distance")
+        out = torch.empty(tuple(m.shape), dtype=torch.float32, device=m.device)
+        self.engine.surface_distance_dev(m.data_ptr(), m.shape, sp, out.data_ptr(),
+                                         stream=torch.cuda.current_stream(m.device).cuda_stream)
+        return back(out)
+
+    def _region_mask(self, mask, what):
+        """(contiguous uint8 CUDA tensor on the engine's device, function turning a result tensor into the caller's type)."""
+        import torch
+        device = torch.device("cuda", self.engine.device)
+        if _is_tensor(mask):
+            if mask.is_cuda and mask.device.index != self.engine.device:
+                raise ValueError("%s: the mask tensor is on %s, the engine on cuda:%d" % (what, mask.device, self.engine.device))
+            kind = "cuda" if mask.is_cuda else "cpu"
+            m = mask.detach()
+        else:
+            kind, m = "numpy", np.asarray(mask)
+            if m.dtype not in (np.uint8, np.bool_):
+                raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, m.dtype))
+            with warnings.catch_warnings():   # a read-only array: the host tensor is only copied from
+                warnings.simplefilter("ignore", UserWarning)
+                m = torch.from_numpy(np.ascontiguousarray(m).view(np.uint8))
+        if m.dtype not in (torch.uint8, torch.bool):
+            raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, m.dtype))
+        if m.dim() != 3:
+            raise ValueError("%s: expected a (slices, H, W) mask, got shape %s" % (what, tuple(m.shape)))
+        m = m.contiguous()
+        if m.dtype == torch.bool:
+            m = m.view(torch.uint8)
+        m = m.to(device)
+        back = {"cuda": lambda t: t, "cpu": lambda t: t.cpu(), "numpy": lambda t: t.cpu().numpy()}[kind]
+        return m, back
+
+    def regional_statistics(self, image, mask, spacing=None, zones=3, zone_by="volume", shells_mm=(10.0,),
+                            percentiles=(15.0,), thresholds=(-950,)):
+        """Statistics of `image` under `mask` by craniocaudal zone and by depth below the lung surface ->
+        lungmask_b200.regions.RegionalStatistics.  The rows of `statistics` (every label value in the mask, every label
+        1..K-1 of the model, then "lung") are each split into `zones` craniocaudal zones and into the depth shells of
+        `shells_mm`; every zone or shell row holds the full statistics.LabelRow of its voxels (see `statistics`).
+
+        Zones are whole planes along the craniocaudal array axis: axis 0, superior at the high index, for numpy arrays
+        and tensors (LPS, as in `apply`); for a Volume or SimpleITK image the axis its orientation names S or I.  Zone 0
+        is the most superior; every row gets its own boundaries.  zone_by="volume" splits each row's planes at equal
+        shares of its voxels (a plane goes to the zone of the midpoint of its share), "height" at equal shares of its
+        first..last plane; see regions.zone_of_planes.  With 3 zones they are named upper / middle / lower.  Each zone row
+        reports its plane range in array indices, and the result holds every row's voxels per plane (the profile).
+
+        Shells: with shells_mm = (b_1, ..., b_m) strictly increasing in mm, shell j holds the voxels with
+        b_j <= depth < b_{j+1} (b_0 = 0, b_{m+1} = inf) where depth = `surface_distance` (float32, compared with the
+        bounds as float32).  Shell 0 is the rind.  Shells need the spacing; shells_mm=() skips them.
+
+        `image`, `mask` and `spacing` (x, y, z) mm as for `statistics`: numpy arrays (the image is uploaded once), a
+        Volume or SimpleITK image (which supplies the spacing), CPU tensors, or CUDA tensors on the engine's device read in
+        place after the work queued on the current stream.  The per-label region map gives each (label, zone) and
+        (label, shell) its own uint8 code, so labels x zones and labels x shells must stay at or below 255."""
+        from . import regions as rg
+        zones, zone_by, shells_mm, q, t = rg.check_arguments(zones, zone_by, shells_mm, percentiles, thresholds)
+        code = "LPS"
+        if not (isinstance(image, np.ndarray) or _is_tensor(image)):
+            if hasattr(image, "GetDirection"):
+                code = orient.orientation_from_direction(image.GetDirection())
+            if spacing is None and (hasattr(image, "spacing") or hasattr(image, "GetSpacing")):
+                spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
+        if spacing is not None:
+            spacing = tuple(float(s) for s in spacing)
+            if len(spacing) != 3:
+                raise ValueError("spacing must be (x, y, z), got %s" % (spacing,))
+        if shells_mm and spacing is None:
+            raise ValueError("regional_statistics: depth shells need the voxel spacing; pass spacing=(x, y, z) in mm, or "
+                             "shells_mm=() for zones only")
+        axis, superior_high = rg.craniocaudal_axis(code)
+        import torch
+        device = torch.device("cuda", self.engine.device)
+
+        def dev_call(v, dtype_code, m, stream):
+            shape = tuple(m.shape)
+            counts = self.engine.plane_label_counts_dev(m.data_ptr(), shape, axis, stream=stream)
+            present = [int(x) for x in np.flatnonzero(counts[:, 1:256].sum(axis=0)) + 1]
+            rg.check_code_budget(present, zones, "zones")
+            if shells_mm:
+                rg.check_code_budget(present, len(shells_mm) + 1, "shells")
+            label_zones = {l: rg.zone_of_planes(counts[:, l], zones, zone_by, superior_high) for l in present}
+            lung_zones = rg.zone_of_planes(counts[:, 256], zones, zone_by, superior_high)
+            region = torch.empty(shape, dtype=torch.uint8, device=m.device)
+
+            def stats_of(lut, **kw):
+                self.engine.region_map_dev(m.data_ptr(), shape, lut, region.data_ptr(), stream=stream, **kw)
+                return self.engine.label_stats_dev(v.data_ptr(), dtype_code, region.data_ptr(), shape, q, t, stream=stream)
+
+            lut, lung_lut = rg.zone_luts(present, label_zones, lung_zones, zones)
+            res = {"counts": counts, "present": present, "label_zones": label_zones, "lung_zones": lung_zones,
+                   "zone": stats_of(lut, axis=axis), "zone_lung": stats_of(lung_lut, axis=axis), "shell": None,
+                   "shell_lung": None}
+            if shells_mm:
+                dist = torch.empty(shape, dtype=torch.float32, device=m.device)
+                self.engine.surface_distance_dev(m.data_ptr(), shape, spacing[::-1], dist.data_ptr(), stream=stream)
+                lut, lung_lut = rg.shell_luts(present, len(shells_mm) + 1)
+                kw = dict(d_dist_ptr=dist.data_ptr(), bounds=shells_mm)
+                res["shell"], res["shell_lung"] = stats_of(lut, **kw), stats_of(lung_lut, **kw)
+            return res
+
+        def host_call(vol, m):
+            vol, dtype_code, m = _native._host_pair(vol, m, "regional_statistics")
+            with warnings.catch_warnings():   # read-only arrays: the host tensors are only copied from
+                warnings.simplefilter("ignore", UserWarning)
+                v = torch.from_numpy(vol).to(device)
+                m = torch.from_numpy(m).to(device)
+            return dev_call(v, dtype_code, m, torch.cuda.current_stream(device).cuda_stream)
+
+        res, spacing = self._per_label_call("regional_statistics", image, mask, spacing, host_call, dev_call)
+        labels = sorted(set(res["present"]) | set(range(1, self.engine.n_classes[0])))
+        return rg.build(labels, res["present"], self.modelname, spacing, res["counts"], axis, superior_high, zones, zone_by,
+                        shells_mm, q, t, res["label_zones"], res["lung_zones"], res["zone"], res["zone_lung"], res["shell"],
+                        res["shell_lung"])
+
     def _mask_labels(self, mask, stream):
         """The non-zero label values of a (S,H,W) uint8 CUDA mask tensor.  lm_label_stats_dev with the mask as its own uint8
         volume and no percentiles or thresholds: its count and histogram passes over the mask bytes."""

@@ -95,19 +95,22 @@ class LabelStatistics:
                 "thresholds": list(self.thresholds), "rows": [r.to_dict() for r in self.rows]}
 
 
+def row_from_native(res, r, label, name, voxel_ml, percentiles, thresholds):
+    """The LabelRow of row r of the arrays of _native.Engine.label_stats*; voxel_ml = the voxel volume in mm^3 or None."""
+    vox, nan = int(res["voxels"][r]), int(res["nan_voxels"][r])
+    n = vox - nan
+    m = res["moments"][r]
+    return LabelRow(
+        label=label, name=name, voxels=vox, nan_voxels=nan, volume_ml=vox * voxel_ml / 1000.0 if voxel_ml is not None else None,
+        mean_hu=float(m[0]), std_hu=float(m[1]), min_hu=float(m[2]), max_hu=float(m[3]),
+        percentile_hu={q: float(res["percentile"][r][k]) for k, q in enumerate(percentiles)},
+        fraction_below={t: (float(res["below_count"][r][k]) / n if n else float("nan")) for k, t in enumerate(thresholds)})
+
+
 def from_native(res, labels, modelname, spacing, percentiles, thresholds):
     """LabelStatistics from the 257-row arrays of _native.Engine.label_stats*: a row for every label in `labels`, then "lung"."""
     voxel_ml = float(np.prod(np.asarray(spacing, dtype=np.float64))) if spacing is not None else None
-    rows = []
-    for r in sorted(int(x) for x in labels) + [256]:
-        vox, nan = int(res["voxels"][r]), int(res["nan_voxels"][r])
-        n = vox - nan
-        m = res["moments"][r]
-        rows.append(LabelRow(
-            label=UNION if r == 256 else r, name=UNION if r == 256 else label_name(modelname, r), voxels=vox,
-            nan_voxels=nan, volume_ml=vox * voxel_ml / 1000.0 if voxel_ml is not None else None,
-            mean_hu=float(m[0]), std_hu=float(m[1]), min_hu=float(m[2]), max_hu=float(m[3]),
-            percentile_hu={q: float(res["percentile"][r][k]) for k, q in enumerate(percentiles)},
-            fraction_below={t: (float(res["below_count"][r][k]) / n if n else float("nan")) for k, t in enumerate(thresholds)}))
+    rows = [row_from_native(res, r, UNION if r == 256 else r, UNION if r == 256 else label_name(modelname, r), voxel_ml,
+                            percentiles, thresholds) for r in sorted(int(x) for x in labels) + [256]]
     return LabelStatistics(tuple(float(s) for s in spacing) if spacing is not None else None, tuple(percentiles),
                            tuple(thresholds), rows)
