@@ -154,9 +154,9 @@ LM_API int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol
 /* Per-label volume and HU statistics of a volume and its label mask (no counterpart in the reference; DESIGN §4.6): what
  * lung-CT tools report from a lungmask result - each lung's or lobe's voxel count, mean / std / min / max HU, percentiles
  * (Perc15) and the fraction of voxels below thresholds (LAA-950).
- *   vol      (n0,n1,n2) of element type `dtype` (every LM_DTYPE_* code; bool as LM_DTYPE_U8).  Values are read as they
+ *   d_vol    (n0,n1,n2) of element type `dtype` (every LM_DTYPE_* code; bool as LM_DTYPE_U8).  Values are read as they
  *            are: not clipped; float16 / bfloat16 are widened to float32, every value statistic is computed in float64.
- *   mask     (n0,n1,n2) uint8, voxel i paired with voxel i of vol (orientation does not matter).
+ *   d_mask   (n0,n1,n2) uint8, voxel i paired with voxel i of d_vol (orientation does not matter).
  *   percentiles  n_q values q in [0, 100]; thresholds  n_t integers t in [-1024, 3072].
  * Results: 257 rows, row l = the voxels with mask == l (row 0: voxels only), row 256 = the union mask > 0.  NaN values
  * are counted in nan_voxels and excluded from everything else; n = voxels - nan_voxels.
@@ -164,14 +164,11 @@ LM_API int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol
  *   moments [257][4]       mean, std (population), min, max of the row's values; NaN when n = 0
  *   percentile [257][n_q]  bit-identical to numpy.percentile(values.astype(float64), q) (method "linear"); NaN when n = 0
  *   below_count [257][n_t] count(value < t); 0 when n = 0
- * lm_label_stats takes host arrays (uploaded into engine buffers); lm_label_stats_dev takes device memory of the engine's
- * device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev.  Both return after the engine's stream
- * has synchronised; the inputs are never written. */
+ * d_vol and d_mask are device memory of the engine's device; `stream` is the caller's cudaStream_t, with the event-wait
+ * rule of lm_apply_dev.  Every argument is checked before any kernel runs; the call returns after the engine's stream has
+ * synchronised, and the inputs are never written. */
 #define LM_STATS_MAX_PERCENTILES 64
 #define LM_STATS_MAX_THRESHOLDS 4097
-LM_API int lm_label_stats(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2,
-                          const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
-                          int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count);
 LM_API int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
                               const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
                               int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count, void* stream);
@@ -179,7 +176,7 @@ LM_API int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const 
 /* Size distributions of the connected clusters of low-attenuation (LAA) voxels per label (no counterpart in the reference;
  * DESIGN §4.7): whether a lobe's LAA-950 is many small holes or a few large bullae (the power-law exponent D of
  * Mishima et al., PNAS 1999, is computed from these pairs by LMInferer.laa_clusters).
- *   vol, mask     as lm_label_stats; a voxel is LAA when mask > 0 and value < threshold, compared in the volume's type
+ *   d_vol, d_mask as lm_label_stats_dev; a voxel is LAA when mask > 0 and value < threshold, compared in the volume's type
  *                 (integers unclipped, float16 / bfloat16 widened to float32; NaN is never LAA).
  *   threshold     integer HU in [-1024, 3072];  connectivity  4 (faces within a slice, per-slice 2-D clusters), 6 (faces)
  *                 or 26 (full).  Fewer than 2^32 voxels.
@@ -190,11 +187,8 @@ LM_API int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const 
  *   sizes, counts       the (size, count) pairs, ascending by size within a row, rows concatenated in row order
  *                       (sum of n_pairs entries).  max_pairs >= lm_laa_max_pairs(n0*n1*n2), which bounds that sum
  *                       (a row of V LAA voxels has at most sqrt(2V) distinct sizes, the rows hold at most 2n voxels).
- * lm_laa_clusters takes host arrays, lm_laa_clusters_dev device memory and the caller's stream, as lm_label_stats*. */
+ * Device memory, the caller's stream, the argument checks and the return as for lm_label_stats_dev. */
 LM_API size_t lm_laa_max_pairs(size_t n_voxels);   /* 32 * ceil(sqrt(n_voxels)) + 256 */
-LM_API int lm_laa_clusters(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2, int threshold,
-                           int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs, int64_t* sizes,
-                           int64_t* counts, size_t max_pairs);
 LM_API int lm_laa_clusters_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
                                int threshold, int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs,
                                int64_t* sizes, int64_t* counts, size_t max_pairs, void* stream);

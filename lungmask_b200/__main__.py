@@ -12,8 +12,8 @@ import argparse
 import os
 import sys
 
-from .io import (check_clusters_path, check_probabilities_path, check_regions_path, check_statistics_path, load_input_image,
-                 save_clusters, save_mask, save_probabilities, save_regional_statistics, save_statistics)
+from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_mask, save_probabilities,
+                 save_regional_statistics, save_statistics)
 from .logger import logger
 from .mask import LMInferer
 
@@ -67,16 +67,16 @@ def main(argv=None):
             sys.exit("--probabilities: the LTRCLobes_R231 fusion has no class probabilities; use LTRCLobes or R231")
         check_probabilities_path(args.probabilities)
     if args.statistics is not None:
-        check_statistics_path(args.statistics)
+        check_table_path(args.statistics, "statistics")
     if args.clusters is not None:
-        check_clusters_path(args.clusters)
+        check_table_path(args.clusters, "clusters")
         from .clusters import check_arguments
         try:
             check_arguments(args.clusters_threshold, args.clusters_connectivity, 1)
         except ValueError as ex:
             sys.exit("--clusters-threshold: %s" % ex)
     if args.regions is not None:
-        check_regions_path(args.regions)
+        check_table_path(args.regions, "regions")
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)

@@ -12,11 +12,6 @@ FLAG_NO_POSTPROCESS = 1
 DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2   # LM_DTYPE_* of lm_apply_volume_probs
 DTYPE_U8, DTYPE_I8, DTYPE_I32, DTYPE_I64, DTYPE_F16, DTYPE_BF16 = 3, 4, 5, 6, 7, 8   # lm_apply_dev only (U8 also bool)
 
-# numpy dtype -> LM_DTYPE_* of lm_label_stats (host arrays)
-_HOST_DTYPE_CODES = {np.dtype(bool): DTYPE_U8, np.dtype(np.uint8): DTYPE_U8, np.dtype(np.int8): DTYPE_I8,
-                     np.dtype(np.int16): DTYPE_I16, np.dtype(np.int32): DTYPE_I32, np.dtype(np.int64): DTYPE_I64,
-                     np.dtype(np.float16): DTYPE_F16, np.dtype(np.float32): DTYPE_F32, np.dtype(np.float64): DTYPE_F64}
-
 _lib = None
 
 
@@ -52,10 +47,8 @@ def lib():
         "lm_apply_volume_oriented": ([vp, i32, i32, i16p, i32, i32, i32, vp, vp, i32, u8p], i32),
         "lm_apply_volume_probs": ([vp, i32, vp, i32, i32, i32, i32, vp, vp, i32, u8p, f32p], i32),
         "lm_apply_dev": ([vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, i32, u8p, f32p, vp], i32),
-        "lm_label_stats": ([vp, vp, i32, u8p, i32, i32, i32, vp, i32, vp, i32, vp, vp, vp, vp, vp], i32),
         "lm_label_stats_dev": ([vp, vp, i32, u8p, i32, i32, i32, vp, i32, vp, i32, vp, vp, vp, vp, vp, vp], i32),
         "lm_laa_max_pairs": ([C.c_size_t], C.c_size_t),
-        "lm_laa_clusters": ([vp, vp, i32, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t], i32),
         "lm_laa_clusters_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, C.c_size_t, vp], i32),
         "lm_plane_label_counts_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
         "lm_surface_distance_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp], i32),
@@ -89,7 +82,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -126,24 +119,6 @@ def _as(a, dtype, ndim=None):
     if ndim is not None and a.ndim != ndim:
         raise ValueError("expected %d-d array, got shape %s" % (ndim, a.shape))
     return a
-
-
-def _host_pair(vol, mask, fn):
-    """The (volume, LM_DTYPE_* code, mask) of a per-label call on host arrays: C-contiguous, bool viewed as uint8,
-    uint16 / uint32 volumes widened to int32 / int64 without loss."""
-    vol = np.asarray(vol)
-    if vol.dtype in (np.uint16, np.uint32):
-        vol = vol.astype(np.int32 if vol.dtype == np.uint16 else np.int64)
-    if vol.dtype not in _HOST_DTYPE_CODES:
-        raise TypeError("%s: volume dtype %s is not supported" % (fn, vol.dtype))
-    code = _HOST_DTYPE_CODES[vol.dtype]
-    vol = np.ascontiguousarray(vol.view(np.uint8) if vol.dtype == bool else vol)
-    mask = np.ascontiguousarray(np.asarray(mask).view(np.uint8) if np.asarray(mask).dtype == bool else mask)
-    if mask.dtype != np.uint8:
-        raise TypeError("%s: the mask must be uint8 or bool, got %s" % (fn, mask.dtype))
-    if vol.ndim != 3 or mask.shape != vol.shape:
-        raise ValueError("%s: expected (S,H,W) volume and mask of one shape, got %s and %s" % (fn, vol.shape, mask.shape))
-    return vol, code, mask
 
 
 class Engine:
@@ -283,62 +258,38 @@ class Engine:
                                   0 if postprocess else FLAG_NO_POSTPROCESS, C.c_void_p(d_out_ptr),
                                   C.c_void_p(d_probs_ptr) if d_probs_ptr else None, C.c_void_p(int(stream)) if stream else None))
 
-    # ---- per-label statistics (lm_label_stats*)
-    def label_stats(self, vol, mask, percentiles=(15.0,), thresholds=(-950,)):
-        """lm_label_stats on host arrays: `vol` (S,H,W) of any dtype with an LM_DTYPE_* code (bool, uint8, int8, int16,
-        int32, int64, float16, float32, float64; uint16 / uint32 are widened to int32 / int64 without loss), `mask` (S,H,W)
-        uint8 or bool.  -> dict of the 257-row arrays (see label_stats_dev)."""
-        vol, code, mask = _host_pair(vol, mask, "label_stats")
-        return self._label_stats(lambda *a: lib().lm_label_stats(self._h, _ptr(vol), code, _ptr(mask), *vol.shape, *a),
-                                 percentiles, thresholds)
-
+    # ---- per-label statistics (lm_label_stats_dev)
     def label_stats_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, percentiles=(15.0,), thresholds=(-950,), stream=0):
         """lm_label_stats_dev on device memory of this engine's device (`stream` as for apply_dev) -> dict of numpy arrays
         over 257 rows (row l = label l, row 256 = the union mask > 0): "voxels", "nan_voxels" (int64), "moments" (257, 4)
         mean / std / min / max, "percentile" (257, n_q), "below_count" (257, n_t) int64."""
         n0, n1, n2 = (int(x) for x in shape)
-        return self._label_stats(lambda *a: lib().lm_label_stats_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code),
-                                                                     C.c_void_p(d_mask_ptr), n0, n1, n2, *a,
-                                                                     C.c_void_p(int(stream)) if stream else None),
-                                 percentiles, thresholds)
-
-    @staticmethod
-    def _label_stats(call, percentiles, thresholds):
         q = np.ascontiguousarray(percentiles, dtype=np.float64).reshape(-1)
         t = np.ascontiguousarray(thresholds, dtype=np.int32).reshape(-1)
         res = {"voxels": np.zeros(257, np.int64), "nan_voxels": np.zeros(257, np.int64),
                "moments": np.zeros((257, 4), np.float64), "percentile": np.zeros((257, max(q.size, 1)), np.float64),
                "below_count": np.zeros((257, max(t.size, 1)), np.int64)}
-        _check(call(_ptr(q), q.size, _ptr(t), t.size, _ptr(res["voxels"]), _ptr(res["nan_voxels"]), _ptr(res["moments"]),
-                    _ptr(res["percentile"]), _ptr(res["below_count"])))
+        _check(lib().lm_label_stats_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), C.c_void_p(d_mask_ptr), n0, n1, n2,
+                                        _ptr(q), q.size, _ptr(t), t.size, _ptr(res["voxels"]), _ptr(res["nan_voxels"]),
+                                        _ptr(res["moments"]), _ptr(res["percentile"]), _ptr(res["below_count"]),
+                                        C.c_void_p(int(stream)) if stream else None))
         res["percentile"] = res["percentile"][:, :q.size]
         res["below_count"] = res["below_count"][:, :t.size]
         return res
 
-    # ---- LAA cluster size distributions (lm_laa_clusters*)
-    def laa_clusters(self, vol, mask, threshold=-950, connectivity=6):
-        """lm_laa_clusters on host arrays (`vol` and `mask` as for label_stats) -> dict (see laa_clusters_dev)."""
-        vol, code, mask = _host_pair(vol, mask, "laa_clusters")
-        return self._laa_clusters(lambda *a: lib().lm_laa_clusters(self._h, _ptr(vol), code, _ptr(mask), *vol.shape, *a),
-                                  vol.size, threshold, connectivity)
-
+    # ---- LAA cluster size distributions (lm_laa_clusters_dev)
     def laa_clusters_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, threshold=-950, connectivity=6, stream=0):
         """lm_laa_clusters_dev on device memory of this engine's device (`stream` as for apply_dev) -> dict over 257 rows
         (row l = label l, row 256 = all LAA voxels): "laa_voxels", "n_clusters", "n_pairs" (int64 [257]) and "sizes",
         "counts" (int64, the rows' (size, count) pairs concatenated; row r's are [offsets[r], offsets[r + 1])), "offsets"."""
         n0, n1, n2 = (int(x) for x in shape)
-        return self._laa_clusters(lambda *a: lib().lm_laa_clusters_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code),
-                                                                       C.c_void_p(d_mask_ptr), n0, n1, n2, *a,
-                                                                       C.c_void_p(int(stream)) if stream else None),
-                                  max(n0, 0) * max(n1, 0) * max(n2, 0), threshold, connectivity)
-
-    @staticmethod
-    def _laa_clusters(call, n_voxels, threshold, connectivity):
-        cap = int(lib().lm_laa_max_pairs(n_voxels))
+        cap = int(lib().lm_laa_max_pairs(max(n0, 0) * max(n1, 0) * max(n2, 0)))
         res = {k: np.zeros(257, np.int64) for k in ("laa_voxels", "n_clusters", "n_pairs")}
         sizes, counts = np.zeros(cap, np.int64), np.zeros(cap, np.int64)
-        _check(call(int(threshold), int(connectivity), _ptr(res["laa_voxels"]), _ptr(res["n_clusters"]), _ptr(res["n_pairs"]),
-                    _ptr(sizes), _ptr(counts), cap))
+        _check(lib().lm_laa_clusters_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), C.c_void_p(d_mask_ptr), n0, n1, n2,
+                                         int(threshold), int(connectivity), _ptr(res["laa_voxels"]), _ptr(res["n_clusters"]),
+                                         _ptr(res["n_pairs"]), _ptr(sizes), _ptr(counts), cap,
+                                         C.c_void_p(int(stream)) if stream else None))
         res["offsets"] = np.concatenate([[0], np.cumsum(res["n_pairs"])])
         total = int(res["offsets"][-1])
         res["sizes"], res["counts"] = sizes[:total].copy(), counts[:total].copy()

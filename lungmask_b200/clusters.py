@@ -1,4 +1,4 @@
-"""Size distributions of low-attenuation clusters: the result of LMInferer.laa_clusters (lm_laa_clusters, DESIGN §4.7).
+"""Size distributions of low-attenuation clusters: the result of LMInferer.laa_clusters (lm_laa_clusters_dev, DESIGN §4.7).
 
 A low-attenuation (LAA) voxel lies inside the mask and below the threshold (-950 HU by default).  Its clusters are the
 connected components of the LAA voxels: per label (a cluster never crosses a label boundary) and for the whole lung,

@@ -1,4 +1,4 @@
-// Size distributions of the connected clusters of low-attenuation (LAA) voxels per label (lm_laa_clusters*, DESIGN §4.7).
+// Size distributions of the connected clusters of low-attenuation (LAA) voxels per label (lm_laa_clusters_dev, DESIGN §4.7).
 //
 // Passes, each grid-stride over the volume:
 //   1. map        reads the mask as 16-byte vectors and the value only under a non-zero label; writes map_l = laa ? mask : 0

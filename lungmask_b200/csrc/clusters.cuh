@@ -12,7 +12,7 @@ constexpr int kClusterDense = 4096;    // cluster sizes below this are counted i
 // The pair-count bound of lm_laa_max_pairs: 32 * ceil(sqrt(n)) + 256.
 size_t laa_max_pairs(size_t n_voxels);
 
-// Where laa_clusters writes its results (host memory, see lm_laa_clusters in the header).
+// Where laa_clusters writes its results (host memory, see lm_laa_clusters_dev in the header).
 struct LaaClustersOut {
   int64_t* laa_voxels;   // [257]
   int64_t* n_clusters;   // [257]

@@ -7,6 +7,7 @@
 #include <stdlib.h>
 #include <stdio.h>
 #include <string.h>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -191,8 +192,8 @@ struct lm_engine {
   DevBuf<float> d_scores, d_norm;   // d_scores: one wave of lm_forward's tap, or a whole volume of scores for the probabilities
   DevBuf<uint32_t> d_scratch;
   PostScratch post;
-  LabelStatsWork stats;   // lm_label_stats*: counts, histograms and selection state (a host call's volume and mask go to d_upload)
-  ClusterWork clusters;   // lm_laa_clusters*: LAA maps, union-find parents, cluster sizes, size histogram (inputs as for stats)
+  LabelStatsWork stats;   // lm_label_stats_dev: counts, histograms and selection state
+  ClusterWork clusters;   // lm_laa_clusters_dev: LAA maps, union-find parents, cluster sizes, size histogram
   RegionWork regions;     // lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev: EDT stacks, counts, LUT
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
@@ -790,82 +791,20 @@ int run_volume(lm_engine* e, VolumeJob j, const void* h_vol, uint8_t* h_out, flo
   return 0;
 }
 
-// The (volume, mask) pair of a per-label call on the engine's stream.  host: *vol and *mask are host arrays, uploaded into
-// d_upload (the pointers then point there); otherwise they are the caller's device memory, checked, and the engine's
-// stream waits for the work queued on *caller.
-int volume_mask_inputs(lm_engine* e, const char* fn, const void** vol, int dtype, const uint8_t** mask, bool host, size_t n,
-                       const cudaStream_t* caller) {
+// A device pointer argument of an analysis call, with its name for the messages.
+struct DevArg {
+  const char* name;
+  const void* p;
+};
+
+// The start of an analysis call (lm_label_stats_dev, lm_laa_clusters_dev, lm_plane_label_counts_dev,
+// lm_surface_distance_dev, lm_region_map_dev), once its other arguments are checked: each device pointer must be memory
+// of the engine's device (a NULL one is an optional input the call does not use), the engine's stream waits for the work
+// queued on the caller's, and the launch count restarts.
+int analysis_inputs(lm_engine* e, const char* fn, void* stream, std::initializer_list<DevArg> ptrs) {
   CU(cudaSetDevice(e->device));
-  const size_t vol_bytes = n * dtype_bytes(dtype), mask_at = (vol_bytes + 255) & ~(size_t)255;
-  if (host) {
-    RC(e->d_upload.reserve(mask_at + n));
-    CU(cudaMemcpyAsync(e->d_upload.p, *vol, vol_bytes, cudaMemcpyHostToDevice, e->st));
-    CU(cudaMemcpyAsync(e->d_upload.p + mask_at, *mask, n, cudaMemcpyHostToDevice, e->st));
-    *vol = e->d_upload.p;
-    *mask = e->d_upload.p + mask_at;
-  } else {
-    RC(check_device_ptr(e, fn, "d_vol", *vol));
-    RC(check_device_ptr(e, fn, "d_mask", *mask));
-    CU(cudaEventRecord(e->ev_in, *caller));
-    CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
-  }
-  return 0;
-}
-
-// lm_label_stats / lm_label_stats_dev: every argument is checked before any kernel runs.  host false: vol / mask are the
-// caller's device memory (and `caller` its stream); otherwise both are uploaded into d_upload.
-int label_stats_call(lm_engine* e, const char* fn, const void* vol, int dtype, const uint8_t* mask, bool host, int n0, int n1,
-                     int n2, const double* q, int n_q, const int* t, int n_t, int64_t* voxels, int64_t* nan_voxels,
-                     double* moments, double* percentile, int64_t* below, const cudaStream_t* caller) {
-  if (!e || !vol || !mask || !voxels || !nan_voxels || !moments || (n_q > 0 && (!q || !percentile)) || (n_t > 0 && (!t || !below)))
-    return fail(-1, "%s: NULL argument", fn);
-  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
-  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
-  if (n_q < 0 || n_q > LM_STATS_MAX_PERCENTILES) return fail(-1, "%s: n_q %d not in [0,%d]", fn, n_q, LM_STATS_MAX_PERCENTILES);
-  if (n_t < 0 || n_t > LM_STATS_MAX_THRESHOLDS) return fail(-1, "%s: n_t %d not in [0,%d]", fn, n_t, LM_STATS_MAX_THRESHOLDS);
-  for (int k = 0; k < n_q; ++k)
-    if (!(q[k] >= 0.0 && q[k] <= 100.0)) return fail(-1, "%s: percentile %g not in [0,100]", fn, q[k]);
-  for (int k = 0; k < n_t; ++k)
-    if (t[k] < -1024 || t[k] > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, t[k]);
-  const size_t n = (size_t)n0 * n1 * n2;
-  RC(volume_mask_inputs(e, fn, &vol, dtype, &mask, host, n, caller));
-  e->launches = 0;
-  const LabelStatsOut out{voxels, nan_voxels, moments, percentile, below};
-  RC(label_stats(e->stats, vol, dtype, mask, n, q, n_q, t, n_t, out, e->num_sms, e->st, &e->launches));
-  return 0;
-}
-
-// lm_laa_clusters / lm_laa_clusters_dev: every argument is checked before any kernel runs; the inputs as label_stats_call.
-int laa_clusters_call(lm_engine* e, const char* fn, const void* vol, int dtype, const uint8_t* mask, bool host, int n0, int n1,
-                      int n2, int threshold, int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs,
-                      int64_t* sizes, int64_t* counts, size_t max_pairs, const cudaStream_t* caller) {
-  if (!e || !vol || !mask || !laa_voxels || !n_clusters || !n_pairs || !sizes || !counts) return fail(-1, "%s: NULL argument", fn);
-  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
-  const size_t n = (size_t)n0 * n1 * n2;
-  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the labelling takes fewer than 2^32", fn, n);
-  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
-  if (threshold < -1024 || threshold > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, threshold);
-  if (connectivity != 4 && connectivity != 6 && connectivity != 26)
-    return fail(-1, "%s: connectivity %d is not 4, 6 or 26", fn, connectivity);
-  if (max_pairs < laa_max_pairs(n))
-    return fail(-1, "%s: max_pairs %zu below lm_laa_max_pairs(%zu) = %zu", fn, max_pairs, n, laa_max_pairs(n));
-  RC(volume_mask_inputs(e, fn, &vol, dtype, &mask, host, n, caller));
-  e->launches = 0;
-  const LaaClustersOut out{laa_voxels, n_clusters, n_pairs, sizes, counts, max_pairs};
-  RC(laa_clusters(e->clusters, vol, dtype, mask, n0, n1, n2, threshold, connectivity, out, e->num_sms, e->st, &e->launches));
-  return 0;
-}
-
-// The region calls (lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev): the common checks, then the
-// engine's stream waits for the work queued on the caller's.
-int region_inputs(lm_engine* e, const char* fn, const uint8_t* d_mask, int n0, int n1, int n2) {
-  if (!e || !d_mask) return fail(-1, "%s: NULL argument", fn);
-  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
-  CU(cudaSetDevice(e->device));
-  RC(check_device_ptr(e, fn, "d_mask", d_mask));
-  return 0;
-}
-int region_wait(lm_engine* e, void* stream) {
+  for (const DevArg& a : ptrs)
+    if (a.p) RC(check_device_ptr(e, fn, a.name, a.p));
   CU(cudaEventRecord(e->ev_in, static_cast<cudaStream_t>(stream)));
   CU(cudaStreamWaitEvent(e->st, e->ev_in, 0));
   e->launches = 0;
@@ -1149,44 +1088,58 @@ int lm_apply_dev(lm_engine* e, int slot, int slot_fill, const void* d_vol, int d
   return run_volume(e, j, nullptr, nullptr, nullptr, &caller);
 }
 
-int lm_label_stats(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2,
-                   const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels, int64_t* nan_voxels,
-                   double* moments, double* percentile, int64_t* below_count) {
-  return label_stats_call(e, "lm_label_stats", vol, dtype, mask, true, n0, n1, n2, percentiles, n_q, thresholds, n_t, voxels,
-                          nan_voxels, moments, percentile, below_count, nullptr);
-}
-
 int lm_label_stats_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
                        const double* percentiles, int n_q, const int* thresholds, int n_t, int64_t* voxels,
                        int64_t* nan_voxels, double* moments, double* percentile, int64_t* below_count, void* stream) {
-  const cudaStream_t caller = static_cast<cudaStream_t>(stream);
-  return label_stats_call(e, "lm_label_stats_dev", d_vol, dtype, d_mask, false, n0, n1, n2, percentiles, n_q, thresholds, n_t,
-                          voxels, nan_voxels, moments, percentile, below_count, &caller);
+  static const char* fn = "lm_label_stats_dev";
+  const double* q = percentiles;
+  const int* t = thresholds;
+  if (!e || !d_vol || !d_mask || !voxels || !nan_voxels || !moments || (n_q > 0 && (!q || !percentile)) ||
+      (n_t > 0 && (!t || !below_count)))
+    return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (n_q < 0 || n_q > LM_STATS_MAX_PERCENTILES) return fail(-1, "%s: n_q %d not in [0,%d]", fn, n_q, LM_STATS_MAX_PERCENTILES);
+  if (n_t < 0 || n_t > LM_STATS_MAX_THRESHOLDS) return fail(-1, "%s: n_t %d not in [0,%d]", fn, n_t, LM_STATS_MAX_THRESHOLDS);
+  for (int k = 0; k < n_q; ++k)
+    if (!(q[k] >= 0.0 && q[k] <= 100.0)) return fail(-1, "%s: percentile %g not in [0,100]", fn, q[k]);
+  for (int k = 0; k < n_t; ++k)
+    if (t[k] < -1024 || t[k] > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, t[k]);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_mask", d_mask}}));
+  const LabelStatsOut out{voxels, nan_voxels, moments, percentile, below_count};
+  RC(label_stats(e->stats, d_vol, dtype, d_mask, (size_t)n0 * n1 * n2, q, n_q, t, n_t, out, e->num_sms, e->st, &e->launches));
+  return 0;
 }
 
 size_t lm_laa_max_pairs(size_t n_voxels) { return laa_max_pairs(n_voxels); }
 
-int lm_laa_clusters(lm_engine* e, const void* vol, int dtype, const uint8_t* mask, int n0, int n1, int n2, int threshold,
-                    int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs, int64_t* sizes, int64_t* counts,
-                    size_t max_pairs) {
-  return laa_clusters_call(e, "lm_laa_clusters", vol, dtype, mask, true, n0, n1, n2, threshold, connectivity, laa_voxels, n_clusters,
-                           n_pairs, sizes, counts, max_pairs, nullptr);
-}
-
 int lm_laa_clusters_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2, int threshold,
                         int connectivity, int64_t* laa_voxels, int64_t* n_clusters, int64_t* n_pairs, int64_t* sizes,
                         int64_t* counts, size_t max_pairs, void* stream) {
-  const cudaStream_t caller = static_cast<cudaStream_t>(stream);
-  return laa_clusters_call(e, "lm_laa_clusters_dev", d_vol, dtype, d_mask, false, n0, n1, n2, threshold, connectivity, laa_voxels,
-                           n_clusters, n_pairs, sizes, counts, max_pairs, &caller);
+  static const char* fn = "lm_laa_clusters_dev";
+  if (!e || !d_vol || !d_mask || !laa_voxels || !n_clusters || !n_pairs || !sizes || !counts)
+    return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the labelling takes fewer than 2^32", fn, n);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (threshold < -1024 || threshold > 3072) return fail(-1, "%s: threshold %d not in [-1024,3072]", fn, threshold);
+  if (connectivity != 4 && connectivity != 6 && connectivity != 26)
+    return fail(-1, "%s: connectivity %d is not 4, 6 or 26", fn, connectivity);
+  if (max_pairs < laa_max_pairs(n))
+    return fail(-1, "%s: max_pairs %zu below lm_laa_max_pairs(%zu) = %zu", fn, max_pairs, n, laa_max_pairs(n));
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_mask", d_mask}}));
+  const LaaClustersOut out{laa_voxels, n_clusters, n_pairs, sizes, counts, max_pairs};
+  RC(laa_clusters(e->clusters, d_vol, dtype, d_mask, n0, n1, n2, threshold, connectivity, out, e->num_sms, e->st, &e->launches));
+  return 0;
 }
 
 int lm_plane_label_counts_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int axis, int64_t* counts, void* stream) {
   static const char* fn = "lm_plane_label_counts_dev";
-  RC(region_inputs(e, fn, d_mask, n0, n1, n2));
-  if (!counts) return fail(-1, "%s: NULL argument", fn);
+  if (!e || !d_mask || !counts) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
   if (axis < 0 || axis > 2) return fail(-1, "%s: axis %d is not 0, 1 or 2", fn, axis);
-  RC(region_wait(e, stream));
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}}));
   RC(plane_label_counts(e->regions, d_mask, n0, n1, n2, axis, counts, e->num_sms, e->st, &e->launches));
   return 0;
 }
@@ -1194,13 +1147,12 @@ int lm_plane_label_counts_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n
 int lm_surface_distance_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, const double* spacing, float* d_out,
                             void* stream) {
   static const char* fn = "lm_surface_distance_dev";
-  RC(region_inputs(e, fn, d_mask, n0, n1, n2));
-  if (!spacing || !d_out) return fail(-1, "%s: NULL argument", fn);
+  if (!e || !d_mask || !spacing || !d_out) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
   for (int k = 0; k < 3; ++k)
     if (!(spacing[k] > 0.0 && spacing[k] < INFINITY)) return fail(-1, "%s: spacing[%d] = %g is not finite and positive", fn, k, spacing[k]);
   if (n0 >= (1 << 30) || n1 >= (1 << 30) || n2 >= (1 << 30)) return fail(-1, "%s: (%d,%d,%d): an axis of 2^30 or more", fn, n0, n1, n2);
-  RC(check_device_ptr(e, fn, "d_out", d_out));
-  RC(region_wait(e, stream));
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}, {"d_out", d_out}}));
   RC(surface_distance(e->regions, d_mask, n0, n1, n2, spacing, d_out, e->num_sms, e->st, &e->launches));
   CU(cudaStreamSynchronize(e->st));
   return 0;
@@ -1209,8 +1161,8 @@ int lm_surface_distance_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1,
 int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, int n0, int n1, int n2, int axis,
                       const float* bounds, int n_bounds, const uint8_t* lut, size_t lut_size, uint8_t* d_map, void* stream) {
   static const char* fn = "lm_region_map_dev";
-  RC(region_inputs(e, fn, d_mask, n0, n1, n2));
-  if (!lut || !d_map || (d_dist && n_bounds > 0 && !bounds)) return fail(-1, "%s: NULL argument", fn);
+  if (!e || !d_mask || !lut || !d_map || (d_dist && n_bounds > 0 && !bounds)) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
   size_t buckets;
   if (d_dist) {
     if (n_bounds < 0 || n_bounds > 254) return fail(-1, "%s: n_bounds %d not in [0,254]", fn, n_bounds);
@@ -1219,7 +1171,6 @@ int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, 
       if (k > 0 && !(bounds[k] > bounds[k - 1])) return fail(-1, "%s: bounds are not strictly increasing", fn);
     }
     buckets = (size_t)n_bounds + 1;
-    RC(check_device_ptr(e, fn, "d_dist", d_dist));
   } else {
     if (axis < 0 || axis > 2) return fail(-1, "%s: axis %d is not 0, 1 or 2", fn, axis);
     if (n_bounds != 0) return fail(-1, "%s: shell bounds without d_dist", fn);
@@ -1228,8 +1179,7 @@ int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, 
   if (lut_size != buckets * 256) return fail(-1, "%s: lut_size %zu, expected %zu buckets x 256 = %zu", fn, lut_size, buckets, buckets * 256);
   for (size_t b = 0; b < buckets; ++b)
     if (lut[b * 256]) return fail(-1, "%s: lut[%zu][0] = %d, label 0 must map to 0", fn, b, (int)lut[b * 256]);
-  RC(check_device_ptr(e, fn, "d_map", d_map));
-  RC(region_wait(e, stream));
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}, {"d_dist", d_dist}, {"d_map", d_map}}));
   RC(region_map(e->regions, d_mask, d_dist, n0, n1, n2, d_dist ? -1 : axis, bounds, d_dist ? n_bounds : 0, lut, lut_size, d_map,
                 e->num_sms, e->st, &e->launches));
   return 0;

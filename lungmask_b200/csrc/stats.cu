@@ -1,4 +1,4 @@
-// Per-label volume and HU statistics (lm_label_stats / lm_label_stats_dev, DESIGN §4.6).
+// Per-label volume and HU statistics (lm_label_stats_dev, DESIGN §4.6).
 //
 // Passes over the (volume, mask) pair, each grid-stride over 16-voxel chunks (one 16-byte mask vector per thread); the
 // value of a voxel is read only where the mask is non-zero:

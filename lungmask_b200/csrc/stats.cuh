@@ -9,7 +9,7 @@ namespace lm {
 constexpr int kStatsBins = 4098;   // [under (< -1024), -1024, ..., 3071, over (>= 3072)]: 1-HU bins of floor(value)
 constexpr int kStatsRows = 257;    // rows 0..255 = label values, row 256 = the union (mask > 0)
 
-// Where label_stats writes its results (host memory, kStatsRows rows each, see lm_label_stats in the header).
+// Where label_stats writes its results (host memory, kStatsRows rows each, see lm_label_stats_dev in the header).
 struct LabelStatsOut {
   int64_t* voxels;       // [257]
   int64_t* nan_voxels;   // [257]

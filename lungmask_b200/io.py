@@ -407,10 +407,19 @@ def save_probabilities(path, probs, like=None):
         _write_nifti(path, probs, like)
 
 
-def check_statistics_path(path):
-    """Refuses, before any work is done, an output path save_statistics cannot write."""
+def check_table_path(path, kind):
+    """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
+    ("clusters") or save_regional_statistics ("regions") cannot write."""
     if not path.lower().endswith((".json", ".csv")):
-        raise SystemExit("unsupported statistics output format (use .json or .csv): %s" % path)
+        raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
+
+
+def _save_json(path, result):
+    """Writes result.to_dict() as indented JSON (to_dict gives NaN as None)."""
+    import json
+    with open(path, "w") as f:
+        json.dump(result.to_dict(), f, indent=1, allow_nan=False)
+        f.write("\n")
 
 
 def _csv_cell(v):
@@ -426,13 +435,9 @@ def save_statistics(path, stats):
     """Writes the LabelStatistics of LMInferer.statistics: .json (spacing, percentiles, thresholds and one object per row,
     NaN as null) or .csv (a header, then one line per row: label, name, voxels, nan_voxels, volume_ml, mean_hu, std_hu,
     min_hu, max_hu, percentile_<q>..., fraction_below_<t>...; an unknown volume is an empty cell, NaN is "nan")."""
-    check_statistics_path(path)
+    check_table_path(path, "statistics")
     if path.lower().endswith(".json"):
-        import json
-        with open(path, "w") as f:
-            json.dump(stats.to_dict(), f, indent=1, allow_nan=False)
-            f.write("\n")
-        return
+        return _save_json(path, stats)
     base = ["label", "name", "voxels", "nan_voxels", "volume_ml", "mean_hu", "std_hu", "min_hu", "max_hu"]
     header = base + ["percentile_%g" % q for q in stats.percentiles] + ["fraction_below_%d" % t for t in stats.thresholds]
     lines = [",".join(header)]
@@ -444,24 +449,14 @@ def save_statistics(path, stats):
         f.write("\n".join(lines) + "\n")
 
 
-def check_clusters_path(path):
-    """Refuses, before any work is done, an output path save_clusters cannot write."""
-    if not path.lower().endswith((".json", ".csv")):
-        raise SystemExit("unsupported clusters output format (use .json or .csv): %s" % path)
-
-
 def save_clusters(path, clusters):
     """Writes the LaaClusters of LMInferer.laa_clusters: .json (spacing, threshold, connectivity, min_cluster_voxels and
     one object per row with its sizes / counts pairs, NaN as null) or .csv (a header, then one summary line per row:
     label, name, laa_voxels, laa_volume_ml, clusters, largest_voxels, largest_ml, d; an unknown volume is an empty cell,
     NaN is "nan")."""
-    check_clusters_path(path)
+    check_table_path(path, "clusters")
     if path.lower().endswith(".json"):
-        import json
-        with open(path, "w") as f:
-            json.dump(clusters.to_dict(), f, indent=1, allow_nan=False)
-            f.write("\n")
-        return
+        return _save_json(path, clusters)
     from .clusters import ClusterRow
     lines = [",".join(ClusterRow.SUMMARY)]
     for r in clusters.rows:
@@ -470,24 +465,14 @@ def save_clusters(path, clusters):
         f.write("\n".join(lines) + "\n")
 
 
-def check_regions_path(path):
-    """Refuses, before any work is done, an output path save_regional_statistics cannot write."""
-    if not path.lower().endswith((".json", ".csv")):
-        raise SystemExit("unsupported regions output format (use .json or .csv): %s" % path)
-
-
 def save_regional_statistics(path, regions):
     """Writes the RegionalStatistics of LMInferer.regional_statistics: .json (the parameters, one object per zone / shell
     row with its statistics, and the per-plane profile of every row; NaN as null) or .csv (a header, then one line per
     zone / shell row: label, name, region, index, region_name, first_plane, last_plane, depth_min_mm, depth_max_mm, then
     the statistics columns of save_statistics; an empty cell where a value does not apply or is unknown)."""
-    check_regions_path(path)
+    check_table_path(path, "regions")
     if path.lower().endswith(".json"):
-        import json
-        with open(path, "w") as f:
-            json.dump(regions.to_dict(), f, indent=1, allow_nan=False)
-            f.write("\n")
-        return
+        return _save_json(path, regions)
     stat = ["voxels", "nan_voxels", "volume_ml", "mean_hu", "std_hu", "min_hu", "max_hu"]
     header = ["label", "name", "region", "index", "region_name", "first_plane", "last_plane", "depth_min_mm",
               "depth_max_mm"] + stat + ["percentile_%g" % q for q in regions.percentiles] + \

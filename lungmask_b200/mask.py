@@ -5,6 +5,7 @@ Same public names, arguments and error behaviour as the reference (`MODEL_URLS`,
 work behind `LMInferer.apply` is the CUDA engine in liblungmask_b200.so.  PyTorch is used only to
 read a .pth state_dict into a flat fp32 blob (lungmask_b200.h: lm_load_weights).
 """
+import collections
 import os
 import warnings
 from typing import Optional, Union
@@ -131,6 +132,29 @@ def _tensor_dtype_code(t) -> int:
         raise TypeError("volume tensor dtype %s is not supported: use bool, uint8, a signed integer type, float16, bfloat16, "
                         "float32 or float64" % t.dtype)
     return codes[t.dtype]
+
+
+# numpy dtype -> LM_DTYPE_* of a host volume of the analysis calls
+_HOST_DTYPE_CODES = {np.dtype(bool): _native.DTYPE_U8, np.dtype(np.uint8): _native.DTYPE_U8, np.dtype(np.int8): _native.DTYPE_I8,
+                     np.dtype(np.int16): _native.DTYPE_I16, np.dtype(np.int32): _native.DTYPE_I32,
+                     np.dtype(np.int64): _native.DTYPE_I64, np.dtype(np.float16): _native.DTYPE_F16,
+                     np.dtype(np.float32): _native.DTYPE_F32, np.dtype(np.float64): _native.DTYPE_F64}
+
+
+def _host_volume(vol, what):
+    """(C-contiguous array, LM_DTYPE_* code) of a host volume of the analysis calls: uint16 / uint32 widened to int32 / int64
+    without loss; TypeError for the dtypes the engine does not read."""
+    if vol.dtype in (np.uint16, np.uint32):
+        vol = vol.astype(np.int32 if vol.dtype == np.uint16 else np.int64)
+    if vol.dtype not in _HOST_DTYPE_CODES:
+        raise TypeError("%s: volume dtype %s is not supported" % (what, vol.dtype))
+    return np.ascontiguousarray(vol), _HOST_DTYPE_CODES[vol.dtype]
+
+
+# What LMInferer._stage hands an analysis call: the volume (None for a mask alone), its LM_DTYPE_* code and the uint8 mask
+# as contiguous CUDA tensors on the engine's device, the caller's cudaStream_t, the spacing (x, y, z) or None, the
+# orientation code of the arrays, and back(t): a result tensor of the mask's shape in the type the mask came as.
+_Staged = collections.namedtuple("_Staged", "vol dtype mask stream spacing orientation back")
 
 
 class LMInferer:
@@ -341,12 +365,10 @@ class LMInferer:
         unchanged."""
         from . import statistics as st
         q, t = st.check_arguments(percentiles, thresholds)
-        res, spacing = self._per_label_call(
-            "statistics", image, mask, spacing, lambda vol, m: self.engine.label_stats(vol, m, q, t),
-            lambda v, code, m, stream: self.engine.label_stats_dev(v.data_ptr(), code, m.data_ptr(), v.shape, q, t,
-                                                                   stream=stream))
+        s = self._stage("statistics", image, mask, spacing)
+        res = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), s.mask.shape, q, t, stream=s.stream)
         labels = set(np.nonzero(res["voxels"][1:256])[0] + 1) | set(range(1, self.engine.n_classes[0]))
-        return st.from_native(res, labels, self.modelname, spacing, q, t)
+        return st.from_native(res, labels, self.modelname, s.spacing, q, t)
 
     def laa_clusters(self, image, mask, threshold=-950, connectivity=6, spacing=None, min_cluster_voxels=1):
         """Size distributions of the connected clusters of low-attenuation voxels (mask > 0 and value < `threshold` HU)
@@ -368,21 +390,11 @@ class LMInferer:
         on the engine's device read in place after the work queued on the current stream."""
         from . import clusters as cl
         threshold, connectivity, min_cluster_voxels = cl.check_arguments(threshold, connectivity, min_cluster_voxels)
-        import torch
-        device = torch.device("cuda", self.engine.device)
-
-        def host_call(vol, m):
-            res = self.engine.laa_clusters(vol, m, threshold, connectivity)
-            m = torch.from_numpy(np.ascontiguousarray(m).view(np.uint8)).to(device)
-            return dict(res, labels=self._mask_labels(m, torch.cuda.current_stream(device).cuda_stream))
-
-        def dev_call(v, code, m, stream):
-            res = self.engine.laa_clusters_dev(v.data_ptr(), code, m.data_ptr(), v.shape, threshold, connectivity, stream=stream)
-            return dict(res, labels=self._mask_labels(m, stream))
-
-        res, spacing = self._per_label_call("laa_clusters", image, mask, spacing, host_call, dev_call)
-        return cl.from_native(res, res["labels"] | set(range(1, self.engine.n_classes[0])), self.modelname, spacing, threshold,
-                              connectivity, min_cluster_voxels)
+        s = self._stage("laa_clusters", image, mask, spacing)
+        res = self.engine.laa_clusters_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), s.mask.shape, threshold, connectivity,
+                                           stream=s.stream)
+        labels = self._mask_labels(s.mask, s.stream) | set(range(1, self.engine.n_classes[0]))
+        return cl.from_native(res, labels, self.modelname, s.spacing, threshold, connectivity, min_cluster_voxels)
 
     def surface_distance(self, mask, spacing):
         """The distance in mm from every voxel with mask > 0 to the nearest voxel with mask == 0 -> float32 of the mask's
@@ -402,38 +414,10 @@ class LMInferer:
         sp = tuple(float(s) for s in np.asarray(spacing, dtype=np.float64).reshape(-1))
         if len(sp) != 3 or not all(np.isfinite(s) and s > 0 for s in sp):
             raise ValueError("surface_distance: spacing must be 3 finite positive sizes (s0, s1, s2) in mm, got %s" % (spacing,))
-        m, back = self._region_mask(mask, "surface_distance")
-        out = torch.empty(tuple(m.shape), dtype=torch.float32, device=m.device)
-        self.engine.surface_distance_dev(m.data_ptr(), m.shape, sp, out.data_ptr(),
-                                         stream=torch.cuda.current_stream(m.device).cuda_stream)
-        return back(out)
-
-    def _region_mask(self, mask, what):
-        """(contiguous uint8 CUDA tensor on the engine's device, function turning a result tensor into the caller's type)."""
-        import torch
-        device = torch.device("cuda", self.engine.device)
-        if _is_tensor(mask):
-            if mask.is_cuda and mask.device.index != self.engine.device:
-                raise ValueError("%s: the mask tensor is on %s, the engine on cuda:%d" % (what, mask.device, self.engine.device))
-            kind = "cuda" if mask.is_cuda else "cpu"
-            m = mask.detach()
-        else:
-            kind, m = "numpy", np.asarray(mask)
-            if m.dtype not in (np.uint8, np.bool_):
-                raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, m.dtype))
-            with warnings.catch_warnings():   # a read-only array: the host tensor is only copied from
-                warnings.simplefilter("ignore", UserWarning)
-                m = torch.from_numpy(np.ascontiguousarray(m).view(np.uint8))
-        if m.dtype not in (torch.uint8, torch.bool):
-            raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, m.dtype))
-        if m.dim() != 3:
-            raise ValueError("%s: expected a (slices, H, W) mask, got shape %s" % (what, tuple(m.shape)))
-        m = m.contiguous()
-        if m.dtype == torch.bool:
-            m = m.view(torch.uint8)
-        m = m.to(device)
-        back = {"cuda": lambda t: t, "cpu": lambda t: t.cpu(), "numpy": lambda t: t.cpu().numpy()}[kind]
-        return m, back
+        s = self._stage("surface_distance", None, mask, mask_only=True)
+        out = torch.empty(tuple(s.mask.shape), dtype=torch.float32, device=s.mask.device)
+        self.engine.surface_distance_dev(s.mask.data_ptr(), s.mask.shape, sp, out.data_ptr(), stream=s.stream)
+        return s.back(out)
 
     def regional_statistics(self, image, mask, spacing=None, zones=3, zone_by="volume", shells_mm=(10.0,),
                             percentiles=(15.0,), thresholds=(-950,)):
@@ -457,65 +441,40 @@ class LMInferer:
         Volume or SimpleITK image (which supplies the spacing), CPU tensors, or CUDA tensors on the engine's device read in
         place after the work queued on the current stream.  The per-label region map gives each (label, zone) and
         (label, shell) its own uint8 code, so labels x zones and labels x shells must stay at or below 255."""
+        import torch
         from . import regions as rg
         zones, zone_by, shells_mm, q, t = rg.check_arguments(zones, zone_by, shells_mm, percentiles, thresholds)
-        code = "LPS"
-        if not (isinstance(image, np.ndarray) or _is_tensor(image)):
-            if hasattr(image, "GetDirection"):
-                code = orient.orientation_from_direction(image.GetDirection())
-            if spacing is None and (hasattr(image, "spacing") or hasattr(image, "GetSpacing")):
-                spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
-        if spacing is not None:
-            spacing = tuple(float(s) for s in spacing)
-            if len(spacing) != 3:
-                raise ValueError("spacing must be (x, y, z), got %s" % (spacing,))
-        if shells_mm and spacing is None:
+        s = self._stage("regional_statistics", image, mask, spacing)
+        if shells_mm and s.spacing is None:
             raise ValueError("regional_statistics: depth shells need the voxel spacing; pass spacing=(x, y, z) in mm, or "
                              "shells_mm=() for zones only")
-        axis, superior_high = rg.craniocaudal_axis(code)
-        import torch
-        device = torch.device("cuda", self.engine.device)
+        axis, superior_high = rg.craniocaudal_axis(s.orientation)
+        m, shape = s.mask, tuple(s.mask.shape)
+        counts = self.engine.plane_label_counts_dev(m.data_ptr(), shape, axis, stream=s.stream)
+        present = [int(x) for x in np.flatnonzero(counts[:, 1:256].sum(axis=0)) + 1]
+        rg.check_code_budget(present, zones, "zones")
+        if shells_mm:
+            rg.check_code_budget(present, len(shells_mm) + 1, "shells")
+        label_zones = {l: rg.zone_of_planes(counts[:, l], zones, zone_by, superior_high) for l in present}
+        lung_zones = rg.zone_of_planes(counts[:, 256], zones, zone_by, superior_high)
+        region = torch.empty(shape, dtype=torch.uint8, device=m.device)
 
-        def dev_call(v, dtype_code, m, stream):
-            shape = tuple(m.shape)
-            counts = self.engine.plane_label_counts_dev(m.data_ptr(), shape, axis, stream=stream)
-            present = [int(x) for x in np.flatnonzero(counts[:, 1:256].sum(axis=0)) + 1]
-            rg.check_code_budget(present, zones, "zones")
-            if shells_mm:
-                rg.check_code_budget(present, len(shells_mm) + 1, "shells")
-            label_zones = {l: rg.zone_of_planes(counts[:, l], zones, zone_by, superior_high) for l in present}
-            lung_zones = rg.zone_of_planes(counts[:, 256], zones, zone_by, superior_high)
-            region = torch.empty(shape, dtype=torch.uint8, device=m.device)
+        def stats_of(lut, **kw):
+            self.engine.region_map_dev(m.data_ptr(), shape, lut, region.data_ptr(), stream=s.stream, **kw)
+            return self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, region.data_ptr(), shape, q, t, stream=s.stream)
 
-            def stats_of(lut, **kw):
-                self.engine.region_map_dev(m.data_ptr(), shape, lut, region.data_ptr(), stream=stream, **kw)
-                return self.engine.label_stats_dev(v.data_ptr(), dtype_code, region.data_ptr(), shape, q, t, stream=stream)
-
-            lut, lung_lut = rg.zone_luts(present, label_zones, lung_zones, zones)
-            res = {"counts": counts, "present": present, "label_zones": label_zones, "lung_zones": lung_zones,
-                   "zone": stats_of(lut, axis=axis), "zone_lung": stats_of(lung_lut, axis=axis), "shell": None,
-                   "shell_lung": None}
-            if shells_mm:
-                dist = torch.empty(shape, dtype=torch.float32, device=m.device)
-                self.engine.surface_distance_dev(m.data_ptr(), shape, spacing[::-1], dist.data_ptr(), stream=stream)
-                lut, lung_lut = rg.shell_luts(present, len(shells_mm) + 1)
-                kw = dict(d_dist_ptr=dist.data_ptr(), bounds=shells_mm)
-                res["shell"], res["shell_lung"] = stats_of(lut, **kw), stats_of(lung_lut, **kw)
-            return res
-
-        def host_call(vol, m):
-            vol, dtype_code, m = _native._host_pair(vol, m, "regional_statistics")
-            with warnings.catch_warnings():   # read-only arrays: the host tensors are only copied from
-                warnings.simplefilter("ignore", UserWarning)
-                v = torch.from_numpy(vol).to(device)
-                m = torch.from_numpy(m).to(device)
-            return dev_call(v, dtype_code, m, torch.cuda.current_stream(device).cuda_stream)
-
-        res, spacing = self._per_label_call("regional_statistics", image, mask, spacing, host_call, dev_call)
-        labels = sorted(set(res["present"]) | set(range(1, self.engine.n_classes[0])))
-        return rg.build(labels, res["present"], self.modelname, spacing, res["counts"], axis, superior_high, zones, zone_by,
-                        shells_mm, q, t, res["label_zones"], res["lung_zones"], res["zone"], res["zone_lung"], res["shell"],
-                        res["shell_lung"])
+        lut, lung_lut = rg.zone_luts(present, label_zones, lung_zones, zones)
+        zone, zone_lung = stats_of(lut, axis=axis), stats_of(lung_lut, axis=axis)
+        shell = shell_lung = None
+        if shells_mm:
+            dist = torch.empty(shape, dtype=torch.float32, device=m.device)
+            self.engine.surface_distance_dev(m.data_ptr(), shape, s.spacing[::-1], dist.data_ptr(), stream=s.stream)
+            lut, lung_lut = rg.shell_luts(present, len(shells_mm) + 1)
+            kw = dict(d_dist_ptr=dist.data_ptr(), bounds=shells_mm)
+            shell, shell_lung = stats_of(lut, **kw), stats_of(lung_lut, **kw)
+        labels = sorted(set(present) | set(range(1, self.engine.n_classes[0])))
+        return rg.build(labels, present, self.modelname, s.spacing, counts, axis, superior_high, zones, zone_by, shells_mm, q, t,
+                        label_zones, lung_zones, zone, zone_lung, shell, shell_lung)
 
     def _mask_labels(self, mask, stream):
         """The non-zero label values of a (S,H,W) uint8 CUDA mask tensor.  lm_label_stats_dev with the mask as its own uint8
@@ -524,57 +483,68 @@ class LMInferer:
                                              stream=stream)["voxels"]
         return set(int(x) for x in np.nonzero(voxels[1:256])[0] + 1)
 
-    def _per_label_call(self, what, image, mask, spacing, host_call, dev_call):
-        """The input handling of `statistics` and `laa_clusters` -> (the engine's result, spacing).  CUDA tensors go to
-        dev_call(volume tensor, dtype code, uint8 mask tensor, stream), both contiguous; everything else to
-        host_call(volume array, mask array)."""
-        if _is_tensor(image) and image.is_cuda or _is_tensor(mask) and mask.is_cuda:
-            res = self._per_label_tensor(what, image, mask, dev_call)
+    def _stage(self, what, image, mask, spacing=None, mask_only=False):
+        """The inputs of an analysis call as contiguous tensors on the engine's device -> _Staged.  CUDA tensors must be on
+        the engine's device and are read in place; a CUDA volume needs a CUDA mask and the reverse.  Everything else is
+        uploaded: numpy arrays, CPU tensors as their numpy arrays (bfloat16 widened to float32), a Volume or SimpleITK
+        image, which also supplies the orientation and, unless `spacing` is given, the spacing.  The mask is uint8 or bool
+        of the volume's shape.  mask_only: `image` is not used and the volume and its dtype code are None.  Neither input
+        is modified."""
+        import torch
+        device = torch.device("cuda", self.engine.device)
+        inputs = {"mask": mask} if mask_only else {"volume": image, "mask": mask}
+        on_cuda = [_is_tensor(x) and x.is_cuda for x in inputs.values()]
+        in_place = any(on_cuda)
+        code, vol, dtype = "LPS", None, None
+        if in_place:
+            if not all(on_cuda):
+                raise ValueError("%s: a CUDA tensor needs a CUDA tensor as partner (volume on %s, mask on %s)"
+                                 % (what, getattr(image, "device", "host"), getattr(mask, "device", "host")))
+            for name, x in inputs.items():
+                if x.device.index != self.engine.device:
+                    raise ValueError("%s: the %s tensor is on %s, the engine on cuda:%d" % (what, name, x.device, self.engine.device))
+            m, back = mask.detach(), (lambda t: t)
+            if not mask_only:
+                vol = image.detach()
         else:
-            if _is_tensor(image):
-                image = image.detach()
-                image = (image.float() if str(image.dtype) == "torch.bfloat16" else image).numpy()
-            if _is_tensor(mask):
-                mask = mask.detach().numpy()
-            if isinstance(image, np.ndarray):
-                array = image
-            else:
-                array, _ = self._array_and_orientation(image, what)
-                if spacing is None:
-                    spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
-            array, mask = np.asarray(array), np.asarray(mask)
-            self._check_per_label_inputs(what, array.shape, mask.shape, mask.dtype == np.uint8 or mask.dtype == bool, mask.dtype)
-            res = host_call(array, mask)
+            m = np.asarray(mask.detach().numpy() if _is_tensor(mask) else mask)
+            back = (lambda t: t.cpu()) if _is_tensor(mask) else (lambda t: t.cpu().numpy())
+            if not mask_only:
+                if _is_tensor(image):
+                    image = image.detach()
+                    image = (image.float() if image.dtype == torch.bfloat16 else image).numpy()
+                vol = image
+                if not isinstance(image, np.ndarray):
+                    vol, code = self._array_and_orientation(image, what)
+                    if spacing is None:
+                        spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
+                vol = np.asarray(vol)
         if spacing is not None:
             spacing = tuple(float(s) for s in spacing)
             if len(spacing) != 3:
                 raise ValueError("spacing must be (x, y, z), got %s" % (spacing,))
-        return res, spacing
-
-    @staticmethod
-    def _check_per_label_inputs(what, shape, mask_shape, mask_ok, mask_dtype):
-        if len(shape) != 3:
-            raise ValueError("%s: expected a (slices, H, W) volume, got shape %s" % (what, tuple(shape)))
-        if not mask_ok:
-            raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, mask_dtype))
-        if tuple(mask_shape) != tuple(shape):
-            raise ValueError("%s: the mask's shape %s differs from the volume's %s" % (what, tuple(mask_shape), tuple(shape)))
-
-    def _per_label_tensor(self, what, image, mask, dev_call):
-        import torch
-        if not (_is_tensor(image) and _is_tensor(mask) and image.is_cuda and mask.is_cuda):
-            raise ValueError("%s: a CUDA tensor needs a CUDA tensor as partner (volume on %s, mask on %s)"
-                             % (what, getattr(image, "device", "host"), getattr(mask, "device", "host")))
-        for name, x in (("volume", image), ("mask", mask)):
-            if x.device.index != self.engine.device:
-                raise ValueError("%s: the %s tensor is on %s, the engine on cuda:%d" % (what, name, x.device, self.engine.device))
-        self._check_per_label_inputs(what, image.shape, mask.shape, mask.dtype in (torch.uint8, torch.bool), mask.dtype)
-        code = _tensor_dtype_code(image)
-        image = image.detach().contiguous()
-        mask = mask.detach().contiguous()
-        if mask.dtype == torch.bool:
-            mask = mask.view(torch.uint8)
-        return dev_call(image, code, mask, torch.cuda.current_stream(image.device).cuda_stream)
+        if not mask_only and vol.ndim != 3:
+            raise ValueError("%s: expected a (slices, H, W) volume, got shape %s" % (what, tuple(vol.shape)))
+        if m.dtype not in ((torch.uint8, torch.bool) if _is_tensor(m) else (np.uint8, np.bool_)):
+            raise TypeError("%s: the mask must be uint8 or bool, got %s" % (what, m.dtype))
+        if mask_only and m.ndim != 3:
+            raise ValueError("%s: expected a (slices, H, W) mask, got shape %s" % (what, tuple(m.shape)))
+        if not mask_only and tuple(m.shape) != tuple(vol.shape):
+            raise ValueError("%s: the mask's shape %s differs from the volume's %s" % (what, tuple(m.shape), tuple(vol.shape)))
+        if in_place:
+            if not mask_only:
+                vol, dtype = vol.contiguous(), _tensor_dtype_code(vol)
+            m = m.contiguous()
+        else:
+            if not mask_only:
+                vol, dtype = _host_volume(vol, what)
+            with warnings.catch_warnings():   # read-only arrays: the host tensors are only copied from
+                warnings.simplefilter("ignore", UserWarning)
+                vol = None if mask_only else torch.from_numpy(vol).to(device)
+                m = torch.from_numpy(np.ascontiguousarray(m)).to(device)
+        if m.dtype == torch.bool:
+            m = m.view(torch.uint8)
+        return _Staged(vol, dtype, m, torch.cuda.current_stream(device).cuda_stream, spacing, code, back)
 
 
 def apply(image, model=None, force_cpu=False, batch_size=20, volume_postprocessing=True, tqdm_disable=False):

@@ -1,4 +1,4 @@
-"""Per-label lung volume and density statistics: the result of LMInferer.statistics (lm_label_stats, DESIGN §4.6).
+"""Per-label lung volume and density statistics: the result of LMInferer.statistics (lm_label_stats_dev, DESIGN §4.6).
 
 One row per label value l (the voxels with mask == l) and one for the whole lung, "lung" (mask > 0): voxel count, volume
 in mL when the spacing is known, NaN count, mean / std / min / max HU, HU percentiles (Perc15 by default) and the

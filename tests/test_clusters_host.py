@@ -106,14 +106,13 @@ def test_check_arguments():
             check_arguments(bad, 6, 1)
 
 
-def test_null_engine_refused():
+def test_null_engine_refused_dev():
     from lungmask_b200 import _native
     L = _native.lib()
     z = np.zeros(257, np.int64)
     p = C.c_void_p(z.ctypes.data)
-    assert L.lm_laa_clusters(None, p, 0, p, 1, 1, 1, -950, 6, p, p, p, p, p, 1000, ) == -1
-    assert "NULL" in L.lm_last_error().decode()
     assert L.lm_laa_clusters_dev(None, p, 0, p, 1, 1, 1, -950, 6, p, p, p, p, p, 1000, None) == -1
+    assert "NULL" in L.lm_last_error().decode()
 
 
 def _clusters(spacing=(0.5, 0.5, 2.0)):

@@ -1,4 +1,4 @@
-"""Low-attenuation cluster size distributions on the GPU (LMInferer.laa_clusters, lm_laa_clusters / lm_laa_clusters_dev)
+"""Low-attenuation cluster size distributions on the GPU (LMInferer.laa_clusters, lm_laa_clusters_dev)
 against an oracle written here: scipy.ndimage.label (4 / 6 / 26 structure) plus np.bincount, per label and on the union.
 Every row's (size, count) pairs, LAA voxel count and cluster count must be equal."""
 import ctypes as C
@@ -223,21 +223,23 @@ def test_empty_and_single_slice(inf, bullae):
         assert res["lung"].clusters > 0
 
 
-def test_native_rows(inf, bullae):
+def test_native_rows_dev(inf, bullae):
     """The 257 rows of the C ABI: row 0 and absent labels zero, pairs ascending, row 256 the union; and the count of a
-    row's LAA voxels equals lm_label_stats' below_count at the same threshold."""
+    row's LAA voxels equals lm_label_stats_dev's below_count at the same threshold."""
+    from lungmask_b200 import _native
     vol, mask = bullae
     m = mask.copy()
     m[:5] = 7
+    tv, tm = _cuda(vol), _cuda(m)
     eng = inf.engine
     for t in (-950, -900):
-        res = eng.laa_clusters(vol, m, t, 6)
+        res = eng.laa_clusters_dev(tv.data_ptr(), _native.DTYPE_I16, tm.data_ptr(), vol.shape, t, 6)
         assert res["laa_voxels"][0] == res["n_clusters"][0] == res["n_pairs"][0] == 0
         present = [1, 2, 7, 256]
         for r in range(257):
             if r not in present:
                 assert res["laa_voxels"][r] == res["n_clusters"][r] == res["n_pairs"][r] == 0, r
-        stats = eng.label_stats(vol, m, (), (t,))
+        stats = eng.label_stats_dev(tv.data_ptr(), _native.DTYPE_I16, tm.data_ptr(), vol.shape, (), (t,))
         for r in present:
             s = res["sizes"][res["offsets"][r]:res["offsets"][r + 1]]
             c = res["counts"][res["offsets"][r]:res["offsets"][r + 1]]
@@ -281,7 +283,7 @@ def test_volume_spacing_and_d(inf, bullae):
     assert inf.laa_clusters(vol, mask)["lung"].laa_volume_ml is None
 
 
-def test_errors(inf, bullae):
+def test_errors_dev(inf, bullae):
     import torch
     from lungmask_b200 import _native
     vol, mask = bullae
@@ -304,7 +306,7 @@ def test_errors(inf, bullae):
         inf.laa_clusters(tv.to(torch.complex64), tm)
     eng = inf.engine
     with pytest.raises(_native.NativeError, match="threshold"):
-        eng.laa_clusters(vol, mask, threshold=3073)
+        eng.laa_clusters_dev(tv.data_ptr(), _native.DTYPE_I16, tm.data_ptr(), vol.shape, threshold=3073)
     with pytest.raises(_native.NativeError, match="connectivity"):
         eng.laa_clusters_dev(tv.data_ptr(), _native.DTYPE_I16, tm.data_ptr(), vol.shape, connectivity=8)
     with pytest.raises(_native.NativeError, match="not a CUDA pointer|not device memory"):

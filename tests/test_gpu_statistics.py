@@ -1,4 +1,4 @@
-"""Per-label statistics on the GPU (LMInferer.statistics, lm_label_stats / lm_label_stats_dev) against a numpy oracle
+"""Per-label statistics on the GPU (LMInferer.statistics, lm_label_stats_dev) against a numpy oracle
 written here: counts, min / max, fraction_below and numpy.percentile bit for bit, mean / std within 1e-12 relative."""
 import json
 
@@ -248,7 +248,7 @@ def test_volume_end_to_end(inf6, phantom):
     assert inf6.statistics(vol, mask)["lung"].volume_ml is None
 
 
-def test_errors(inf6, phantom):
+def test_errors_dev(inf6, phantom):
     import torch
     from lungmask_b200 import _native
     vol, mask = phantom
@@ -284,9 +284,9 @@ def test_errors(inf6, phantom):
     # the C entry points refuse bad arguments before any kernel runs
     eng = inf6.engine
     with pytest.raises(_native.NativeError, match="not in \\[0,100\\]"):
-        eng.label_stats(vol, mask, percentiles=(-1.0,))
+        eng.label_stats_dev(tv.data_ptr(), _native.DTYPE_I16, tm.data_ptr(), vol.shape, percentiles=(-1.0,))
     with pytest.raises(_native.NativeError, match="threshold"):
-        eng.label_stats(vol, mask, thresholds=(3073,))
+        eng.label_stats_dev(tv.data_ptr(), _native.DTYPE_I16, tm.data_ptr(), vol.shape, thresholds=(3073,))
     with pytest.raises(_native.NativeError, match="not a CUDA pointer|not device memory"):
         eng.label_stats_dev(vol.ctypes.data, _native.DTYPE_I16, tm.data_ptr(), vol.shape)
     with pytest.raises(_native.NativeError, match="not a CUDA pointer|not device memory"):
