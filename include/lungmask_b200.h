@@ -221,6 +221,30 @@ LM_API int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d
                              const float* bounds, int n_bounds, const uint8_t* lut, size_t lut_size, uint8_t* d_map,
                              void* stream);
 
+/* Grey-level texture matrices of one ROI (no counterpart in the reference; DESIGN §4.9): LMInferer.texture computes the
+ * GLCM and GLSZM features of every row of lm_label_stats_dev from these.  All three take device memory of the engine's
+ * device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev, check every argument before any kernel
+ * runs and return after the engine's stream has synchronised; the inputs are never written.  Fewer than 2^32 voxels.
+ * lm_texture_levels_dev: the uint8 level map of one row.  d_vol, dtype, d_mask as lm_label_stats_dev; row 1..255 (the
+ *   voxels with mask == row) or 256 (mask > 0).  The ROI is the row's voxels with a non-NaN value (float16 / bfloat16
+ *   widened to float32); there d_levels[v] = floor((floor(x) - low) / bin_width) + 1, computed in int64, and 0
+ *   elsewhere.  bin_width >= 1, n_levels 1..255.  d_levels: n0*n1*n2 bytes, 16-byte aligned.  A level outside
+ *   1..n_levels or a non-finite value in the ROI is an error (the map is then incomplete).
+ * lm_glcm_dev: the unordered pair counts of a level map (0 = outside the ROI) with levels 1..n_levels (a larger level is
+ *   an error).  For each of the 13 offsets d of the 26-neighbourhood whose first non-zero component is positive, in the
+ *   order (0,0,1), (0,1,-1), (0,1,0), (0,1,1), then (1,dy,dx) for dy, dx = -1, 0, 1 (array axes 0, 1, 2), U_d(i, j),
+ *   i <= j, is the number of voxel pairs (v, v + d) inside the array with levels {i, j}.  counts (host): int64
+ *   [13][n_levels (n_levels + 1) / 2], (i, j) in row-major upper-triangle order (i = 1: j = 1..n_levels, then i = 2 ...).
+ * lm_zone_sizes_dev: the 26-connected components of equal level of a level map (0 = outside): n_pairs [256] int64 (row =
+ *   level; row 0 is 0), sizes and counts as lm_laa_clusters_dev (ascending sizes within a row, rows in order),
+ *   max_pairs >= lm_laa_max_pairs(n0*n1*n2). */
+LM_API int lm_texture_levels_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                                 int row, int64_t low, int bin_width, int n_levels, uint8_t* d_levels, void* stream);
+LM_API int lm_glcm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts,
+                       void* stream);
+LM_API int lm_zone_sizes_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
+                             int64_t* counts, size_t max_pairs, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -5,15 +5,16 @@ mask is written with the input's geometry as .nii / .nii.gz / .mha / .npy.  `--p
 model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_with_probabilities), and `--statistics PATH`
 the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950),
 `--clusters PATH` the size distributions of the low-attenuation clusters with their exponent D (.json / .csv,
-LMInferer.laa_clusters), and `--regions PATH` the statistics of every label by upper / middle / lower zone and by depth
-below the lung surface (.json / .csv, LMInferer.regional_statistics).
+LMInferer.laa_clusters), `--regions PATH` the statistics of every label by upper / middle / lower zone and by depth
+below the lung surface (.json / .csv, LMInferer.regional_statistics), and `--texture PATH` the GLCM and GLSZM texture
+features of every label and the whole lung (.json / .csv, LMInferer.texture).
 """
 import argparse
 import os
 import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_mask, save_probabilities,
-                 save_regional_statistics, save_statistics)
+                 save_regional_statistics, save_statistics, save_texture)
 from .logger import logger
 from .mask import LMInferer
 
@@ -57,6 +58,11 @@ def build_parser():
                    help="Also write the statistics of --statistics for every label and the whole lung by craniocaudal "
                         "zone (upper / middle / lower thirds of each row's volume) and by depth below the lung surface "
                         "(rind < 10 mm, core): .json (with the per-plane volume profile) or .csv")
+    p.add_argument("--texture", metavar="PATH", type=str, default=None,
+                   help="Also write the GLCM and GLSZM texture features (PyRadiomics names) of every label and the whole "
+                        "lung: .json (with the size-zone triples) or .csv")
+    p.add_argument("--texture-bin-width", metavar="BW", type=int, default=25,
+                   help="Fixed bin width of --texture in HU, a positive integer (default 25)")
     return p
 
 
@@ -77,6 +83,13 @@ def main(argv=None):
             sys.exit("--clusters-threshold: %s" % ex)
     if args.regions is not None:
         check_table_path(args.regions, "regions")
+    if args.texture is not None:
+        check_table_path(args.texture, "texture")
+        from .texture import check_arguments as check_texture_arguments
+        try:
+            check_texture_arguments(args.texture_bin_width)
+        except ValueError as ex:
+            sys.exit("--texture-bin-width: %s" % ex)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -109,6 +122,9 @@ def main(argv=None):
     if args.regions is not None:
         logger.info(f"Save regional statistics to: {args.regions}")
         save_regional_statistics(args.regions, inferer.regional_statistics(image, result))
+    if args.texture is not None:
+        logger.info(f"Save texture features to: {args.texture}")
+        save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width))
 
 
 if __name__ == "__main__":

@@ -53,6 +53,9 @@ def lib():
         "lm_plane_label_counts_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
         "lm_surface_distance_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp], i32),
         "lm_region_map_dev": ([vp, u8p, vp, i32, i32, i32, i32, vp, i32, vp, C.c_size_t, vp, vp], i32),
+        "lm_texture_levels_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32, C.c_int64, i32, i32, u8p, vp], i32),
+        "lm_glcm_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
+        "lm_zone_sizes_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, C.c_size_t, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -82,7 +85,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -325,6 +328,38 @@ class Engine:
         _check(lib().lm_region_map_dev(self._h, C.c_void_p(d_mask_ptr), C.c_void_p(d_dist_ptr) if d_dist_ptr else None,
                                        n0, n1, n2, -1 if axis is None else int(axis), _ptr(b) if b.size else None, int(b.size),
                                        _ptr(lut), lut.size, C.c_void_p(d_map_ptr), C.c_void_p(int(stream)) if stream else None))
+
+    # ---- texture matrices (lm_texture_levels_dev, lm_glcm_dev, lm_zone_sizes_dev)
+    def texture_levels_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, row, low, bin_width, n_levels, d_levels_ptr, stream=0):
+        """Writes the uint8 level map of `row` (1..255, or 256 for mask > 0) to `d_levels_ptr` (16-byte aligned):
+        floor((floor(x) - low) / bin_width) + 1 on the row's non-NaN voxels, 0 elsewhere (`stream` as for apply_dev)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        _check(lib().lm_texture_levels_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), C.c_void_p(d_mask_ptr), n0, n1, n2,
+                                           int(row), int(low), int(bin_width), int(n_levels), C.c_void_p(d_levels_ptr),
+                                           C.c_void_p(int(stream)) if stream else None))
+
+    def glcm_dev(self, d_levels_ptr, shape, n_levels, stream=0):
+        """-> int64 (13, n_levels (n_levels + 1) / 2): the unordered pair counts U_d(i <= j) of a uint8 level map, in the
+        direction order of lm_glcm_dev and the order of np.triu_indices(n_levels)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ng = int(n_levels)
+        counts = np.zeros((13, max(ng * (ng + 1) // 2, 1)), np.int64)
+        _check(lib().lm_glcm_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, ng, _ptr(counts),
+                                 C.c_void_p(int(stream)) if stream else None))
+        return counts
+
+    def zone_sizes_dev(self, d_levels_ptr, shape, stream=0):
+        """-> dict: "n_pairs" (int64 [256], row = level), "sizes", "counts" (the rows' (size, count) pairs concatenated;
+        row r's are [offsets[r], offsets[r + 1])), "offsets": the 26-connected zones of equal level of a uint8 level map."""
+        n0, n1, n2 = (int(x) for x in shape)
+        cap = int(lib().lm_laa_max_pairs(max(n0, 0) * max(n1, 0) * max(n2, 0)))
+        n_pairs = np.zeros(256, np.int64)
+        sizes, counts = np.zeros(cap, np.int64), np.zeros(cap, np.int64)
+        _check(lib().lm_zone_sizes_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, _ptr(n_pairs), _ptr(sizes), _ptr(counts),
+                                       cap, C.c_void_p(int(stream)) if stream else None))
+        offsets = np.concatenate([[0], np.cumsum(n_pairs)])
+        total = int(offsets[-1])
+        return {"n_pairs": n_pairs, "sizes": sizes[:total].copy(), "counts": counts[:total].copy(), "offsets": offsets}
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

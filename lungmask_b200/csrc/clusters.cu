@@ -13,6 +13,8 @@
 //                 overflow list of (row, size)
 // Passes 2-4 run once for map_l and once for map_u.  The host then reads each row's dense extent, copies those bins and
 // the overflow list, and compacts them into (size, count) pairs: sorted overflow entries after the scanned dense bins.
+// zone_sizes (lm_zone_sizes_dev, DESIGN §4.9) runs passes 2-4 and the compaction once, 26-connected, on a caller's
+// texture level map: the size-zone matrix, row = level.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -131,18 +133,20 @@ struct ClusterDev {
   u64* over;                 // [over_cap]
 };
 
-// Each labelling has at most n / kClusterDense clusters of kClusterDense voxels or more, and there are two labellings.
+// Each labelling has at most n / kClusterDense clusters of kClusterDense voxels or more, and there are at most two
+// labellings.
 size_t over_cap(size_t n) { return 2 * (n / kClusterDense) + 2; }
 
-// Carves the work area; returns its size (d == nullptr: size only).
-size_t layout(char* d, size_t n, ClusterDev* g) {
+// Carves the work area; returns its size (d == nullptr: size only).  maps: with the two LAA maps (laa_clusters);
+// zone_sizes labels the caller's map.
+size_t layout(char* d, size_t n, bool maps, ClusterDev* g) {
   size_t off = 0;
   auto take = [&](size_t bytes) { char* p = d ? d + off : nullptr; off += align256(bytes); return p; };
-  const size_t padded = (n + kChunk - 1) / kChunk * kChunk;
+  const size_t padded = maps ? (n + kChunk - 1) / kChunk * kChunk : 0;
   g->parent = (uint32_t*)take(n * 4);
   g->area = (uint32_t*)take(n * 4);
-  g->map_l = (uint8_t*)take(padded);
-  g->map_u = (uint8_t*)take(padded);
+  g->map_l = maps ? (uint8_t*)take(padded) : nullptr;
+  g->map_u = maps ? (uint8_t*)take(padded) : nullptr;
   g->dense = (uint32_t*)take((size_t)kClusterRows * kClusterDense * 4);
   g->row_max = (uint32_t*)take(kClusterRows * 4);
   g->n_over = (uint32_t*)take(4);
@@ -181,58 +185,34 @@ int map_pass(int dtype, const void* vol, const uint8_t* mask, size_t n, int t, c
   }
 }
 
-}  // namespace
-
-size_t laa_max_pairs(size_t n_voxels) {
-  // ceil(sqrt(n)), exact for every size_t
-  unsigned __int128 s = (unsigned __int128)sqrtl((long double)n_voxels);
-  while (s * s < n_voxels) ++s;
-  while (s > 0 && (s - 1) * (s - 1) >= n_voxels) --s;
-  return (size_t)(32 * s + 256);
-}
-
-int ClusterWork::reserve(size_t bytes) {
-  if (bytes <= d_bytes) return 0;
-  release();
-  const cudaError_t e = cudaMalloc(&d, bytes);
-  if (e != cudaSuccess) { d = nullptr; return (int)e; }
-  d_bytes = bytes;
-  return 0;
-}
-
-void ClusterWork::release() {
-  if (d) cudaFree(d);
-  d = nullptr;
-  d_bytes = 0;
-}
-
-int laa_clusters(ClusterWork& w, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2, int threshold,
-                 int conn, const LaaClustersOut& out, int num_sms, cudaStream_t st, int64_t* launches) {
-  if (conn != 4 && conn != 6 && conn != 26) return -1;
-  const size_t n = (size_t)n0 * n1 * n2;
-  for (int r = 0; r < kClusterRows; ++r) out.laa_voxels[r] = out.n_clusters[r] = out.n_pairs[r] = 0;
-  ClusterDev g;
-  SC((cudaError_t)w.reserve(layout(nullptr, n, &g)));
-  layout(static_cast<char*>(w.d), n, &g);
-
+// Clears the size histogram of the work area.
+int clear_histogram(const ClusterDev& g, cudaStream_t st) {
   SC(cudaMemsetAsync(g.dense, 0, (size_t)kClusterRows * kClusterDense * 4, st));
   SC(cudaMemsetAsync(g.row_max, 0, kClusterRows * 4, st));
   SC(cudaMemsetAsync(g.n_over, 0, 4, st));
-  const int rc = map_pass(dtype, d_vol, d_mask, n, threshold, g, num_sms, st);
-  if (rc) return rc;
-  ++*launches;
-  const int g_area = grid_for(cluster_area_kernel, 0, n, num_sms), g_hist = grid_for(cluster_hist_kernel, 0, n, num_sms);
-  for (int pass = 0; pass < 2; ++pass) {
-    const uint8_t* map = pass ? g.map_u : g.map_l;
-    const int lrc = ccl_volume_device(map, g.parent, n0, n1, n2, conn, num_sms, st, launches);
-    if (lrc) return lrc;
-    SC(cudaMemsetAsync(g.area, 0, n * 4, st));
-    cluster_area_kernel<<<g_area, kThreads, 0, st>>>(g.parent, g.area, n);
-    cluster_hist_kernel<<<g_hist, kThreads, 0, st>>>(g.parent, g.area, map, n, pass ? 256 : 0, g.dense, g.row_max, g.over, g.n_over);
-    SC(cudaGetLastError());
-    *launches += 2;
-  }
+  return 0;
+}
 
+// Passes 2-4 on one map: the equal-value components, their sizes, and their count in the histogram at row = the map
+// value (fixed_row 0) or fixed_row.
+int count_components(const ClusterDev& g, const uint8_t* map, int n0, int n1, int n2, int conn, int fixed_row, int num_sms,
+                     cudaStream_t st, int64_t* launches) {
+  const size_t n = (size_t)n0 * n1 * n2;
+  const int lrc = ccl_volume_device(map, g.parent, n0, n1, n2, conn, num_sms, st, launches);
+  if (lrc) return lrc;
+  SC(cudaMemsetAsync(g.area, 0, n * 4, st));
+  cluster_area_kernel<<<grid_for(cluster_area_kernel, 0, n, num_sms), kThreads, 0, st>>>(g.parent, g.area, n);
+  cluster_hist_kernel<<<grid_for(cluster_hist_kernel, 0, n, num_sms), kThreads, 0, st>>>(g.parent, g.area, map, n, fixed_row,
+                                                                                        g.dense, g.row_max, g.over, g.n_over);
+  SC(cudaGetLastError());
+  *launches += 2;
+  return 0;
+}
+
+// The histogram of rows 1..256 as (size, count) pairs: reads each row's dense extent, copies those bins and the
+// overflow list, and writes sorted overflow entries after the scanned dense bins.  Synchronises `st` twice.
+int compact_histogram(const ClusterDev& g, const LaaClustersOut& out, cudaStream_t st) {
+  for (int r = 0; r < kClusterRows; ++r) out.laa_voxels[r] = out.n_clusters[r] = out.n_pairs[r] = 0;
   // the extent of every row's dense bins and the overflow count, then only those bins and entries
   uint32_t row_max[kClusterRows], n_over = 0;
   SC(cudaMemcpyAsync(row_max, g.row_max, sizeof(row_max), cudaMemcpyDeviceToHost, st));
@@ -274,6 +254,68 @@ int laa_clusters(ClusterWork& w, const void* d_vol, int dtype, const uint8_t* d_
     out.n_pairs[r] = pairs;
   }
   return k <= out.max_pairs ? 0 : -1;   // unreachable: max_pairs >= laa_max_pairs(n) bounds k
+}
+
+}  // namespace
+
+size_t laa_max_pairs(size_t n_voxels) {
+  // ceil(sqrt(n)), exact for every size_t
+  unsigned __int128 s = (unsigned __int128)sqrtl((long double)n_voxels);
+  while (s * s < n_voxels) ++s;
+  while (s > 0 && (s - 1) * (s - 1) >= n_voxels) --s;
+  return (size_t)(32 * s + 256);
+}
+
+int ClusterWork::reserve(size_t bytes) {
+  if (bytes <= d_bytes) return 0;
+  release();
+  const cudaError_t e = cudaMalloc(&d, bytes);
+  if (e != cudaSuccess) { d = nullptr; return (int)e; }
+  d_bytes = bytes;
+  return 0;
+}
+
+void ClusterWork::release() {
+  if (d) cudaFree(d);
+  d = nullptr;
+  d_bytes = 0;
+}
+
+int laa_clusters(ClusterWork& w, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2, int threshold,
+                 int conn, const LaaClustersOut& out, int num_sms, cudaStream_t st, int64_t* launches) {
+  if (conn != 4 && conn != 6 && conn != 26) return -1;
+  const size_t n = (size_t)n0 * n1 * n2;
+  for (int r = 0; r < kClusterRows; ++r) out.laa_voxels[r] = out.n_clusters[r] = out.n_pairs[r] = 0;
+  ClusterDev g;
+  SC((cudaError_t)w.reserve(layout(nullptr, n, true, &g)));
+  layout(static_cast<char*>(w.d), n, true, &g);
+
+  const int crc = clear_histogram(g, st);
+  if (crc) return crc;
+  const int rc = map_pass(dtype, d_vol, d_mask, n, threshold, g, num_sms, st);
+  if (rc) return rc;
+  ++*launches;
+  for (int pass = 0; pass < 2; ++pass) {
+    const int lrc = count_components(g, pass ? g.map_u : g.map_l, n0, n1, n2, conn, pass ? 256 : 0, num_sms, st, launches);
+    if (lrc) return lrc;
+  }
+  return compact_histogram(g, out, st);
+}
+
+int zone_sizes(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
+               int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches) {
+  const size_t n = (size_t)n0 * n1 * n2;
+  ClusterDev g;
+  SC((cudaError_t)w.reserve(layout(nullptr, n, false, &g)));
+  layout(static_cast<char*>(w.d), n, false, &g);
+  const int crc = clear_histogram(g, st);
+  if (crc) return crc;
+  const int lrc = count_components(g, d_levels, n0, n1, n2, 26, 0, num_sms, st, launches);
+  if (lrc) return lrc;
+  int64_t voxels[kClusterRows], zones[kClusterRows], pairs[kClusterRows];
+  const int rc = compact_histogram(g, {voxels, zones, pairs, sizes, counts, max_pairs}, st);
+  for (int r = 0; r < 256; ++r) n_pairs[r] = pairs[r];   // row 256 (the union) stays empty: fixed_row is 0
+  return rc;
 }
 
 }  // namespace lm

@@ -38,4 +38,10 @@ struct ClusterWork {
 int laa_clusters(ClusterWork& w, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2, int threshold,
                  int conn, const LaaClustersOut& out, int num_sms, cudaStream_t st, int64_t* launches);
 
+// The 26-connected equal-value zones of the uint8 (n0,n1,n2) map `d_levels` (0 = outside): n_pairs [256] (row = the map
+// value, row 0 zero) and the rows' (size, count) pairs as laa_clusters gives them.  The work area holds parent and area
+// (8 B / voxel) and the histogram.  The caller checks the arguments (n < 2^32, max_pairs >= laa_max_pairs(n)).
+int zone_sizes(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
+               int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches);
+
 }  // namespace lm

@@ -20,6 +20,7 @@
 #include "stats.cuh"
 #include "clusters.cuh"
 #include "regions.cuh"
+#include "texture.cuh"
 
 using namespace lm;
 
@@ -195,6 +196,7 @@ struct lm_engine {
   LabelStatsWork stats;   // lm_label_stats_dev: counts, histograms and selection state
   ClusterWork clusters;   // lm_laa_clusters_dev: LAA maps, union-find parents, cluster sizes, size histogram
   RegionWork regions;     // lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev: EDT stacks, counts, LUT
+  TextureWork texture;    // lm_texture_levels_dev, lm_glcm_dev: error flag, pair counts (lm_zone_sizes_dev uses `clusters`)
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -798,7 +800,7 @@ struct DevArg {
 };
 
 // The start of an analysis call (lm_label_stats_dev, lm_laa_clusters_dev, lm_plane_label_counts_dev,
-// lm_surface_distance_dev, lm_region_map_dev), once its other arguments are checked: each device pointer must be memory
+// lm_surface_distance_dev, lm_region_map_dev and the texture calls), once its other arguments are checked: each device pointer must be memory
 // of the engine's device (a NULL one is an optional input the call does not use), the engine's stream waits for the work
 // queued on the caller's, and the launch count restarts.
 int analysis_inputs(lm_engine* e, const char* fn, void* stream, std::initializer_list<DevArg> ptrs) {
@@ -905,6 +907,7 @@ void lm_destroy(lm_engine* e) {
   e->stats.release();
   e->clusters.release();
   e->regions.release();
+  e->texture.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1182,6 +1185,62 @@ int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, 
   RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}, {"d_dist", d_dist}, {"d_map", d_map}}));
   RC(region_map(e->regions, d_mask, d_dist, n0, n1, n2, d_dist ? -1 : axis, bounds, d_dist ? n_bounds : 0, lut, lut_size, d_map,
                 e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+// The argument checks the three texture calls share: the shape (fewer than 2^32 voxels) and n_levels.
+static int check_texture_volume(const char* fn, int n0, int n1, int n2) {
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the texture calls take fewer than 2^32", fn, n);
+  return 0;
+}
+
+// A level outside 1..n_levels or a non-finite value found on the device.
+static int texture_device_error(const char* fn, int rc, int n_levels) {
+  if (rc == kLevelRange) return fail(rc, "%s: a level outside 1..%d (n_levels) in the ROI", fn, n_levels);
+  if (rc == kLevelNonFinite) return fail(rc, "%s: a non-finite value (+-inf) in the ROI", fn);
+  return rc;
+}
+
+int lm_texture_levels_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2, int row,
+                          int64_t low, int bin_width, int n_levels, uint8_t* d_levels, void* stream) {
+  static const char* fn = "lm_texture_levels_dev";
+  if (!e || !d_vol || !d_mask || !d_levels) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (row < 1 || row > 256) return fail(-1, "%s: row %d not in [1,256]", fn, row);
+  if (bin_width < 1) return fail(-1, "%s: bin_width %d is not positive", fn, bin_width);
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  if (reinterpret_cast<uintptr_t>(d_levels) & 15) return fail(-1, "%s: d_levels is not 16-byte aligned", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_mask", d_mask}, {"d_levels", d_levels}}));
+  const int rc = texture_levels(e->texture, d_vol, dtype, d_mask, (size_t)n0 * n1 * n2, row, low, bin_width, n_levels, d_levels,
+                                e->num_sms, e->st, &e->launches);
+  if (rc) return texture_device_error(fn, rc, n_levels);
+  return 0;
+}
+
+int lm_glcm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts, void* stream) {
+  static const char* fn = "lm_glcm_dev";
+  if (!e || !d_levels || !counts) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  const int rc = glcm(e->texture, d_levels, n0, n1, n2, n_levels, counts, e->num_sms, e->st, &e->launches);
+  if (rc) return texture_device_error(fn, rc, n_levels);
+  return 0;
+}
+
+int lm_zone_sizes_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
+                      int64_t* counts, size_t max_pairs, void* stream) {
+  static const char* fn = "lm_zone_sizes_dev";
+  if (!e || !d_levels || !n_pairs || !sizes || !counts) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (max_pairs < laa_max_pairs(n))
+    return fail(-1, "%s: max_pairs %zu below lm_laa_max_pairs(%zu) = %zu", fn, max_pairs, n, laa_max_pairs(n));
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  RC(zone_sizes(e->clusters, d_levels, n0, n1, n2, n_pairs, sizes, counts, max_pairs, e->num_sms, e->st, &e->launches));
   return 0;
 }
 

@@ -1,0 +1,246 @@
+// Grey-level texture matrices of one ROI (lm_texture_levels_dev, lm_glcm_dev, DESIGN §4.9).
+//
+//   levels  reads the mask as 16-byte vectors and the value only under the row; writes the row's discretised level (0
+//           outside the ROI) 16 bytes at a time, the last partial chunk byte by byte.  A level outside 1..n_levels or a
+//           non-finite value raises a flag instead of being written.
+//   glcm    one warp per 32-voxel run along x, one lane per voxel: for each of the 13 directions d the lane reads the
+//           level of v + d, and the lanes holding equal pair keys (i <= j) add their count with one atomic
+//           (__match_any_sync).  Parenchyma fills a few near-diagonal bins, so the counters are privatised in shared
+//           memory: the whole upper triangle of every direction while n_levels <= kSmemLevels, above that the band
+//           j - i < kBand (where nearly all pairs of neighbouring voxels fall) with the rest going to global atomics.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <math.h>
+
+#include <algorithm>
+#include <type_traits>
+#include <vector>
+
+#include "../../include/lungmask_b200.h"
+#include "mask_chunk.cuh"
+#include "texture.cuh"
+
+namespace lm {
+namespace {
+
+constexpr int kThreads = 512;
+constexpr int kSmemLevels = 90;    // triangle of 13 directions: 13 x 4095 x 4 B = 212,940 B
+constexpr int kBand = 16;          // n_levels > kSmemLevels: 13 x 255 x 16 x 4 B = 212,160 B
+constexpr unsigned kFull = 0xffffffffu;
+
+// ---- levels ---------------------------------------------------------------------------------------------------------
+// flag bit 0: a level outside 1..n_levels, bit 1: a non-finite value.
+template <typename T>
+__device__ __forceinline__ int level_of(T x, long long low, int bw, int ng, int* flag) {
+  long long f;
+  if constexpr (std::is_integral<T>::value) {
+    f = (long long)x;
+  } else {
+    double d;
+    if constexpr (std::is_same<T, __half>::value) d = (double)__half2float(x);
+    else if constexpr (std::is_same<T, __nv_bfloat16>::value) d = (double)__bfloat162float(x);
+    else d = (double)x;
+    if (isnan(d)) return 0;
+    if (isinf(d)) { atomicOr(flag, 2); return 0; }
+    d = floor(d);
+    if (d < -9.0e18 || d > 9.0e18) { atomicOr(flag, 1); return 0; }
+    f = (long long)d;
+  }
+  // x >= low, so the difference is exact in uint64
+  const unsigned long long q = f < low ? 0ull : ((unsigned long long)f - (unsigned long long)low) / (unsigned)bw + 1;
+  if (q < 1 || q > (unsigned long long)ng) { atomicOr(flag, 1); return 0; }
+  return (int)q;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) texture_level_kernel(const T* __restrict__ vol, const uint8_t* __restrict__ mask,
+                                                                 size_t n, int row, long long low, int bw, int ng,
+                                                                 uint8_t* __restrict__ out, int* __restrict__ flag) {
+  const size_t chunks = (n + kChunk - 1) / kChunk;
+  for (size_t c = blockIdx.x * (size_t)blockDim.x + threadIdx.x; c < chunks; c += (size_t)gridDim.x * blockDim.x) {
+    const size_t base = c * kChunk;
+    const uint4 lab = load_labels(mask, base, n);
+    unsigned w[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int k = 0; k < kChunk; ++k) {
+      const int l = label_at(lab, k);
+      if (row == 256 ? l != 0 : l == row) w[k >> 2] |= (unsigned)level_of(vol[base + k], low, bw, ng, flag) << (8 * (k & 3));
+    }
+    const uint4 lv = make_uint4(w[0], w[1], w[2], w[3]);
+    if (base + kChunk <= n) {
+      reinterpret_cast<uint4*>(out)[c] = lv;
+    } else {
+      for (int k = 0; base + k < n; ++k) out[base + k] = (uint8_t)label_at(lv, k);
+    }
+  }
+}
+
+// ---- GLCM -----------------------------------------------------------------------------------------------------------
+// Direction d: (0,0,1); (0,1,-1..1); (1,-1..1,-1..1), as (dz, dy, dx) over array axes (0, 1, 2).
+__host__ __device__ constexpr int dir_z(int d) { return d < 4 ? 0 : 1; }
+__host__ __device__ constexpr int dir_y(int d) { return d == 0 ? 0 : (d < 4 ? 1 : (d - 4) / 3 - 1); }
+__host__ __device__ constexpr int dir_x(int d) { return d == 0 ? 1 : (d < 4 ? d - 2 : (d - 4) % 3 - 1); }
+
+// (i, j), 1 <= i <= j <= ng -> row-major upper-triangle index
+__host__ __device__ __forceinline__ int tri(int i, int j, int ng) { return (i - 1) * ng - (i - 1) * (i - 2) / 2 + (j - i); }
+
+// kTri: shared counters s[d][tri(i, j)].  Otherwise s[d][(j - i) * ng + i - 1] for j - i < kBand, global for the rest.
+template <bool kTri>
+__global__ void __launch_bounds__(kThreads) glcm_kernel(const uint8_t* __restrict__ lev, int n0, int n1, int n2, int ng,
+                                                        uint32_t* __restrict__ counts, int* __restrict__ flag) {
+  extern __shared__ uint32_t s_cnt[];
+  const int t_len = ng * (ng + 1) / 2;
+  const int per_dir = kTri ? t_len : ng * kBand;
+  for (int i = threadIdx.x; i < kGlcmDirections * per_dir; i += blockDim.x) s_cnt[i] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const size_t warp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5, n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+  const int runs_x = (n2 + 31) / 32;
+  const size_t runs = (size_t)n0 * n1 * runs_x;
+  for (size_t r = warp; r < runs; r += n_warps) {   // warp-uniform
+    const size_t line = r / runs_x;
+    const int x = (int)(r % runs_x) * 32 + lane, y = (int)(line % n1), z = (int)(line / n1);
+    const size_t v = line * n2 + x;
+    int a = x < n2 ? lev[v] : 0;
+    if (a > ng) { atomicOr(flag, 1); a = 0; }
+    if (!__any_sync(kFull, a != 0)) continue;
+#pragma unroll
+    for (int d = 0; d < kGlcmDirections; ++d) {
+      const int zz = z + dir_z(d), yy = y + dir_y(d), xx = x + dir_x(d);
+      int b = 0;
+      if (a && zz < n0 && (unsigned)yy < (unsigned)n1 && (unsigned)xx < (unsigned)n2)
+        b = lev[(size_t)((long long)v + ((long long)dir_z(d) * n1 + dir_y(d)) * n2 + dir_x(d))];
+      if (b > ng) { atomicOr(flag, 1); b = 0; }
+      if (b) {
+        const int i = min(a, b), j = max(a, b);
+        const bool shared = kTri || j - i < kBand;
+        const int key = kTri ? tri(i, j, ng) : (shared ? (j - i) * ng + i - 1 : per_dir + tri(i, j, ng));
+        const unsigned peers = __match_any_sync(__activemask(), key);
+        if (lane == __ffs(peers) - 1) {
+          if (shared) atomicAdd(&s_cnt[d * per_dir + key], (uint32_t)__popc(peers));
+          else atomicAdd(&counts[(size_t)d * t_len + (key - per_dir)], (uint32_t)__popc(peers));
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < kGlcmDirections * per_dir; k += blockDim.x) {
+    if (!s_cnt[k]) continue;
+    const int d = k / per_dir, e = k % per_dir;
+    const int t = kTri ? e : tri(e % ng + 1, e % ng + 1 + e / ng, ng);
+    atomicAdd(&counts[(size_t)d * t_len + t], s_cnt[k]);
+  }
+}
+
+// ---- host -----------------------------------------------------------------------------------------------------------
+#define SC(x)                                   \
+  do {                                          \
+    const cudaError_t e_ = (x);                 \
+    if (e_ != cudaSuccess) return (int)e_;      \
+  } while (0)
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// The work area: the flag, then the pair counts.
+size_t work_bytes(int n_levels) {
+  return align256(sizeof(int)) + align256((size_t)kGlcmDirections * n_levels * (n_levels + 1) / 2 * 4);
+}
+
+template <typename K>
+int grid_for(K kernel, size_t smem, size_t work, int num_sms) {
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  const size_t need = (work + kThreads - 1) / kThreads;
+  return (int)std::max<size_t>(std::min((size_t)per_sm * num_sms, need), 1);
+}
+
+template <typename T>
+int launch_levels(const void* vol, const uint8_t* mask, size_t n, int row, long long low, int bw, int ng, uint8_t* out,
+                  int* flag, int num_sms, cudaStream_t st) {
+  const size_t chunks = (n + kChunk - 1) / kChunk;
+  texture_level_kernel<T><<<grid_for(texture_level_kernel<T>, 0, chunks, num_sms), kThreads, 0, st>>>(
+      static_cast<const T*>(vol), mask, n, row, low, bw, ng, out, flag);
+  return (int)cudaGetLastError();
+}
+
+int flag_result(const int* d_flag, cudaStream_t st) {
+  int flag = 0;
+  SC(cudaMemcpyAsync(&flag, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+  SC(cudaStreamSynchronize(st));
+  return (flag & 2) ? kLevelNonFinite : ((flag & 1) ? kLevelRange : 0);
+}
+
+}  // namespace
+
+int TextureWork::reserve(size_t bytes) {
+  if (bytes <= d_bytes) return 0;
+  release();
+  const cudaError_t e = cudaMalloc(&d, bytes);
+  if (e != cudaSuccess) { d = nullptr; return (int)e; }
+  d_bytes = bytes;
+  return 0;
+}
+
+void TextureWork::release() {
+  if (d) cudaFree(d);
+  d = nullptr;
+  d_bytes = 0;
+}
+
+int texture_levels(TextureWork& w, const void* d_vol, int dtype, const uint8_t* d_mask, size_t n, int row, int64_t low,
+                   int bin_width, int n_levels, uint8_t* d_levels, int num_sms, cudaStream_t st, int64_t* launches) {
+  SC((cudaError_t)w.reserve(work_bytes(1)));
+  int* flag = static_cast<int*>(w.d);
+  SC(cudaMemsetAsync(flag, 0, sizeof(int), st));
+  int rc;
+#define LM_LEVELS_CASE(code, T) \
+  case code: rc = launch_levels<T>(d_vol, d_mask, n, row, low, bin_width, n_levels, d_levels, flag, num_sms, st); break
+  switch (dtype) {
+    LM_LEVELS_CASE(LM_DTYPE_U8, uint8_t);
+    LM_LEVELS_CASE(LM_DTYPE_I8, int8_t);
+    LM_LEVELS_CASE(LM_DTYPE_I16, int16_t);
+    LM_LEVELS_CASE(LM_DTYPE_I32, int32_t);
+    LM_LEVELS_CASE(LM_DTYPE_I64, int64_t);
+    LM_LEVELS_CASE(LM_DTYPE_F16, __half);
+    LM_LEVELS_CASE(LM_DTYPE_BF16, __nv_bfloat16);
+    LM_LEVELS_CASE(LM_DTYPE_F32, float);
+    LM_LEVELS_CASE(LM_DTYPE_F64, double);
+    default: return -1;
+  }
+#undef LM_LEVELS_CASE
+  if (rc) return rc;
+  ++*launches;
+  return flag_result(flag, st);
+}
+
+int glcm(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts, int num_sms,
+         cudaStream_t st, int64_t* launches) {
+  const size_t t_len = (size_t)n_levels * (n_levels + 1) / 2, total = kGlcmDirections * t_len;
+  SC((cudaError_t)w.reserve(work_bytes(n_levels)));
+  int* flag = static_cast<int*>(w.d);
+  uint32_t* d_counts = reinterpret_cast<uint32_t*>(static_cast<char*>(w.d) + align256(sizeof(int)));
+  SC(cudaMemsetAsync(flag, 0, sizeof(int), st));
+  SC(cudaMemsetAsync(d_counts, 0, total * 4, st));
+  const size_t runs = (size_t)n0 * n1 * ((n2 + 31) / 32), threads = runs * 32;
+  if (n_levels <= kSmemLevels) {
+    const size_t smem = total * 4;
+    SC(cudaFuncSetAttribute(glcm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    glcm_kernel<true><<<grid_for(glcm_kernel<true>, smem, threads, num_sms), kThreads, smem, st>>>(d_levels, n0, n1, n2, n_levels,
+                                                                                                   d_counts, flag);
+  } else {
+    const size_t smem = (size_t)kGlcmDirections * n_levels * kBand * 4;
+    SC(cudaFuncSetAttribute(glcm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    glcm_kernel<false><<<grid_for(glcm_kernel<false>, smem, threads, num_sms), kThreads, smem, st>>>(d_levels, n0, n1, n2,
+                                                                                                     n_levels, d_counts, flag);
+  }
+  SC(cudaGetLastError());
+  ++*launches;
+  std::vector<uint32_t> h(total);
+  SC(cudaMemcpyAsync(h.data(), d_counts, total * 4, cudaMemcpyDeviceToHost, st));
+  const int rc = flag_result(flag, st);
+  if (rc) return rc;
+  for (size_t k = 0; k < total; ++k) counts[k] = h[k];
+  return 0;
+}
+
+}  // namespace lm

@@ -409,7 +409,7 @@ def save_probabilities(path, probs, like=None):
 
 def check_table_path(path, kind):
     """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
-    ("clusters") or save_regional_statistics ("regions") cannot write."""
+    ("clusters"), save_regional_statistics ("regions") or save_texture ("texture") cannot write."""
     if not path.lower().endswith((".json", ".csv")):
         raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
 
@@ -461,6 +461,25 @@ def save_clusters(path, clusters):
     lines = [",".join(ClusterRow.SUMMARY)]
     for r in clusters.rows:
         lines.append(",".join(_csv_cell(getattr(r, k)) for k in ClusterRow.SUMMARY))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def save_texture(path, texture):
+    """Writes the TextureFeatures of LMInferer.texture: .json (spacing, bin_width and one object per row with its GLCM and
+    GLSZM features and the GLSZM (level, size, count) triples, NaN as null) or .csv (a header, then one line per row:
+    label, name, voxels, low, bin_width, n_levels, glcm_<Name>..., glszm_<Name>...; an unknown value is an empty cell,
+    NaN is "nan")."""
+    check_table_path(path, "texture")
+    if path.lower().endswith(".json"):
+        return _save_json(path, texture)
+    from .texture import GLCM_FEATURES, GLSZM_FEATURES, TextureRow
+    header = list(TextureRow.SUMMARY) + ["glcm_" + k for k in GLCM_FEATURES] + ["glszm_" + k for k in GLSZM_FEATURES]
+    lines = [",".join(header)]
+    for r in texture.rows:
+        cells = [getattr(r, k) for k in TextureRow.SUMMARY] + [r.glcm[k] for k in GLCM_FEATURES] + \
+            [r.glszm[k] for k in GLSZM_FEATURES]
+        lines.append(",".join(_csv_cell(v) for v in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")
 

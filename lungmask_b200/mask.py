@@ -476,6 +476,54 @@ class LMInferer:
         return rg.build(labels, present, self.modelname, s.spacing, counts, axis, superior_high, zones, zone_by, shells_mm, q, t,
                         label_zones, lung_zones, zone, zone_lung, shell, shell_lung)
 
+    def texture(self, image, mask, bin_width=25, spacing=None):
+        """GLCM and GLSZM texture features of `image` under `mask` -> lungmask_b200.texture.TextureFeatures, with the rows
+        of `statistics`: every label value in the mask and every label 1..K-1 of the model (absent ones with 0 voxels and
+        NaN features), then "lung" (mask > 0).  A row's ROI is its voxels with a non-NaN value, read in the volume's dtype
+        (float16 / bfloat16 as float32); a non-finite value in an ROI is a ValueError.
+
+        Each row is discretised with the fixed `bin_width` (a positive integer, PyRadiomics' binWidth): low = bw *
+        floor(min / bw), level(x) = floor((floor(x) - low) / bw) + 1, Ng = the level of the row's maximum; more than 255
+        levels is a ValueError before any texture kernel runs.  GLCM: the symmetric co-occurrence matrices of the 13
+        directions of the 26-neighbourhood at distance 1 voxel (spacing is not used), a pair counted only when both voxels
+        are in the row (so a pair across a lobe boundary counts in "lung" only); the features are averaged over the
+        directions with pairs.  GLSZM: the 26-connected zones of equal level.  Each row holds the features (dicts keyed by
+        the PyRadiomics names of texture.GLCM_FEATURES / GLSZM_FEATURES) and the exact matrices: the pair counts
+        `glcm_counts` (13, Ng (Ng + 1) / 2) and the (level, size, count) `zones`.
+
+        `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image, CPU tensors, or CUDA
+        tensors on the engine's device read in place after the work queued on the current stream; both are left
+        unchanged."""
+        import torch
+        from . import texture as tx
+        from .statistics import label_name
+        bw = tx.check_arguments(bin_width)
+        s = self._stage("texture", image, mask, spacing)
+        shape = tuple(s.mask.shape)
+        st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, (), (), stream=s.stream)
+        present = set(int(x) for x in np.nonzero(st["voxels"][1:256])[0] + 1)
+        rows = sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]
+        names = {r: tx.UNION if r == 256 else label_name(self.modelname, r) for r in rows}
+        plan = {}   # every row's discretisation first: a refused row stops the call before any texture kernel
+        for r in rows:
+            n = int(st["voxels"][r] - st["nan_voxels"][r])
+            if n:
+                plan[r] = (n,) + tx.discretisation(float(st["moments"][r][2]), float(st["moments"][r][3]), bw,
+                                                   "row %s (%s)" % ("lung" if r == 256 else r, names[r]))
+        out = []
+        levels = torch.empty(shape, dtype=torch.uint8, device=s.mask.device) if plan else None
+        for r in rows:
+            if r not in plan:
+                out.append(tx.build_row(r, names[r], 0, bw))
+                continue
+            n, low, ng = plan[r]
+            self.engine.texture_levels_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, r, low, bw, ng,
+                                           levels.data_ptr(), stream=s.stream)
+            U = self.engine.glcm_dev(levels.data_ptr(), shape, ng, stream=s.stream)
+            zones = tx.zones_from_native(self.engine.zone_sizes_dev(levels.data_ptr(), shape, stream=s.stream))
+            out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones))
+        return tx.TextureFeatures(s.spacing, bw, out)
+
     def _mask_labels(self, mask, stream):
         """The non-zero label values of a (S,H,W) uint8 CUDA mask tensor.  lm_label_stats_dev with the mask as its own uint8
         volume and no percentiles or thresholds: its count and histogram passes over the mask bytes."""
