@@ -303,7 +303,11 @@ def postprocessing(label_image: np.ndarray, spare=(), skip_below: int = 3, taps:
     if taps is not None:
         taps["regions1"] = regionmask.copy()
         taps["mapped"] = mapped.copy()
+    return finish_labels(mapped)
 
+
+def finish_labels(mapped: np.ndarray) -> np.ndarray:
+    """utils.py:344-358, step 6 of `postprocessing`: per label, largest component and holes filled."""
     if mapped.shape[0] == 1:
         def fill(x):
             return area_closing(x[0].astype(int), area_threshold=64)[None, :, :] == 1

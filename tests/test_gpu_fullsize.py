@@ -1,6 +1,7 @@
 """BASELINE.json's full-size configurations through size-independent properties (the CPU oracle would need
 minutes to hours at these sizes): slice independence of the per-slice stages, run-to-run determinism,
-label range, and the fusion rule's invariants."""
+label range, and the fusion rule's invariants.  The exact full-size checks of C3 and C4 - every output voxel explained
+by the network's labels through oracle.postfast - are in tests/test_gpu_post_fullsize.py."""
 import os
 
 import numpy as np
