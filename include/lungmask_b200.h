@@ -245,6 +245,31 @@ LM_API int lm_glcm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, in
 LM_API int lm_zone_sizes_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
                              int64_t* counts, size_t max_pairs, void* stream);
 
+/* Mesh shape support (no counterpart in the reference; DESIGN §4.10): LMInferer.shape computes PyRadiomics-style shape
+ * features (surface area, mesh volume, sphericity, maximum diameters, principal axes) of every row of lm_label_stats_dev
+ * from these.  Both take device memory of the engine's device and the caller's cudaStream_t with the event-wait rule of
+ * lm_apply_dev, check every argument before any kernel runs and return after the engine's stream has synchronised; the
+ * mask is never written.  mask (n0,n1,n2) uint8, fewer than 2^32 voxels and every axis below 2^30.  A voxel is in row l
+ * (1..255) when mask == l and in row 256 when mask != 0; voxels outside the array are in no row (the mask is padded with
+ * one voxel of outside, the opposite of lm_surface_distance_dev).  A cube is each 2x2x2 block of the padded grid, with
+ * lowest corner p (p_k in -1..n_k-1); its configuration has bit c set when corner p + ((c >> 2) & 1, (c >> 1) & 1, c & 1)
+ * is in the row.
+ * lm_shape_sums_dev: one pass for all rows (host int64 results; row 0 stays zero):
+ *   cube_counts [257][256]     the cubes of each configuration (0 and 255 stay zero)
+ *   cube_possum [257][256][3]  the sum of their lowest corners p over the array axes
+ *   moments [257][10]          N, sum i, sum j, sum k, sum i^2, sum j^2, sum k^2, sum ij, sum ik, sum jk over the row's
+ *                              voxels (i, j, k) in array axes
+ * lm_max_diameters_dev: d2 [4] (host doubles), the largest squared distance (mm^2) between two mesh vertices of `row`
+ *   (1..256) - all pairs, pairs with equal axis-0, equal axis-1 and equal axis-2 coordinate.  A vertex is the midpoint
+ *   u + v (doubled integer coordinates) of two face-adjacent grid points of the padded grid that differ in membership;
+ *   d^2 = ((D2 h2)^2 + (D1 h1)^2) + (D0 h0)^2 with h_k = spacing[k] / 2 (spacing per ARRAY axis, finite and positive),
+ *   every product and sum rounded on its own; 0 without a pair.  Work area: 8 bytes per line of the grid along each axis
+ *   and edge direction, and 16 bytes per candidate vertex, kept by the engine. */
+LM_API int lm_shape_sums_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int64_t* cube_counts,
+                             int64_t* cube_possum, int64_t* moments, void* stream);
+LM_API int lm_max_diameters_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const double* spacing,
+                                double* d2, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -6,15 +6,17 @@ model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_wit
 the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950),
 `--clusters PATH` the size distributions of the low-attenuation clusters with their exponent D (.json / .csv,
 LMInferer.laa_clusters), `--regions PATH` the statistics of every label by upper / middle / lower zone and by depth
-below the lung surface (.json / .csv, LMInferer.regional_statistics), and `--texture PATH` the GLCM and GLSZM texture
-features of every label and the whole lung (.json / .csv, LMInferer.texture).
+below the lung surface (.json / .csv, LMInferer.regional_statistics), `--texture PATH` the GLCM and GLSZM texture
+features of every label and the whole lung (.json / .csv, LMInferer.texture), and `--shape PATH` the mesh shape features
+(surface area, mesh volume, sphericity, maximum diameters, principal axes) of every label and the whole lung (.json /
+.csv, LMInferer.shape).
 """
 import argparse
 import os
 import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_mask, save_probabilities,
-                 save_regional_statistics, save_statistics, save_texture)
+                 save_regional_statistics, save_shape, save_statistics, save_texture)
 from .logger import logger
 from .mask import LMInferer
 
@@ -63,6 +65,10 @@ def build_parser():
                         "lung: .json (with the size-zone triples) or .csv")
     p.add_argument("--texture-bin-width", metavar="BW", type=int, default=25,
                    help="Fixed bin width of --texture in HU, a positive integer (default 25)")
+    p.add_argument("--shape", metavar="PATH", type=str, default=None,
+                   help="Also write the mesh shape features (PyRadiomics names: surface area, mesh volume, sphericity, "
+                        "maximum 3-D and 2-D diameters, principal axis lengths) of every label and the whole lung: .json "
+                        "(with the exact sums) or .csv")
     return p
 
 
@@ -90,6 +96,8 @@ def main(argv=None):
             check_texture_arguments(args.texture_bin_width)
         except ValueError as ex:
             sys.exit("--texture-bin-width: %s" % ex)
+    if args.shape is not None:
+        check_table_path(args.shape, "shape")
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -125,6 +133,9 @@ def main(argv=None):
     if args.texture is not None:
         logger.info(f"Save texture features to: {args.texture}")
         save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width))
+    if args.shape is not None:
+        logger.info(f"Save shape features to: {args.shape}")
+        save_shape(args.shape, inferer.shape(result, image=image))
 
 
 if __name__ == "__main__":

@@ -56,6 +56,8 @@ def lib():
         "lm_texture_levels_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32, C.c_int64, i32, i32, u8p, vp], i32),
         "lm_glcm_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
         "lm_zone_sizes_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, C.c_size_t, vp], i32),
+        "lm_shape_sums_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, vp], i32),
+        "lm_max_diameters_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -85,7 +87,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -360,6 +362,30 @@ class Engine:
         offsets = np.concatenate([[0], np.cumsum(n_pairs)])
         total = int(offsets[-1])
         return {"n_pairs": n_pairs, "sizes": sizes[:total].copy(), "counts": counts[:total].copy(), "offsets": offsets}
+
+    # ---- mesh shape support (lm_shape_sums_dev, lm_max_diameters_dev)
+    def shape_sums_dev(self, d_mask_ptr, shape, stream=0):
+        """-> dict over 257 rows (row l = mask == l, row 256 = mask != 0) of a (n0,n1,n2) uint8 device mask padded with
+        outside: "cube_counts" int64 (257, 256) marching-cube configurations, "cube_possum" int64 (257, 256, 3) the sums of
+        their lowest corners, "moments" int64 (257, 10) (`stream` as for apply_dev)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        res = {"cube_counts": np.zeros((257, 256), np.int64), "cube_possum": np.zeros((257, 256, 3), np.int64),
+               "moments": np.zeros((257, 10), np.int64)}
+        _check(lib().lm_shape_sums_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, _ptr(res["cube_counts"]),
+                                       _ptr(res["cube_possum"]), _ptr(res["moments"]), C.c_void_p(int(stream)) if stream else None))
+        return res
+
+    def max_diameters_dev(self, d_mask_ptr, shape, row, spacing, stream=0):
+        """-> float64 [4]: the largest squared distances (mm^2) between mesh vertices of `row` (1..255, or 256 for
+        mask != 0) - all pairs, equal axis-0, axis-1, axis-2 coordinate; `spacing` per array axis (s0, s1, s2)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        sp = np.ascontiguousarray(spacing, dtype=np.float64).reshape(-1)
+        if sp.size != 3:
+            raise ValueError("max_diameters_dev: spacing needs 3 values, got %d" % sp.size)
+        d2 = np.zeros(4, np.float64)
+        _check(lib().lm_max_diameters_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, int(row), _ptr(sp), _ptr(d2),
+                                          C.c_void_p(int(stream)) if stream else None))
+        return d2
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

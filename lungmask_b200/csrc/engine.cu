@@ -21,6 +21,7 @@
 #include "clusters.cuh"
 #include "regions.cuh"
 #include "texture.cuh"
+#include "shape.cuh"
 
 using namespace lm;
 
@@ -197,6 +198,7 @@ struct lm_engine {
   ClusterWork clusters;   // lm_laa_clusters_dev: LAA maps, union-find parents, cluster sizes, size histogram
   RegionWork regions;     // lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev: EDT stacks, counts, LUT
   TextureWork texture;    // lm_texture_levels_dev, lm_glcm_dev: error flag, pair counts (lm_zone_sizes_dev uses `clusters`)
+  ShapeWork shape;        // lm_shape_sums_dev, lm_max_diameters_dev: sums, line tables, diameter candidates
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -800,7 +802,7 @@ struct DevArg {
 };
 
 // The start of an analysis call (lm_label_stats_dev, lm_laa_clusters_dev, lm_plane_label_counts_dev,
-// lm_surface_distance_dev, lm_region_map_dev and the texture calls), once its other arguments are checked: each device pointer must be memory
+// lm_surface_distance_dev, lm_region_map_dev, the texture and the shape calls), once its other arguments are checked: each device pointer must be memory
 // of the engine's device (a NULL one is an optional input the call does not use), the engine's stream waits for the work
 // queued on the caller's, and the launch count restarts.
 int analysis_inputs(lm_engine* e, const char* fn, void* stream, std::initializer_list<DevArg> ptrs) {
@@ -908,6 +910,7 @@ void lm_destroy(lm_engine* e) {
   e->clusters.release();
   e->regions.release();
   e->texture.release();
+  e->shape.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1241,6 +1244,38 @@ int lm_zone_sizes_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int
     return fail(-1, "%s: max_pairs %zu below lm_laa_max_pairs(%zu) = %zu", fn, max_pairs, n, laa_max_pairs(n));
   RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
   RC(zone_sizes(e->clusters, d_levels, n0, n1, n2, n_pairs, sizes, counts, max_pairs, e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+// The argument checks the two shape calls share: the shape (fewer than 2^32 voxels, every axis below 2^30).
+static int check_shape_volume(const char* fn, int n0, int n1, int n2) {
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the shape calls take fewer than 2^32", fn, n);
+  if (n0 >= (1 << 30) || n1 >= (1 << 30) || n2 >= (1 << 30)) return fail(-1, "%s: (%d,%d,%d): an axis of 2^30 or more", fn, n0, n1, n2);
+  return 0;
+}
+
+int lm_shape_sums_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int64_t* cube_counts, int64_t* cube_possum,
+                      int64_t* moments, void* stream) {
+  static const char* fn = "lm_shape_sums_dev";
+  if (!e || !d_mask || !cube_counts || !cube_possum || !moments) return fail(-1, "%s: NULL argument", fn);
+  RC(check_shape_volume(fn, n0, n1, n2));
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}}));
+  RC(shape_sums(e->shape, d_mask, n0, n1, n2, cube_counts, cube_possum, moments, e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+int lm_max_diameters_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const double* spacing, double* d2,
+                         void* stream) {
+  static const char* fn = "lm_max_diameters_dev";
+  if (!e || !d_mask || !spacing || !d2) return fail(-1, "%s: NULL argument", fn);
+  RC(check_shape_volume(fn, n0, n1, n2));
+  if (row < 1 || row > 256) return fail(-1, "%s: row %d not in [1,256]", fn, row);
+  for (int k = 0; k < 3; ++k)
+    if (!(spacing[k] > 0.0 && spacing[k] < INFINITY)) return fail(-1, "%s: spacing[%d] = %g is not finite and positive", fn, k, spacing[k]);
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}}));
+  RC(max_diameters(e->shape, d_mask, n0, n1, n2, row, spacing, d2, e->num_sms, e->st, &e->launches));
   return 0;
 }
 

@@ -409,7 +409,7 @@ def save_probabilities(path, probs, like=None):
 
 def check_table_path(path, kind):
     """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
-    ("clusters"), save_regional_statistics ("regions") or save_texture ("texture") cannot write."""
+    ("clusters"), save_regional_statistics ("regions"), save_texture ("texture") or save_shape ("shape") cannot write."""
     if not path.lower().endswith((".json", ".csv")):
         raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
 
@@ -503,6 +503,22 @@ def save_regional_statistics(path, regions):
         cells = [r.label, r.name, r.region, r.index, r.region_name, planes[0], planes[1], depth[0], depth[1]] + \
             [getattr(r.stats, k) for k in stat] + [r.stats.percentile_hu[q] for q in regions.percentiles] + \
             [r.stats.fraction_below[t] for t in regions.thresholds]
+        lines.append(",".join(_csv_cell(v) for v in cells))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def save_shape(path, shape):
+    """Writes the ShapeFeatures of LMInferer.shape: .json (spacing and one object per row with its features, the non-zero
+    cube counts and corner sums by configuration, the moments and the squared diameters, NaN as null) or .csv (a header,
+    then one line per row: label, name, voxels, then the 14 features of shape.SHAPE_FEATURES; NaN is "nan")."""
+    check_table_path(path, "shape")
+    if path.lower().endswith(".json"):
+        return _save_json(path, shape)
+    from .shape import SHAPE_FEATURES, ShapeRow
+    lines = [",".join(list(ShapeRow.SUMMARY) + list(SHAPE_FEATURES))]
+    for r in shape.rows:
+        cells = [getattr(r, k) for k in ShapeRow.SUMMARY] + [r.features[k] for k in SHAPE_FEATURES]
         lines.append(",".join(_csv_cell(v) for v in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")

@@ -524,6 +524,45 @@ class LMInferer:
             out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones))
         return tx.TextureFeatures(s.spacing, bw, out)
 
+    def shape(self, mask, spacing=None, image=None):
+        """Mesh shape features of every row of `statistics` -> lungmask_b200.shape.ShapeFeatures: every label value in the
+        mask and every label 1..K-1 of the model (absent ones with 0 voxels and NaN features), then "lung" (mask != 0).
+        A voxel is in label l's row when mask == l, so the fissures between lobes are surfaces of each lobe but interior
+        to "lung".
+
+        Each row is meshed by marching cubes on the mask padded with one voxel of outside, as PyRadiomics does: a lung cut
+        by the first or last slice is closed there by a flat face (the opposite of `surface_distance`, where voxels
+        outside the array are not background).  The 14 features of shape.SHAPE_FEATURES use PyRadiomics' names:
+        SurfaceArea and MeshVolume of the mesh, VoxelVolume, SurfaceVolumeRatio, Sphericity, the maximum 3-D diameter and
+        the maximum 2-D diameters within slices (equal axis-0 index), columns (axis 1) and rows (axis 2) between mesh
+        vertices, and the principal axis lengths, Elongation and Flatness of the voxel positions.  Each row also holds
+        the exact sums they come from (cube_counts, cube_possum, moments) and the squared diameters d2.
+
+        `spacing` (x, y, z) in mm is required: given, or supplied by `image` (a Volume or SimpleITK image, used for
+        nothing else); without one this is a ValueError before any kernel runs.  `mask`: (S, H, W) uint8 or bool, numpy,
+        a CPU tensor, or a CUDA tensor on the engine's device read in place after the work queued on the current stream;
+        it is left unchanged."""
+        from . import shape as sh
+        from .statistics import label_name
+        if spacing is None and image is not None:
+            spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
+        spacing = sh.check_spacing(spacing)
+        s = self._stage("shape", None, mask, mask_only=True)
+        shape = tuple(s.mask.shape)
+        res = self.engine.shape_sums_dev(s.mask.data_ptr(), shape, stream=s.stream)
+        present = set(int(x) for x in np.nonzero(res["moments"][1:256, 0])[0] + 1)
+        rows = sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]
+        geometry = sh.config_geometry(spacing)
+        out = []
+        for r in rows:
+            d2 = np.zeros(4)
+            if r == 256 and present or r in present:
+                d2 = self.engine.max_diameters_dev(s.mask.data_ptr(), shape, r, spacing[::-1], stream=s.stream)
+            name = sh.UNION if r == 256 else label_name(self.modelname, r)
+            out.append(sh.build_row(r, name, spacing, res["cube_counts"][r], res["cube_possum"][r], res["moments"][r], d2,
+                                    geometry))
+        return sh.ShapeFeatures(spacing, out)
+
     def _mask_labels(self, mask, stream):
         """The non-zero label values of a (S,H,W) uint8 CUDA mask tensor.  lm_label_stats_dev with the mask as its own uint8
         volume and no percentiles or thresholds: its count and histogram passes over the mask bytes."""
