@@ -222,7 +222,7 @@ LM_API int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d
                              void* stream);
 
 /* Grey-level texture matrices of one ROI (no counterpart in the reference; DESIGN §4.9): LMInferer.texture computes the
- * GLCM and GLSZM features of every row of lm_label_stats_dev from these.  All three take device memory of the engine's
+ * GLCM, GLSZM, GLRLM, GLDM and NGTDM features of every row of lm_label_stats_dev from these.  All take device memory of the engine's
  * device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev, check every argument before any kernel
  * runs and return after the engine's stream has synchronised; the inputs are never written.  Fewer than 2^32 voxels.
  * lm_texture_levels_dev: the uint8 level map of one row.  d_vol, dtype, d_mask as lm_label_stats_dev; row 1..255 (the
@@ -237,13 +237,25 @@ LM_API int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d
  *   [13][n_levels (n_levels + 1) / 2], (i, j) in row-major upper-triangle order (i = 1: j = 1..n_levels, then i = 2 ...).
  * lm_zone_sizes_dev: the 26-connected components of equal level of a level map (0 = outside): n_pairs [256] int64 (row =
  *   level; row 0 is 0), sizes and counts as lm_laa_clusters_dev (ascending sizes within a row, rows in order),
- *   max_pairs >= lm_laa_max_pairs(n0*n1*n2). */
+ *   max_pairs >= lm_laa_max_pairs(n0*n1*n2).
+ * lm_glrlm_dev: the run counts of a level map with levels 1..n_levels (a larger level is an error).  For each of the 13
+ *   offsets d of lm_glcm_dev, in its order, a run is a maximal sequence v, v+d, ..., v+(k-1)d of voxels inside the array
+ *   that all have level i >= 1.  counts (host): int64 [13][n_levels][max(n0,n1,n2)], the runs of level i+1 and length
+ *   k+1 along direction d.
+ * lm_neighbour_counts_dev: for each voxel v of level i >= 1 (levels 1..n_levels as lm_glrlm_dev), W(v) is the number of
+ *   its 26 neighbours inside the array with level >= 1, S(v) the sum of their levels, and c(v) the number of those with
+ *   |level - i| <= alpha (alpha >= 0).  dependence, ngtdm_counts, ngtdm_sums (host): int64 [n_levels][27], G(i, c) the
+ *   voxels of level i with c(v) = c, N(i, W) those with W(v) = W, A(i, W) = the sum of |W i - S(v)| over them. */
 LM_API int lm_texture_levels_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
                                  int row, int64_t low, int bin_width, int n_levels, uint8_t* d_levels, void* stream);
 LM_API int lm_glcm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts,
                        void* stream);
 LM_API int lm_zone_sizes_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
                              int64_t* counts, size_t max_pairs, void* stream);
+LM_API int lm_glrlm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts,
+                        void* stream);
+LM_API int lm_neighbour_counts_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                                   int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums, void* stream);
 
 /* Mesh shape support (no counterpart in the reference; DESIGN §4.10): LMInferer.shape computes PyRadiomics-style shape
  * features (surface area, mesh volume, sphericity, maximum diameters, principal axes) of every row of lm_label_stats_dev

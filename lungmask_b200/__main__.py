@@ -6,8 +6,9 @@ model's per-class probabilities (.npy or 4-D .nii / .nii.gz, LMInferer.apply_wit
 the volume and HU statistics of every label and of the whole lung (.json / .csv, LMInferer.statistics: Perc15, LAA-950),
 `--clusters PATH` the size distributions of the low-attenuation clusters with their exponent D (.json / .csv,
 LMInferer.laa_clusters), `--regions PATH` the statistics of every label by upper / middle / lower zone and by depth
-below the lung surface (.json / .csv, LMInferer.regional_statistics), `--texture PATH` the GLCM and GLSZM texture
-features of every label and the whole lung (.json / .csv, LMInferer.texture), and `--shape PATH` the mesh shape features
+below the lung surface (.json / .csv, LMInferer.regional_statistics), `--texture PATH` the texture features of every
+label and the whole lung (GLCM and GLSZM by default, `--texture-classes` adds GLRLM, GLDM and NGTDM; .json / .csv,
+LMInferer.texture), and `--shape PATH` the mesh shape features
 (surface area, mesh volume, sphericity, maximum diameters, principal axes) of every label and the whole lung (.json /
 .csv, LMInferer.shape).
 """
@@ -61,10 +62,13 @@ def build_parser():
                         "zone (upper / middle / lower thirds of each row's volume) and by depth below the lung surface "
                         "(rind < 10 mm, core): .json (with the per-plane volume profile) or .csv")
     p.add_argument("--texture", metavar="PATH", type=str, default=None,
-                   help="Also write the GLCM and GLSZM texture features (PyRadiomics names) of every label and the whole "
-                        "lung: .json (with the size-zone triples) or .csv")
+                   help="Also write the texture features (PyRadiomics names) of every label and the whole lung, of the "
+                        "classes of --texture-classes: .json (with the exact matrices) or .csv")
     p.add_argument("--texture-bin-width", metavar="BW", type=int, default=25,
                    help="Fixed bin width of --texture in HU, a positive integer (default 25)")
+    p.add_argument("--texture-classes", metavar="NAMES", type=str, default="glcm,glszm",
+                   help="Comma-separated texture classes of --texture: any of glcm, glszm, glrlm, gldm, ngtdm "
+                        "(default glcm,glszm)")
     p.add_argument("--shape", metavar="PATH", type=str, default=None,
                    help="Also write the mesh shape features (PyRadiomics names: surface area, mesh volume, sphericity, "
                         "maximum 3-D and 2-D diameters, principal axis lengths) of every label and the whole lung: .json "
@@ -91,11 +95,15 @@ def main(argv=None):
         check_table_path(args.regions, "regions")
     if args.texture is not None:
         check_table_path(args.texture, "texture")
-        from .texture import check_arguments as check_texture_arguments
+        from .texture import check_arguments as check_texture_arguments, check_classes
         try:
             check_texture_arguments(args.texture_bin_width)
         except ValueError as ex:
             sys.exit("--texture-bin-width: %s" % ex)
+        try:
+            texture_classes = check_classes([c.strip() for c in args.texture_classes.split(",") if c.strip()])
+        except ValueError as ex:
+            sys.exit("--texture-classes: %s" % ex)
     if args.shape is not None:
         check_table_path(args.shape, "shape")
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
@@ -132,7 +140,7 @@ def main(argv=None):
         save_regional_statistics(args.regions, inferer.regional_statistics(image, result))
     if args.texture is not None:
         logger.info(f"Save texture features to: {args.texture}")
-        save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width))
+        save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width, classes=texture_classes))
     if args.shape is not None:
         logger.info(f"Save shape features to: {args.shape}")
         save_shape(args.shape, inferer.shape(result, image=image))

@@ -56,6 +56,8 @@ def lib():
         "lm_texture_levels_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32, C.c_int64, i32, i32, u8p, vp], i32),
         "lm_glcm_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
         "lm_zone_sizes_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, C.c_size_t, vp], i32),
+        "lm_glrlm_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
+        "lm_neighbour_counts_dev": ([vp, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_shape_sums_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_max_diameters_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
@@ -87,7 +89,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -331,7 +333,7 @@ class Engine:
                                        n0, n1, n2, -1 if axis is None else int(axis), _ptr(b) if b.size else None, int(b.size),
                                        _ptr(lut), lut.size, C.c_void_p(d_map_ptr), C.c_void_p(int(stream)) if stream else None))
 
-    # ---- texture matrices (lm_texture_levels_dev, lm_glcm_dev, lm_zone_sizes_dev)
+    # ---- texture matrices (lm_texture_levels_dev, lm_glcm_dev, lm_zone_sizes_dev, lm_glrlm_dev, lm_neighbour_counts_dev)
     def texture_levels_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, row, low, bin_width, n_levels, d_levels_ptr, stream=0):
         """Writes the uint8 level map of `row` (1..255, or 256 for mask > 0) to `d_levels_ptr` (16-byte aligned):
         floor((floor(x) - low) / bin_width) + 1 on the row's non-NaN voxels, 0 elsewhere (`stream` as for apply_dev)."""
@@ -362,6 +364,27 @@ class Engine:
         offsets = np.concatenate([[0], np.cumsum(n_pairs)])
         total = int(offsets[-1])
         return {"n_pairs": n_pairs, "sizes": sizes[:total].copy(), "counts": counts[:total].copy(), "offsets": offsets}
+
+    def glrlm_dev(self, d_levels_ptr, shape, n_levels, stream=0):
+        """-> int64 (13, n_levels, max(shape)): the runs of level i + 1 and length k + 1 of a uint8 level map along each
+        direction d of lm_glcm_dev."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ng = int(n_levels)
+        counts = np.zeros((13, max(ng, 1), max(n0, n1, n2, 1)), np.int64)
+        _check(lib().lm_glrlm_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, ng, _ptr(counts),
+                                  C.c_void_p(int(stream)) if stream else None))
+        return counts
+
+    def neighbour_counts_dev(self, d_levels_ptr, shape, n_levels, alpha=0, stream=0):
+        """-> (G, N, A), each int64 (n_levels, 27), of a uint8 level map: G(i, c) the voxels of level i + 1 with c
+        neighbours in the ROI within `alpha` levels, N(i, W) those with W neighbours in the ROI, A(i, W) the sum of
+        |W (i + 1) - S| over them (S the sum of the neighbours' levels)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ng = int(n_levels)
+        G, N, A = (np.zeros((max(ng, 1), 27), np.int64) for _ in range(3))
+        _check(lib().lm_neighbour_counts_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, ng, int(alpha), _ptr(G), _ptr(N),
+                                             _ptr(A), C.c_void_p(int(stream)) if stream else None))
+        return G, N, A
 
     # ---- mesh shape support (lm_shape_sums_dev, lm_max_diameters_dev)
     def shape_sums_dev(self, d_mask_ptr, shape, stream=0):

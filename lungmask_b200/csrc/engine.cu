@@ -197,7 +197,8 @@ struct lm_engine {
   LabelStatsWork stats;   // lm_label_stats_dev: counts, histograms and selection state
   ClusterWork clusters;   // lm_laa_clusters_dev: LAA maps, union-find parents, cluster sizes, size histogram
   RegionWork regions;     // lm_plane_label_counts_dev, lm_surface_distance_dev, lm_region_map_dev: EDT stacks, counts, LUT
-  TextureWork texture;    // lm_texture_levels_dev, lm_glcm_dev: error flag, pair counts (lm_zone_sizes_dev uses `clusters`)
+  TextureWork texture;    // lm_texture_levels_dev, lm_glcm_dev, lm_glrlm_dev, lm_neighbour_counts_dev: error flag, counters
+                          // (lm_zone_sizes_dev uses `clusters`)
   ShapeWork shape;        // lm_shape_sums_dev, lm_max_diameters_dev: sums, line tables, diameter candidates
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
@@ -1191,7 +1192,7 @@ int lm_region_map_dev(lm_engine* e, const uint8_t* d_mask, const float* d_dist, 
   return 0;
 }
 
-// The argument checks the three texture calls share: the shape (fewer than 2^32 voxels) and n_levels.
+// The argument checks the texture calls share: the shape (fewer than 2^32 voxels).
 static int check_texture_volume(const char* fn, int n0, int n1, int n2) {
   if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
   const size_t n = (size_t)n0 * n1 * n2;
@@ -1230,6 +1231,31 @@ int lm_glcm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, i
   if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
   RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
   const int rc = glcm(e->texture, d_levels, n0, n1, n2, n_levels, counts, e->num_sms, e->st, &e->launches);
+  if (rc) return texture_device_error(fn, rc, n_levels);
+  return 0;
+}
+
+int lm_glrlm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts, void* stream) {
+  static const char* fn = "lm_glrlm_dev";
+  if (!e || !d_levels || !counts) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  const int rc = glrlm(e->texture, d_levels, n0, n1, n2, n_levels, counts, e->num_sms, e->st, &e->launches);
+  if (rc) return texture_device_error(fn, rc, n_levels);
+  return 0;
+}
+
+int lm_neighbour_counts_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                            int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums, void* stream) {
+  static const char* fn = "lm_neighbour_counts_dev";
+  if (!e || !d_levels || !dependence || !ngtdm_counts || !ngtdm_sums) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  if (alpha < 0) return fail(-1, "%s: alpha %d is negative", fn, alpha);
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  const int rc = neighbour_counts(e->texture, d_levels, n0, n1, n2, n_levels, alpha, dependence, ngtdm_counts, ngtdm_sums,
+                                  e->num_sms, e->st, &e->launches);
   if (rc) return texture_device_error(fn, rc, n_levels);
   return 0;
 }

@@ -1,4 +1,5 @@
-// Grey-level texture matrices of one ROI (lm_texture_levels_dev, lm_glcm_dev, DESIGN §4.9).
+// Grey-level texture matrices of one ROI (lm_texture_levels_dev, lm_glcm_dev, lm_glrlm_dev, lm_neighbour_counts_dev,
+// DESIGN §4.9).
 //
 //   levels  reads the mask as 16-byte vectors and the value only under the row; writes the row's discretised level (0
 //           outside the ROI) 16 bytes at a time, the last partial chunk byte by byte.  A level outside 1..n_levels or a
@@ -8,6 +9,13 @@
 //           (__match_any_sync).  Parenchyma fills a few near-diagonal bins, so the counters are privatised in shared
 //           memory: the whole upper triangle of every direction while n_levels <= kSmemLevels, above that the band
 //           j - i < kBand (where nearly all pairs of neighbouring voxels fall) with the rest going to global atomics.
+//   glrlm   the same layout: for each direction d a lane whose voxel starts a run (its predecessor v - d is outside the
+//           array, outside the ROI or at another level) walks along d to the run's end and counts the run once; lanes
+//           with equal (level, length) keys add with one atomic.  Runs up to a length derived from n_levels are counted
+//           in shared memory, longer ones with global atomics.
+//   neighbour  the same layout: each ROI voxel reads its 26 neighbours and forms, in registers, W (neighbours in the
+//           ROI), S (the sum of their levels) and c (those within alpha of its level); G(i, c), N(i, W) and
+//           A(i, W) += |W i - S| are warp-aggregated by key into shared counters that hold every level.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -27,6 +35,7 @@ constexpr int kThreads = 512;
 constexpr int kSmemLevels = 90;    // triangle of 13 directions: 13 x 4095 x 4 B = 212,940 B
 constexpr int kBand = 16;          // n_levels > kSmemLevels: 13 x 255 x 16 x 4 B = 212,160 B
 constexpr unsigned kFull = 0xffffffffu;
+constexpr int kSmemWords = 53235;  // the shared budget of the GLCM triangle, 212,940 B, in 4-byte counters
 
 // ---- levels ---------------------------------------------------------------------------------------------------------
 // flag bit 0: a level outside 1..n_levels, bit 1: a non-finite value.
@@ -129,6 +138,120 @@ __global__ void __launch_bounds__(kThreads) glcm_kernel(const uint8_t* __restric
     const int d = k / per_dir, e = k % per_dir;
     const int t = kTri ? e : tri(e % ng + 1, e % ng + 1 + e / ng, ng);
     atomicAdd(&counts[(size_t)d * t_len + t], s_cnt[k]);
+  }
+}
+
+// ---- GLRLM ----------------------------------------------------------------------------------------------------------
+// counts: global [13][ng][max_len] uint32 (a direction holds at most n runs).  Shared s[d][i - 1][len - 1] for
+// len <= k_short; longer runs go straight to global.
+__global__ void __launch_bounds__(kThreads) glrlm_kernel(const uint8_t* __restrict__ lev, int n0, int n1, int n2, int ng,
+                                                         int max_len, int k_short, uint32_t* __restrict__ counts,
+                                                         int* __restrict__ flag) {
+  extern __shared__ uint32_t s_runs[];
+  const int per_dir = ng * k_short;
+  for (int i = threadIdx.x; i < kGlcmDirections * per_dir; i += blockDim.x) s_runs[i] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const size_t warp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5, n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+  const int runs_x = (n2 + 31) / 32;
+  const size_t segs = (size_t)n0 * n1 * runs_x;
+  for (size_t r = warp; r < segs; r += n_warps) {   // warp-uniform
+    const size_t line = r / runs_x;
+    const int x = (int)(r % runs_x) * 32 + lane, y = (int)(line % n1), z = (int)(line / n1);
+    const size_t v = line * n2 + x;
+    int a = x < n2 ? lev[v] : 0;
+    if (a > ng) { atomicOr(flag, 1); a = 0; }
+    if (!__any_sync(kFull, a != 0)) continue;
+#pragma unroll 1
+    for (int d = 0; d < kGlcmDirections; ++d) {
+      const int dz = dir_z(d), dy = dir_y(d), dx = dir_x(d);
+      const long long step = ((long long)dz * n1 + dy) * n2 + dx;
+      int len = 0;
+      if (a) {
+        const int pz = z - dz, py = y - dy, px = x - dx;
+        const bool continues = pz >= 0 && (unsigned)py < (unsigned)n1 && (unsigned)px < (unsigned)n2 &&
+                               lev[(size_t)((long long)v - step)] == a;
+        if (!continues) {   // v starts a run: walk to its end
+          len = 1;
+          int zz = z + dz, yy = y + dy, xx = x + dx;
+          long long u = (long long)v + step;
+          while (zz < n0 && (unsigned)yy < (unsigned)n1 && (unsigned)xx < (unsigned)n2 && lev[(size_t)u] == a) {
+            ++len;
+            zz += dz, yy += dy, xx += dx, u += step;
+          }
+        }
+      }
+      const unsigned long long key = len ? ((unsigned long long)len << 8) | (unsigned)a : 0ull;
+      const unsigned peers = __match_any_sync(kFull, key);
+      if (len && lane == __ffs(peers) - 1) {
+        if (len <= k_short) atomicAdd(&s_runs[d * per_dir + (a - 1) * k_short + len - 1], (uint32_t)__popc(peers));
+        else atomicAdd(&counts[((size_t)d * ng + a - 1) * max_len + len - 1], (uint32_t)__popc(peers));
+      }
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < kGlcmDirections * per_dir; k += blockDim.x) {
+    if (!s_runs[k]) continue;
+    const int d = k / per_dir, e = k % per_dir;
+    atomicAdd(&counts[((size_t)d * ng + e / k_short) * max_len + e % k_short], s_runs[k]);
+  }
+}
+
+// ---- GLDM / NGTDM ---------------------------------------------------------------------------------------------------
+// Per (level i, 0..26) cell: dependence G(i, c), count N(i, W), sum A(i, W).  Shared: the uint64 sums, then the two
+// uint32 arrays, ng * 27 each (110,160 B at ng = 255).
+__global__ void __launch_bounds__(kThreads) neighbour_kernel(const uint8_t* __restrict__ lev, int n0, int n1, int n2, int ng,
+                                                             int alpha, uint32_t* __restrict__ dep, uint32_t* __restrict__ cnt,
+                                                             unsigned long long* __restrict__ sums, int* __restrict__ flag) {
+  extern __shared__ unsigned long long s_sum[];
+  const int cells = ng * kNeighbourCells;
+  uint32_t* s_dep = reinterpret_cast<uint32_t*>(s_sum + cells);
+  uint32_t* s_cnt = s_dep + cells;
+  for (int i = threadIdx.x; i < cells; i += blockDim.x) s_sum[i] = 0, s_dep[i] = 0, s_cnt[i] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const size_t warp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5, n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+  const int runs_x = (n2 + 31) / 32;
+  const size_t segs = (size_t)n0 * n1 * runs_x;
+  for (size_t r = warp; r < segs; r += n_warps) {   // warp-uniform
+    const size_t line = r / runs_x;
+    const int x = (int)(r % runs_x) * 32 + lane, y = (int)(line % n1), z = (int)(line / n1);
+    const size_t v = line * n2 + x;
+    int a = x < n2 ? lev[v] : 0;
+    if (a > ng) { atomicOr(flag, 1); a = 0; }
+    if (!__any_sync(kFull, a != 0)) continue;
+    int w = 0, s = 0, c = 0;
+    if (a) {
+#pragma unroll
+      for (int k = 0; k < 27; ++k) {
+        if (k == 13) continue;   // the voxel itself
+        const int dz = k / 9 - 1, dy = k / 3 % 3 - 1, dx = k % 3 - 1;
+        const int zz = z + dz, yy = y + dy, xx = x + dx;
+        int b = 0;
+        if ((unsigned)zz < (unsigned)n0 && (unsigned)yy < (unsigned)n1 && (unsigned)xx < (unsigned)n2)
+          b = lev[(size_t)((long long)v + ((long long)dz * n1 + dy) * n2 + dx)];
+        if (b > ng) b = 0;   // flagged by the lane that holds it
+        if (b) {
+          ++w;
+          s += b;
+          c += abs(b - a) <= alpha;
+        }
+      }
+    }
+    const int kd = a ? (a - 1) * kNeighbourCells + c : -1, kn = a ? (a - 1) * kNeighbourCells + w : -1;
+    const unsigned pd = __match_any_sync(kFull, kd), pn = __match_any_sync(kFull, kn);
+    const unsigned sum = __reduce_add_sync(pn, (unsigned)abs(w * a - s));   // < 32 * 2^13 over a peer group
+    if (a && lane == __ffs(pd) - 1) atomicAdd(&s_dep[kd], (uint32_t)__popc(pd));
+    if (a && lane == __ffs(pn) - 1) {
+      atomicAdd(&s_cnt[kn], (uint32_t)__popc(pn));
+      if (sum) atomicAdd(&s_sum[kn], (unsigned long long)sum);
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < cells; k += blockDim.x) {
+    if (s_dep[k]) atomicAdd(&dep[k], s_dep[k]);
+    if (s_cnt[k]) atomicAdd(&cnt[k], s_cnt[k]);
+    if (s_sum[k]) atomicAdd(&sums[k], s_sum[k]);
   }
 }
 
@@ -240,6 +363,61 @@ int glcm(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_
   const int rc = flag_result(flag, st);
   if (rc) return rc;
   for (size_t k = 0; k < total; ++k) counts[k] = h[k];
+  return 0;
+}
+
+int glrlm(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int64_t* counts, int num_sms,
+          cudaStream_t st, int64_t* launches) {
+  const int max_len = std::max(n0, std::max(n1, n2));
+  const int k_short = std::min(kSmemWords / (kGlcmDirections * n_levels), max_len);
+  const size_t total = (size_t)kGlcmDirections * n_levels * max_len;
+  SC((cudaError_t)w.reserve(align256(sizeof(int)) + align256(total * 4)));
+  int* flag = static_cast<int*>(w.d);
+  uint32_t* d_counts = reinterpret_cast<uint32_t*>(static_cast<char*>(w.d) + align256(sizeof(int)));
+  SC(cudaMemsetAsync(flag, 0, sizeof(int), st));
+  SC(cudaMemsetAsync(d_counts, 0, total * 4, st));
+  const size_t threads = (size_t)n0 * n1 * ((n2 + 31) / 32) * 32;
+  const size_t smem = (size_t)kGlcmDirections * n_levels * k_short * 4;
+  SC(cudaFuncSetAttribute(glrlm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  glrlm_kernel<<<grid_for(glrlm_kernel, smem, threads, num_sms), kThreads, smem, st>>>(d_levels, n0, n1, n2, n_levels, max_len,
+                                                                                      k_short, d_counts, flag);
+  SC(cudaGetLastError());
+  ++*launches;
+  std::vector<uint32_t> h(total);
+  SC(cudaMemcpyAsync(h.data(), d_counts, total * 4, cudaMemcpyDeviceToHost, st));
+  const int rc = flag_result(flag, st);
+  if (rc) return rc;
+  for (size_t k = 0; k < total; ++k) counts[k] = h[k];
+  return 0;
+}
+
+int neighbour_counts(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                     int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums, int num_sms, cudaStream_t st,
+                     int64_t* launches) {
+  const size_t cells = (size_t)n_levels * kNeighbourCells;
+  const size_t sums_at = align256(sizeof(int)), dep_at = sums_at + align256(cells * 8), cnt_at = dep_at + align256(cells * 4);
+  SC((cudaError_t)w.reserve(cnt_at + align256(cells * 4)));
+  char* base = static_cast<char*>(w.d);
+  int* flag = reinterpret_cast<int*>(base);
+  unsigned long long* d_sums = reinterpret_cast<unsigned long long*>(base + sums_at);
+  uint32_t* d_dep = reinterpret_cast<uint32_t*>(base + dep_at);
+  uint32_t* d_cnt = reinterpret_cast<uint32_t*>(base + cnt_at);
+  SC(cudaMemsetAsync(base, 0, cnt_at + cells * 4, st));
+  const size_t threads = (size_t)n0 * n1 * ((n2 + 31) / 32) * 32;
+  const size_t smem = cells * 16;
+  SC(cudaFuncSetAttribute(neighbour_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  neighbour_kernel<<<grid_for(neighbour_kernel, smem, threads, num_sms), kThreads, smem, st>>>(d_levels, n0, n1, n2, n_levels,
+                                                                                              alpha, d_dep, d_cnt, d_sums, flag);
+  SC(cudaGetLastError());
+  ++*launches;
+  std::vector<unsigned long long> hs(cells);
+  std::vector<uint32_t> hd(cells), hc(cells);
+  SC(cudaMemcpyAsync(hs.data(), d_sums, cells * 8, cudaMemcpyDeviceToHost, st));
+  SC(cudaMemcpyAsync(hd.data(), d_dep, cells * 4, cudaMemcpyDeviceToHost, st));
+  SC(cudaMemcpyAsync(hc.data(), d_cnt, cells * 4, cudaMemcpyDeviceToHost, st));
+  const int rc = flag_result(flag, st);
+  if (rc) return rc;
+  for (size_t k = 0; k < cells; ++k) dependence[k] = hd[k], ngtdm_counts[k] = hc[k], ngtdm_sums[k] = (int64_t)hs[k];
   return 0;
 }
 

@@ -466,19 +466,21 @@ def save_clusters(path, clusters):
 
 
 def save_texture(path, texture):
-    """Writes the TextureFeatures of LMInferer.texture: .json (spacing, bin_width and one object per row with its GLCM and
-    GLSZM features and the GLSZM (level, size, count) triples, NaN as null) or .csv (a header, then one line per row:
-    label, name, voxels, low, bin_width, n_levels, glcm_<Name>..., glszm_<Name>...; an unknown value is an empty cell,
-    NaN is "nan")."""
+    """Writes the TextureFeatures of LMInferer.texture: .json (spacing, bin_width and one object per row with the
+    features of every computed class and their exact matrices, such as the GLSZM (level, size, count) triples, NaN as
+    null) or .csv (a header, then one line per row: label, name, voxels, low, bin_width, n_levels, then <class>_<Name>
+    for every computed class in the order glcm, glszm, glrlm, gldm, ngtdm; an unknown value is an empty cell, NaN is
+    "nan")."""
     check_table_path(path, "texture")
     if path.lower().endswith(".json"):
         return _save_json(path, texture)
-    from .texture import GLCM_FEATURES, GLSZM_FEATURES, TextureRow
-    header = list(TextureRow.SUMMARY) + ["glcm_" + k for k in GLCM_FEATURES] + ["glszm_" + k for k in GLSZM_FEATURES]
+    from .texture import CLASSES, GLCM_FEATURES, GLDM_FEATURES, GLRLM_FEATURES, GLSZM_FEATURES, NGTDM_FEATURES, TextureRow
+    names = dict(zip(CLASSES, (GLCM_FEATURES, GLSZM_FEATURES, GLRLM_FEATURES, GLDM_FEATURES, NGTDM_FEATURES)))
+    columns = [(c, k) for c in CLASSES if c in texture.classes for k in names[c]]
+    header = list(TextureRow.SUMMARY) + ["%s_%s" % ck for ck in columns]
     lines = [",".join(header)]
     for r in texture.rows:
-        cells = [getattr(r, k) for k in TextureRow.SUMMARY] + [r.glcm[k] for k in GLCM_FEATURES] + \
-            [r.glszm[k] for k in GLSZM_FEATURES]
+        cells = [getattr(r, k) for k in TextureRow.SUMMARY] + [getattr(r, c)[k] for c, k in columns]
         lines.append(",".join(_csv_cell(v) for v in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")

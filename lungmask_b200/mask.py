@@ -476,8 +476,8 @@ class LMInferer:
         return rg.build(labels, present, self.modelname, s.spacing, counts, axis, superior_high, zones, zone_by, shells_mm, q, t,
                         label_zones, lung_zones, zone, zone_lung, shell, shell_lung)
 
-    def texture(self, image, mask, bin_width=25, spacing=None):
-        """GLCM and GLSZM texture features of `image` under `mask` -> lungmask_b200.texture.TextureFeatures, with the rows
+    def texture(self, image, mask, bin_width=25, spacing=None, classes=("glcm", "glszm"), gldm_alpha=0):
+        """Grey-level texture features of `image` under `mask` -> lungmask_b200.texture.TextureFeatures, with the rows
         of `statistics`: every label value in the mask and every label 1..K-1 of the model (absent ones with 0 voxels and
         NaN features), then "lung" (mask > 0).  A row's ROI is its voxels with a non-NaN value, read in the volume's dtype
         (float16 / bfloat16 as float32); a non-finite value in an ROI is a ValueError.
@@ -491,6 +491,14 @@ class LMInferer:
         the PyRadiomics names of texture.GLCM_FEATURES / GLSZM_FEATURES) and the exact matrices: the pair counts
         `glcm_counts` (13, Ng (Ng + 1) / 2) and the (level, size, count) `zones`.
 
+        `classes` is a non-empty collection of the names "glcm", "glszm", "glrlm", "gldm" and "ngtdm", in any order; only
+        those are computed, and only their keys appear in to_dict() and the writers.  GLRLM: the maximal runs of equal
+        level along the 13 directions, features averaged over the directions; `glrlm_runs` holds the (direction, level,
+        length, count) rows.  GLDM: per voxel the number c of its 26 neighbours in the row within `gldm_alpha` levels (a
+        non-negative integer, PyRadiomics' gldm_a), dependence size c + 1; `gldm_counts` (Ng, 27).  NGTDM: per voxel the
+        number W of its neighbours in the row and the sum S of their levels; `ngtdm_counts` N(i, W) and `ngtdm_sums`
+        A(i, W) = sum |W i - S|, (Ng, 27).  A bad `classes` or `gldm_alpha` raises before any kernel runs.
+
         `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image, CPU tensors, or CUDA
         tensors on the engine's device read in place after the work queued on the current stream; both are left
         unchanged."""
@@ -498,6 +506,8 @@ class LMInferer:
         from . import texture as tx
         from .statistics import label_name
         bw = tx.check_arguments(bin_width)
+        classes = tx.check_classes(classes)
+        alpha = tx.check_alpha(gldm_alpha)
         s = self._stage("texture", image, mask, spacing)
         shape = tuple(s.mask.shape)
         st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, (), (), stream=s.stream)
@@ -514,15 +524,24 @@ class LMInferer:
         levels = torch.empty(shape, dtype=torch.uint8, device=s.mask.device) if plan else None
         for r in rows:
             if r not in plan:
-                out.append(tx.build_row(r, names[r], 0, bw))
+                out.append(tx.build_row(r, names[r], 0, bw, classes=classes))
                 continue
             n, low, ng = plan[r]
             self.engine.texture_levels_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, r, low, bw, ng,
                                            levels.data_ptr(), stream=s.stream)
-            U = self.engine.glcm_dev(levels.data_ptr(), shape, ng, stream=s.stream)
-            zones = tx.zones_from_native(self.engine.zone_sizes_dev(levels.data_ptr(), shape, stream=s.stream))
-            out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones))
-        return tx.TextureFeatures(s.spacing, bw, out)
+            U = zones = runs = neighbours = None
+            if "glcm" in classes:
+                U = self.engine.glcm_dev(levels.data_ptr(), shape, ng, stream=s.stream)
+            if "glszm" in classes:
+                zones = tx.zones_from_native(self.engine.zone_sizes_dev(levels.data_ptr(), shape, stream=s.stream))
+            if "glrlm" in classes:
+                runs = self.engine.glrlm_dev(levels.data_ptr(), shape, ng, stream=s.stream)
+            if "gldm" in classes or "ngtdm" in classes:
+                # |level difference| <= ng - 1 always, so a larger alpha counts the same neighbours
+                neighbours = self.engine.neighbour_counts_dev(levels.data_ptr(), shape, ng, min(alpha, tx.MAX_LEVELS),
+                                                              stream=s.stream)
+            out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones, classes, runs, neighbours))
+        return tx.TextureFeatures(s.spacing, bw, out, classes, alpha)
 
     def shape(self, mask, spacing=None, image=None):
         """Mesh shape features of every row of `statistics` -> lungmask_b200.shape.ShapeFeatures: every label value in the

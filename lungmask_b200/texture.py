@@ -1,14 +1,18 @@
-"""GLCM and GLSZM texture features per lung and lobe: the result of LMInferer.texture (lm_texture_levels_dev, lm_glcm_dev,
-lm_zone_sizes_dev; DESIGN §4.9).
+"""GLCM, GLSZM, GLRLM, GLDM and NGTDM texture features per lung and lobe: the result of LMInferer.texture
+(lm_texture_levels_dev, lm_glcm_dev, lm_zone_sizes_dev, lm_glrlm_dev, lm_neighbour_counts_dev; DESIGN §4.9).
 
 Every row of `statistics` (each label, then "lung", mask > 0) is discretised with a fixed bin width as PyRadiomics does:
 low = bw * floor(min / bw) and level(x) = floor((floor(x) - low) / bw) + 1, so the row's minimum has level 1 and its
-maximum level Ng.  Two matrices of the level map are counted exactly on the GPU:
+maximum level Ng.  The matrices of the level map are counted exactly on the GPU:
   GLCM   for each of the 13 directions d of the 26-neighbourhood, the symmetric co-occurrence matrix of the voxel pairs
          (v, v + d) with both voxels in the row; the features are computed per direction and averaged over the
          directions that have pairs.
   GLSZM  the number of 26-connected zones of equal level per (level, zone size).
-The feature formulas are those of PyRadiomics (see glcm_features / glszm_features; the differences are listed in DESIGN
+  GLRLM  for each of the 13 directions, the number of maximal runs of equal level per (level, run length); the features
+         are averaged over the directions.
+  GLDM   the number of voxels per (level, number of the 26 neighbours in the row within gldm_alpha levels).
+  NGTDM  per level, the voxels that have neighbours in the row and the sum of |level - mean level of the neighbours|.
+The feature formulas are those of PyRadiomics (see the *_features functions; the differences are listed in DESIGN
 §4.9).  Everything here is pure numpy in float64; the tests apply the same functions to reference matrices.
 """
 import math
@@ -33,6 +37,28 @@ GLSZM_FEATURES = ("SmallAreaEmphasis", "LargeAreaEmphasis", "GrayLevelNonUniform
                   "SmallAreaLowGrayLevelEmphasis", "SmallAreaHighGrayLevelEmphasis", "LargeAreaLowGrayLevelEmphasis",
                   "LargeAreaHighGrayLevelEmphasis")
 
+# GLRLM and GLDM use the GLSZM formulas with runs / dependence sizes in place of zones (glszm_features); these are the
+# GLSZM names they take, in the order of GLRLM_FEATURES and GLDM_FEATURES.
+GLRLM_FEATURES = ("ShortRunEmphasis", "LongRunEmphasis", "GrayLevelNonUniformity", "GrayLevelNonUniformityNormalized",
+                  "RunLengthNonUniformity", "RunLengthNonUniformityNormalized", "RunPercentage", "GrayLevelVariance",
+                  "RunVariance", "RunEntropy", "LowGrayLevelRunEmphasis", "HighGrayLevelRunEmphasis",
+                  "ShortRunLowGrayLevelEmphasis", "ShortRunHighGrayLevelEmphasis", "LongRunLowGrayLevelEmphasis",
+                  "LongRunHighGrayLevelEmphasis")
+GLDM_FEATURES = ("SmallDependenceEmphasis", "LargeDependenceEmphasis", "GrayLevelNonUniformity", "DependenceNonUniformity",
+                 "DependenceNonUniformityNormalized", "GrayLevelVariance", "DependenceVariance", "DependenceEntropy",
+                 "LowGrayLevelEmphasis", "HighGrayLevelEmphasis", "SmallDependenceLowGrayLevelEmphasis",
+                 "SmallDependenceHighGrayLevelEmphasis", "LargeDependenceLowGrayLevelEmphasis",
+                 "LargeDependenceHighGrayLevelEmphasis")
+_GLDM_AS_GLSZM = ("SmallAreaEmphasis", "LargeAreaEmphasis", "GrayLevelNonUniformity", "SizeZoneNonUniformity",
+                  "SizeZoneNonUniformityNormalized", "GrayLevelVariance", "ZoneVariance", "ZoneEntropy",
+                  "LowGrayLevelZoneEmphasis", "HighGrayLevelZoneEmphasis", "SmallAreaLowGrayLevelEmphasis",
+                  "SmallAreaHighGrayLevelEmphasis", "LargeAreaLowGrayLevelEmphasis", "LargeAreaHighGrayLevelEmphasis")
+NGTDM_FEATURES = ("Coarseness", "Contrast", "Busyness", "Complexity", "Strength")
+
+CLASSES = ("glcm", "glszm", "glrlm", "gldm", "ngtdm")
+DEFAULT_CLASSES = ("glcm", "glszm")
+NEIGHBOURS = 27   # the columns of the GLDM / NGTDM matrices: c or W = 0..26 neighbours
+
 _EPS = np.spacing(1)
 
 
@@ -45,6 +71,31 @@ def check_arguments(bin_width):
     if int(v) < 1:
         raise ValueError("bin_width must be a positive integer, got %d" % int(v))
     return int(v)
+
+
+def check_classes(classes):
+    """-> the texture classes as a tuple in the order of CLASSES: a non-empty collection of names from CLASSES.
+    TypeError for a string or a non-string name, ValueError for an unknown name or an empty collection."""
+    if isinstance(classes, (str, bytes)):
+        raise TypeError("classes must be a collection of names such as ('glcm', 'glrlm'), got the string %r" % (classes,))
+    names = list(classes)
+    for c in names:
+        if not isinstance(c, str):
+            raise TypeError("classes: %r is not a name" % (c,))
+        if c not in CLASSES:
+            raise ValueError("classes: unknown texture class %r (known: %s)" % (c, ", ".join(CLASSES)))
+    if not names:
+        raise ValueError("classes: at least one of %s is needed" % ", ".join(CLASSES))
+    return tuple(c for c in CLASSES if c in names)
+
+
+def check_alpha(alpha):
+    """-> the GLDM coarseness parameter as a non-negative int; TypeError / ValueError otherwise."""
+    if isinstance(alpha, (bool, np.bool_)) or not isinstance(alpha, (int, np.integer)):
+        raise TypeError("gldm_alpha must be an integer, got %r" % (alpha,))
+    if int(alpha) < 0:
+        raise ValueError("gldm_alpha must be a non-negative integer, got %d" % int(alpha))
+    return int(alpha)
 
 
 def discretisation(vmin, vmax, bin_width, row="the ROI"):
@@ -178,6 +229,72 @@ def glszm_features(levels, sizes, counts, n_voxels):
     return {name: float(f[name]) for name in GLSZM_FEATURES}
 
 
+def glrlm_features(counts):
+    """The GLRLM features of the run counts (13, Ng, L) int64 of lm_glrlm_dev (runs of level i + 1 and length k + 1
+    along direction d): per direction the GLSZM formulas with runs for zones and lengths for sizes, Nr = the runs and
+    Np = sum k P_d(i, k) (the ROI voxels), then the mean over the directions with runs.  All NaN without runs."""
+    per = []
+    for p in np.asarray(counts, dtype=np.int64):
+        i, k = np.nonzero(p)
+        if i.size == 0:
+            continue
+        c = p[i, k]
+        f = glszm_features(i + 1, k + 1, c, int(np.sum((k + 1) * c)))
+        per.append(dict(zip(GLRLM_FEATURES, (f[g] for g in GLSZM_FEATURES))))
+    if not per:
+        return {name: float("nan") for name in GLRLM_FEATURES}
+    return {name: float(np.mean([f[name] for f in per])) for name in GLRLM_FEATURES}
+
+
+def gldm_features(G):
+    """The GLDM features of the dependence counts G (Ng, 27) int64 of lm_neighbour_counts_dev (voxels of level i + 1 with
+    c neighbours within alpha): the GLSZM formulas with dependence size j = c + 1 for the zone size and Nz = sum G = Np.
+    All NaN without voxels."""
+    G = np.asarray(G, dtype=np.int64).reshape(-1, NEIGHBOURS)
+    i, c = np.nonzero(G)
+    f = glszm_features(i + 1, c + 1, G[i, c], int(G.sum()))
+    return dict(zip(GLDM_FEATURES, (f[g] for g in _GLDM_AS_GLSZM)))
+
+
+def ngtdm_features(N, A):
+    """The NGTDM features of the counts N (Ng, 27) and sums A (Ng, 27) int64 of lm_neighbour_counts_dev (voxels of level
+    i + 1 with W neighbours in the ROI, and the sum of |W (i + 1) - S| over them).  Voxels without neighbours are left
+    out: n_i = sum_{W >= 1} N(i, W), s_i = sum_{W >= 1} A(i, W) / W (math.fsum), Nvp = sum n_i, p_i = n_i / Nvp; the sums
+    run over the Ngp levels with p_i > 0.  All NaN when Nvp = 0."""
+    N = np.asarray(N, dtype=np.int64).reshape(-1, NEIGHBOURS)
+    A = np.asarray(A, dtype=np.int64).reshape(-1, NEIGHBOURS)
+    n = N[:, 1:].sum(axis=1)
+    nvp = int(n.sum())
+    if nvp == 0:
+        return {name: float("nan") for name in NGTDM_FEATURES}
+    keep = np.nonzero(n)[0]
+    i = (keep + 1).astype(np.float64)
+    p = n[keep] / float(nvp)
+    s = np.array([math.fsum(float(A[l, w]) / w for w in range(1, NEIGHBOURS)) for l in keep])
+    ngp = keep.size
+    ps = p * s
+    sum_ps, sum_s = np.sum(ps), np.sum(s)
+    dist = np.abs(i[:, None] - i[None, :])
+    d2 = dist ** 2
+    ip = i * p
+    busy = np.sum(np.abs(ip[:, None] - ip[None, :]))
+    f = {
+        "Coarseness": 1e6 if sum_ps == 0 else 1.0 / sum_ps,
+        "Contrast": 0.0 if ngp == 1 else np.sum(p[:, None] * p[None, :] * d2) / (ngp * (ngp - 1)) * sum_s / nvp,
+        "Busyness": 0.0 if busy == 0 else sum_ps / busy,
+        "Complexity": np.sum(dist * (ps[:, None] + ps[None, :]) / (p[:, None] + p[None, :])) / nvp,
+        "Strength": 0.0 if sum_s == 0 else np.sum((p[:, None] + p[None, :]) * d2) / sum_s,
+    }
+    return {name: float(f[name]) for name in NGTDM_FEATURES}
+
+
+def runs_from_counts(counts):
+    """(k, 4) int64 (direction, level, length, count) rows of the non-zero run counts (13, Ng, L), sorted."""
+    P = np.asarray(counts, dtype=np.int64)
+    d, i, k = np.nonzero(P)
+    return np.stack([d, i + 1, k + 1, P[d, i, k]], axis=1).astype(np.int64).reshape(-1, 4)
+
+
 def _json_value(v):
     return None if isinstance(v, float) and math.isnan(v) else v
 
@@ -190,18 +307,37 @@ class TextureRow:
     low: Optional[int]         # bin_width * floor(min / bin_width); None without voxels
     bin_width: int
     n_levels: int              # Ng, the level of the row's maximum; 0 without voxels
-    glcm: dict = field(default_factory=dict)    # GLCM_FEATURES -> float (NaN without pairs)
-    glszm: dict = field(default_factory=dict)   # GLSZM_FEATURES -> float (NaN without voxels)
+    # The feature dicts of a class that was not computed are None.
+    glcm: Optional[dict] = field(default_factory=dict)    # GLCM_FEATURES -> float (NaN without pairs)
+    glszm: Optional[dict] = field(default_factory=dict)   # GLSZM_FEATURES -> float (NaN without voxels)
     glcm_counts: np.ndarray = field(default_factory=lambda: np.zeros((len(OFFSETS), 0), np.int64))   # U, (13, T) int64
     zones: np.ndarray = field(default_factory=lambda: np.zeros((0, 3), np.int64))   # (level, size, count) int64 triples
+    glrlm: Optional[dict] = None   # GLRLM_FEATURES -> float (NaN without voxels)
+    gldm: Optional[dict] = None    # GLDM_FEATURES -> float (NaN without voxels)
+    ngtdm: Optional[dict] = None   # NGTDM_FEATURES -> float (NaN without a voxel that has a neighbour in the ROI)
+    glrlm_runs: Optional[np.ndarray] = None     # (direction, level, length, count) int64 rows, non-zero, sorted
+    gldm_counts: Optional[np.ndarray] = None    # G(i, c), (Ng, 27) int64
+    ngtdm_counts: Optional[np.ndarray] = None   # N(i, W), (Ng, 27) int64
+    ngtdm_sums: Optional[np.ndarray] = None     # A(i, W) = sum |W i - S|, (Ng, 27) int64
 
     SUMMARY = ("label", "name", "voxels", "low", "bin_width", "n_levels")
 
     def to_dict(self):
+        """JSON-ready: NaN becomes None; the keys of a class appear only when it was computed."""
         d = {k: _json_value(getattr(self, k)) for k in self.SUMMARY}
-        d["glcm"] = {k: _json_value(v) for k, v in self.glcm.items()}
-        d["glszm"] = {k: _json_value(v) for k, v in self.glszm.items()}
-        d["glszm_zones"] = [[int(x) for x in z] for z in self.zones]
+        for cls in CLASSES:
+            f = getattr(self, cls)
+            if f is not None:
+                d[cls] = {k: _json_value(v) for k, v in f.items()}
+            if cls == "glszm" and f is not None:
+                d["glszm_zones"] = [[int(x) for x in z] for z in self.zones]
+            elif cls == "glrlm" and f is not None:
+                d["glrlm_runs"] = self.glrlm_runs.tolist()
+            elif cls == "gldm" and f is not None:
+                d["gldm_counts"] = self.gldm_counts.tolist()
+            elif cls == "ngtdm" and f is not None:
+                d["ngtdm_counts"] = self.ngtdm_counts.tolist()
+                d["ngtdm_sums"] = self.ngtdm_sums.tolist()
         return d
 
 
@@ -210,6 +346,8 @@ class TextureFeatures:
     spacing: Optional[tuple]   # (x, y, z) mm, or None; the features do not use it
     bin_width: int
     rows: list
+    classes: tuple = DEFAULT_CLASSES   # the computed classes, in the order of CLASSES
+    gldm_alpha: int = 0
 
     def __getitem__(self, label):
         """The row of a label value, or of "lung"."""
@@ -219,9 +357,15 @@ class TextureFeatures:
         raise KeyError(label)
 
     def to_dict(self):
-        """JSON-ready: NaN becomes None."""
-        return {"spacing": list(self.spacing) if self.spacing is not None else None, "bin_width": self.bin_width,
-                "rows": [r.to_dict() for r in self.rows]}
+        """JSON-ready: NaN becomes None.  "classes" appears only when they are not DEFAULT_CLASSES, "gldm_alpha" only
+        with GLDM."""
+        d = {"spacing": list(self.spacing) if self.spacing is not None else None, "bin_width": self.bin_width}
+        if tuple(self.classes) != DEFAULT_CLASSES:
+            d["classes"] = list(self.classes)
+        if "gldm" in self.classes:
+            d["gldm_alpha"] = self.gldm_alpha
+        d["rows"] = [r.to_dict() for r in self.rows]
+        return d
 
 
 def zones_from_native(res):
@@ -230,12 +374,40 @@ def zones_from_native(res):
     return np.stack([lev, res["sizes"], res["counts"]], axis=1).astype(np.int64)
 
 
-def build_row(label, name, voxels, bin_width, low=None, n_levels=0, U=None, zones=None):
-    """The TextureRow of one row from its exact matrices; voxels == 0 gives an empty row with NaN features."""
+def build_row(label, name, voxels, bin_width, low=None, n_levels=0, U=None, zones=None, classes=DEFAULT_CLASSES, runs=None,
+              neighbours=None):
+    """The TextureRow of one row from its exact matrices; voxels == 0 gives an empty row with NaN features.  Only the
+    `classes` are filled in, from U and zones (GLCM, GLSZM), the run counts `runs` (13, Ng, L) of lm_glrlm_dev (GLRLM)
+    and the (G, N, A) `neighbours` of lm_neighbour_counts_dev (GLDM, NGTDM)."""
+    classes = check_classes(classes)
+    nan = lambda names: {k: float("nan") for k in names}   # noqa: E731
+    lab = UNION if label == 256 else label
     if voxels == 0:
-        return TextureRow(UNION if label == 256 else label, name, 0, None, int(bin_width), 0,
-                          {k: float("nan") for k in GLCM_FEATURES}, {k: float("nan") for k in GLSZM_FEATURES})
-    U = np.asarray(U, dtype=np.int64)
-    zones = np.asarray(zones, dtype=np.int64).reshape(-1, 3)
-    return TextureRow(UNION if label == 256 else label, name, int(voxels), int(low), int(bin_width), int(n_levels),
-                      glcm_features(U, n_levels), glszm_features(zones[:, 0], zones[:, 1], zones[:, 2], voxels), U, zones)
+        row = TextureRow(lab, name, 0, None, int(bin_width), 0, nan(GLCM_FEATURES), nan(GLSZM_FEATURES))
+        empty = np.zeros((0, NEIGHBOURS), np.int64)
+        row.glrlm, row.glrlm_runs = nan(GLRLM_FEATURES), np.zeros((0, 4), np.int64)
+        row.gldm, row.gldm_counts = nan(GLDM_FEATURES), empty
+        row.ngtdm, row.ngtdm_counts, row.ngtdm_sums = nan(NGTDM_FEATURES), empty, empty.copy()
+    else:
+        row = TextureRow(lab, name, int(voxels), int(low), int(bin_width), int(n_levels))
+        if "glcm" in classes:
+            row.glcm_counts = np.asarray(U, dtype=np.int64)
+            row.glcm = glcm_features(row.glcm_counts, n_levels)
+        if "glszm" in classes:
+            row.zones = np.asarray(zones, dtype=np.int64).reshape(-1, 3)
+            row.glszm = glszm_features(row.zones[:, 0], row.zones[:, 1], row.zones[:, 2], voxels)
+        if "glrlm" in classes:
+            row.glrlm_runs = runs_from_counts(runs)
+            row.glrlm = glrlm_features(runs)
+        if "gldm" in classes or "ngtdm" in classes:
+            G, N, A = (np.asarray(m, dtype=np.int64).reshape(-1, NEIGHBOURS) for m in neighbours)
+            row.gldm_counts, row.gldm = G, gldm_features(G)
+            row.ngtdm_counts, row.ngtdm_sums, row.ngtdm = N, A, ngtdm_features(N, A)
+    for cls in CLASSES:
+        if cls not in classes:
+            setattr(row, cls, None)
+    for cls, fields in (("gldm", ("gldm_counts",)), ("ngtdm", ("ngtdm_counts", "ngtdm_sums")), ("glrlm", ("glrlm_runs",))):
+        if cls not in classes:
+            for f in fields:
+                setattr(row, f, None)
+    return row

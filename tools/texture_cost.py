@@ -2,7 +2,10 @@
 """What the GLCM / GLSZM texture features cost: LMInferer.texture on CUDA tensors and on numpy arrays, the lm_glcm_dev
 call alone, and the same matrices on the host with numpy / scipy.
 
-    python tools/texture_cost.py [--out DIR] [--rounds 3]
+    python tools/texture_cost.py [--out DIR] [--rounds 3] [--classes glcm,glszm,glrlm,gldm,ngtdm]
+
+With --classes, the run below is replaced by the one of classes_cost: the GLRLM / GLDM / NGTDM calls alone and the
+whole call with those classes against the default one, on the int16 phantoms at both sizes and bin widths.
 
 Builds the engine as bench.py does (R231, the seeded weights of bench.get_weights) and runs, on two 300-slice phantoms
 (seed 100) at 256x256 and 512x512, each as int16 and as float32 (the int16 values plus a uniform fraction in [0, 1)),
@@ -30,6 +33,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))   # _texture_ref: the numpy GLRLM / GLDM / NGTDM references
 
 SLICES = 300
 
@@ -66,10 +70,75 @@ def host_rows(vol, mask, bw):
     return out
 
 
+def classes_cost(inferer, classes, rounds, info):
+    """--classes: on the int16 phantoms, lm_glrlm_dev and lm_neighbour_counts_dev alone on the "lung" row's level map,
+    and LMInferer.texture with `classes` and with the default classes, CUDA events around each call.  The "lung" row's
+    device matrices (of the calls alone and of the whole call) are checked against the numpy references of
+    tests/_texture_ref.py."""
+    import torch
+    from statistics_cost import lung_mask
+    from _texture_ref import glrlm_ref, neighbour_ref
+    from lungmask_b200 import texture as tx
+    from oracle import synth
+    classes = tx.check_classes(classes)
+    result = {"gpu": info, "workload": "300-slice int16 phantoms seed 100, two-lung ellipsoid mask, classes %s" % ",".join(classes),
+              "rounds": rounds, "unit": "ms", "cases": {}}
+    print("\n%-26s %5s %14s %14s %14s %14s" % ("case", "Ng", "glrlm ms", "neighbour ms", "call ms", "default ms"))
+    for H in (256, 512):
+        vol = synth.phantom(SLICES, H, H, seed=100)
+        mask = lung_mask(SLICES, H, H)
+        tv, tm = torch.from_numpy(vol).to("cuda:0"), torch.from_numpy(mask).to("cuda:0")
+        sel = mask > 0
+        for bw in (25, 10):
+            name = "%dx%dx%d int16 bw %d" % (SLICES, H, H, bw)
+            vals = vol[sel]
+            low, ng = tx.discretisation(float(vals.min()), float(vals.max()), bw)
+            L = np.zeros(vol.shape, np.uint8)
+            L[sel] = tx.levels(vals, bw, low)
+            P, (G, N, A) = glrlm_ref(L, ng), neighbour_ref(L, ng, 0)
+            tL = torch.from_numpy(L).to("cuda:0")
+            st = torch.cuda.current_stream().cuda_stream
+            inferer.texture(tv, tm, bin_width=bw, classes=classes)     # warm-up: work buffers, module load
+            inferer.texture(tv, tm, bin_width=bw)
+            times = {"glrlm": [], "neighbour": [], "call": [], "default": []}
+            for _ in range(rounds):
+                e = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
+                e[0].record()
+                runs = inferer.engine.glrlm_dev(tL.data_ptr(), L.shape, ng, stream=st)
+                e[1].record()
+                nb = inferer.engine.neighbour_counts_dev(tL.data_ptr(), L.shape, ng, 0, stream=st)
+                e[2].record()
+                res = inferer.texture(tv, tm, bin_width=bw, classes=classes)
+                e[3].record()
+                inferer.texture(tv, tm, bin_width=bw)
+                e[4].record()
+                e[4].synchronize()
+                for k, (a, b) in zip(times, ((0, 1), (1, 2), (2, 3), (3, 4))):
+                    times[k].append(e[a].elapsed_time(e[b]))
+                assert np.array_equal(runs, P) and all(np.array_equal(x, y) for x, y in zip(nb, (G, N, A))), name
+                r = res["lung"]
+                if "glrlm" in classes:
+                    assert np.array_equal(r.glrlm_runs, tx.runs_from_counts(P)), name
+                if "gldm" in classes:
+                    assert np.array_equal(r.gldm_counts, G), name
+                if "ngtdm" in classes:
+                    assert np.array_equal(r.ngtdm_counts, N) and np.array_equal(r.ngtdm_sums, A), name
+            med = {k: float(np.median(v)) for k, v in times.items()}
+            spread = {k: float(np.max(v) - np.min(v)) for k, v in times.items()}
+            result["cases"][name] = {"median": med, "spread": spread, "n_levels_lung": ng, "rounds": times}
+            print("%-26s %5d %7.2f (%5.2f) %7.2f (%5.2f) %7.1f (%5.1f) %7.1f (%5.1f)" % (
+                name, ng, med["glrlm"], spread["glrlm"], med["neighbour"], spread["neighbour"], med["call"], spread["call"],
+                med["default"], spread["default"]), flush=True)
+    return result
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", default=None, help="directory for texture_cost.json")
+    ap.add_argument("--out", default=None, help="directory for texture_cost.json (texture_classes_cost.json with --classes)")
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--classes", default=None,
+                    help="comma-separated texture classes, e.g. glcm,glszm,glrlm,gldm,ngtdm: time lm_glrlm_dev and "
+                         "lm_neighbour_counts_dev alone and the whole call with these classes instead of the default run")
     args = ap.parse_args()
 
     import torch
@@ -88,6 +157,13 @@ def main():
         inferer = LMInferer(modelname="R231", modelpath=wpath, batch_size=20, tqdm_disable=True, device=0)
     finally:
         os.remove(wpath)
+    if args.classes is not None:
+        result = classes_cost(inferer, [c.strip() for c in args.classes.split(",") if c.strip()], args.rounds, info)
+        if args.out:
+            os.makedirs(args.out, exist_ok=True)
+            with open(os.path.join(args.out, "texture_classes_cost.json"), "w") as f:
+                json.dump(result, f, indent=1)
+        return
     rng = np.random.default_rng(100)
     result = {"gpu": info, "workload": "300-slice phantoms seed 100, two-lung ellipsoid mask, GLCM + GLSZM per row",
               "rounds": args.rounds, "unit": "ms", "cases": {}}
