@@ -371,6 +371,9 @@ LM_API int lm_last_conv_timing(const lm_engine* e, float* conv_ms, int64_t* conv
  * 26 L3 27 U3 28 C3 (decoder: L = 1x1 conv below the upsample, U = upsampled, C = first conv, E = block output). */
 LM_API int lm_debug_activation_info(int act_id, int* level, int* channels, int* split);
 LM_API int lm_debug_read_activation(lm_engine* e, int act_id, int n, float* out);
+/* The power-of-two scale the split planes of activation `act_id` are stored at in weight slot `slot` (1 until a value
+ * of the tensor's scale group left fp16's range; 1 for the fp32 "L" tensors).  lm_load_weights resets it to 1. */
+LM_API int lm_debug_activation_scale(lm_engine* e, int slot, int act_id, float* scale);
 
 /* Forward-only benchmark hook: runs the forward pass on `S` device-resident resized slices and
  * reports the device time of the convolution kernels alone (ms) for the roofline. */

@@ -79,6 +79,7 @@ def lib():
         "lm_set_option": ([vp, C.c_char_p, i32], i32),
         "lm_debug_activation_info": ([i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)], i32),
         "lm_debug_read_activation": ([vp, i32, i32, f32p], i32),
+        "lm_debug_activation_scale": ([vp, i32, i32, C.POINTER(C.c_float)], i32),
         "lm_last_conv_timing": ([vp, C.POINTER(C.c_float), C.POINTER(C.c_int64)], i32),
     }
     for name, (argtypes, restype) in sig.items():
@@ -95,7 +96,7 @@ EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_ca
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
            "lm_keep_largest_component",
            "lm_last_timings", "lm_set_option", "lm_last_conv_timing",
-           "lm_debug_activation_info", "lm_debug_read_activation"]
+           "lm_debug_activation_info", "lm_debug_read_activation", "lm_debug_activation_scale"]
 
 
 def _ptr(a):
@@ -519,6 +520,12 @@ class Engine:
         out = np.empty((n, hw, hw, ch.value), np.float32)
         _check(lib().lm_debug_read_activation(self._h, act_id, n, _ptr(out)))
         return out
+
+    def activation_scale(self, slot, act_id):
+        """The power-of-two scale activation `act_id` of weight slot `slot` is stored at (1.0 unless it was rescued)."""
+        s = C.c_float(0)
+        _check(lib().lm_debug_activation_scale(self._h, slot, act_id, C.byref(s)))
+        return float(s.value)
 
     def set_option(self, key, value):
         _check(lib().lm_set_option(self._h, key.encode(), int(value)))

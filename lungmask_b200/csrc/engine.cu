@@ -178,7 +178,6 @@ struct lm_engine {
                             // weight) of that slot's network left the operand format's range (fp16 build: |x * scale| > 65504)
   int* h_range = nullptr;   // pinned host copy, refreshed at the end of every forward
   int range_slot = -1;      // the slot of the last forward (lm_debug_read_activation unscales with its scales)
-  int range_retries = 0;
   Slot slots[LM_MAX_SLOTS];
   // Whole-volume calls (run_volume): a host volume is uploaded to d_upload; volume_enqueue stages a volume that needs
   // re-orientation or conversion into d_vol / d_fvol, keeps the LPS mask in d_lps_out and the fusion's two masks in
@@ -482,42 +481,56 @@ int inference_dev(lm_engine* e, int slot, const void* d_vol, int vtype, int S, i
   return 0;
 }
 
+// The lowest scale of a group: 4 steps of 2^-8, for values up to 65504 * 2^32 = 2.8e14.
+constexpr float kMinActScale = 0x1p-32f;
+
 // After a stream synchronisation: did any activation leave the operand format's range during the forward passes?
-// Returns 0 (no), 1 (yes: the offending tensors' power-of-two scales were lowered - run the forward again) or an error.
+// Returns 0 (no), 1 (yes: the offending groups' power-of-two scales were lowered - run the forward again) or an error.
+// A flag counts only when no tensor upstream of it flagged in the same forward.  An overflowing tensor is stored as
+// +inf / -inf planes: behind a ReLU its consumers see 0 instead of NaN, behind a 1x1 layer (no ReLU) NaN reaches the
+// upsample, which flags it - either way every tensor downstream holds wrong values, and lowering their groups would
+// only cost them precision.  The first flag of a cascade is always genuine (its inputs were in range), so every re-run
+// lowers at least one group; a group that would go below kMinActScale ends the call with LM_ERR_RANGE.
 int range_finish(lm_engine* e) {
   bool any = false;
   for (int i = 0; i < LM_MAX_SLOTS * RANGE_STRIDE; ++i) any |= e->h_range[i] != 0;
-  if (!any) { e->range_retries = 0; return 0; }
+  if (!any) return 0;
   cudaMemsetAsync(e->d_range, 0, LM_MAX_SLOTS * RANGE_STRIDE * sizeof(int), e->st);
-  const bool give_up = ++e->range_retries > 4;
-  bool weight_flag = false;
+  bool weight_flag = false, give_up = false;
+  bool lower[LM_MAX_SLOTS][NUM_ACT] = {};   // [slot][group representative]: one step of 2^-8 this re-run
   for (int sl = 0; sl < LM_MAX_SLOTS; ++sl) {
     int* h = e->h_range + sl * RANGE_STRIDE;
-    Slot& s = e->slots[sl];
     weight_flag |= h[NUM_ACT] != 0;
-    h[NUM_ACT] = 0;
-    for (int a = 0; a < NUM_ACT; ++a) {
-      if (!h[a]) continue;
-      const int g = scale_group(a);
-      for (int b = 0; b < NUM_ACT; ++b) {   // one step per group and re-run, whichever members raised their flags
-        if (scale_group(b) != g) continue;
-        if (!give_up && s.act_scale[b] > 1e-30f) { s.act_scale[b] *= (1.f / 256.f); e->graph_epoch++; }
-        h[b] = 0;
-      }
+    bool tainted[NUM_ACT] = {};   // a tensor upstream of this one flagged (execution order visits sources first)
+    auto feed = [&](int src, int dst) { if (src >= 0 && dst >= 0 && (h[src] || tainted[src])) tainted[dst] = true; };
+    for (int i = 0, up = 0; i < NUM_LAYERS; ++i) {
+      const LayerSpec& L = LAYERS[i];
+      for (int d : {L.dst, L.dst_pool}) { feed(L.src0, d); feed(L.src1, d); }
+      if (up < 4 && UPS[up].after_layer == i) { feed(UPS[up].src, UPS[up].dst); ++up; }
     }
+    for (int a = 0; a < NUM_ACT; ++a) {
+      if (!h[a] || tainted[a]) continue;
+      const int g = scale_group(a);
+      lower[sl][g] = true;
+      give_up |= e->slots[sl].act_scale[g] <= kMinActScale;
+    }
+    for (int i = 0; i < RANGE_STRIDE; ++i) h[i] = 0;
   }
-  if (weight_flag || give_up) {
-    e->range_retries = 0;
+  if (weight_flag || give_up)
     return fail(LM_ERR_RANGE, "an activation exceeded the fp16 operand range even after rescaling by 2^-32 (|x| > 2.8e14): "
                               "the weights are not a usable network (rebuild with -DLM_OPERAND_F16=0 for tf32 operands)");
-  }
+  for (int sl = 0; sl < LM_MAX_SLOTS; ++sl)
+    for (int b = 0; b < NUM_ACT; ++b)   // one step per group and re-run, whichever members raised their flags
+      if (lower[sl][scale_group(b)]) e->slots[sl].act_scale[b] *= (1.f / 256.f);
+  e->graph_epoch++;
   return 1;
 }
 
 // Enqueue-synchronise-verify: `enqueue` puts a whole call on the engine stream; after the synchronisation the
 // post-processing reports whether its region tables were large enough (the region count lives on the device).  If not,
 // the tables grow to the reported size and the call is enqueued once more (a label map with more than one region per 32
-// voxels; never seen with a trained network).
+// voxels; never seen with a trained network).  range_finish lowers at least one group's scale per re-run and at most
+// 4 times per group, so range rescues end on their own after fewer than 4 * NUM_ACT re-runs.
 template <typename F>
 int run_checked(lm_engine* e, F&& enqueue) {
   for (int attempt = 0;; ++attempt) {
@@ -527,7 +540,7 @@ int run_checked(lm_engine* e, F&& enqueue) {
     if (rr < 0) return rr;
     const int pf = postprocess_finish(e->post);
     if (!rr && !pf) return 0;
-    if (attempt >= 8) return fail(-22, "the call did not settle after %d re-runs (region tables %u regions / operand range)", attempt, e->post.last_regions);
+    if (attempt >= 8 + 4 * NUM_ACT) return fail(-22, "the call did not settle after %d re-runs (region tables %u regions / operand range)", attempt, e->post.last_regions);
     if (pf) RC(e->post.reserve_regions(e->post.want_regions));
   }
 }
@@ -1565,6 +1578,14 @@ int lm_debug_read_activation(lm_engine* e, int act_id, int n, float* out) {
   for (int i = 0; i < n; ++i)
     for (size_t k = 0; k < per; ++k)
       out[(size_t)i * per + k] = ((float)tmp[((size_t)i * 2) * per + k] + (float)tmp[((size_t)i * 2 + 1) * per + k] * kLoUnscale) * unscale;
+  return 0;
+}
+
+int lm_debug_activation_scale(lm_engine* e, int slot, int act_id, float* scale) {
+  if (!e || !scale) return fail(-1, "lm_debug_activation_scale: NULL argument");
+  if (slot < 0 || slot >= LM_MAX_SLOTS) return fail(-1, "lm_debug_activation_scale: slot %d out of range", slot);
+  if (act_id < 0 || act_id >= NUM_ACT) return fail(-1, "activation id %d out of range", act_id);
+  *scale = ACT[act_id].split ? e->slots[slot].act_scale[act_id] : 1.f;
   return 0;
 }
 
