@@ -282,6 +282,42 @@ LM_API int lm_shape_sums_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1
 LM_API int lm_max_diameters_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const double* spacing,
                                 double* d2, void* stream);
 
+/* First-order (histogram) sums (no counterpart in the reference; DESIGN §4.11): LMInferer.first_order computes
+ * PyRadiomics' 18 default firstorder features of every row of lm_label_stats_dev from these two passes.  Both take
+ * device memory of the engine's device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev, check
+ * every argument before any kernel runs and return after the engine's stream has synchronised; the inputs are never
+ * written.  d_vol, dtype, d_mask as lm_label_stats_dev, fewer than 2^32 voxels.  A voxel is in row l (1..255) when
+ * mask == l and in row 256 when mask > 0; a row's ROI is its voxels with a non-NaN value (float16 / bfloat16 widened to
+ * float32, every value read as float64).
+ * Row inputs (host arrays indexed 0..256, row 0 unused): mode 0 (skip), 1 (float) or 2 (exact: integer volumes only);
+ *   a label row with a mode needs row 256 with one.  band_lo <= band_hi: the band, compared in float64, both inclusive.
+ *   base: an exact row's integer minimum (|base| <= 2^53); its values must lie in [base, base + 2^20).  centre: a float
+ *   row's finite centre.
+ * lm_first_order_sums_dev (pass A): level = floor((floor(x) - low) / bin_width) + 1 in int64 as lm_texture_levels_dev,
+ *   which must lie in 1..n_levels (1..255).  Host results, zero for skipped rows:
+ *   histogram [257][256] int64    the ROI's voxels per level (index 0 unused)
+ *   int_sums [257][10] uint64     exact rows: S1, S2, S3, S4, S_B as 128-bit (low word, high word) pairs, S_k = sum d^k
+ *                                 with d = x - base, S_B = sum d over the band
+ *   band_count [257] int64        the ROI's voxels in the band
+ *   float_sums [257][5] float64   float rows: sum e, e^2, e^3, e^4 with e = x - centre, and sum e over the band
+ * lm_first_order_splits_dev (pass B).  Host results, zero for skipped rows:
+ *   below [257][4] int64          exact rows: the count and the sum of d of the ROI's voxels with d <= split, then of the
+ *                                 band's voxels with d <= split_band (split, split_band in [0, 2^20))
+ *   abs_dev [257][2] float64      float rows: sum |x - centre| over the ROI, sum |x - centre_band| over the band
+ * The integer results are exact and independent of the schedule; the float sums are order-dependent in the last bits.
+ * A value of an exact row outside its span or a level outside 1..n_levels is an error.  Work area: a row table, a
+ * 2 KB histogram and 88 bytes of sums per row, kept by the engine. */
+LM_API int lm_first_order_sums_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                                   int bin_width, const int* mode, const int64_t* low, const int* n_levels,
+                                   const int64_t* base, const double* centre, const double* band_lo, const double* band_hi,
+                                   int64_t* histogram, uint64_t* int_sums, int64_t* band_count, double* float_sums,
+                                   void* stream);
+LM_API int lm_first_order_splits_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1,
+                                     int n2, const int* mode, const int64_t* base, const int64_t* split,
+                                     const int64_t* split_band, const double* centre, const double* centre_band,
+                                     const double* band_lo, const double* band_hi, int64_t* below, double* abs_dev,
+                                     void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

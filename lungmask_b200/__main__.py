@@ -8,16 +8,17 @@ the volume and HU statistics of every label and of the whole lung (.json / .csv,
 LMInferer.laa_clusters), `--regions PATH` the statistics of every label by upper / middle / lower zone and by depth
 below the lung surface (.json / .csv, LMInferer.regional_statistics), `--texture PATH` the texture features of every
 label and the whole lung (GLCM and GLSZM by default, `--texture-classes` adds GLRLM, GLDM and NGTDM; .json / .csv,
-LMInferer.texture), and `--shape PATH` the mesh shape features
+LMInferer.texture), `--shape PATH` the mesh shape features
 (surface area, mesh volume, sphericity, maximum diameters, principal axes) of every label and the whole lung (.json /
-.csv, LMInferer.shape).
+.csv, LMInferer.shape), and `--first-order PATH` PyRadiomics' first-order features (percentiles, moments, mean absolute
+deviations, energy, entropy, uniformity) of every label and the whole lung (.json / .csv, LMInferer.first_order).
 """
 import argparse
 import os
 import sys
 
-from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_mask, save_probabilities,
-                 save_regional_statistics, save_shape, save_statistics, save_texture)
+from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_first_order, save_mask,
+                 save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture)
 from .logger import logger
 from .mask import LMInferer
 
@@ -73,6 +74,16 @@ def build_parser():
                    help="Also write the mesh shape features (PyRadiomics names: surface area, mesh volume, sphericity, "
                         "maximum 3-D and 2-D diameters, principal axis lengths) of every label and the whole lung: .json "
                         "(with the exact sums) or .csv")
+    p.add_argument("--first-order", metavar="PATH", type=str, default=None,
+                   help="Also write the first-order features (PyRadiomics names: percentiles, mean, variance, skewness, "
+                        "kurtosis, mean absolute deviations, energy, entropy, uniformity) of every label and the whole "
+                        "lung: .json (with the level histograms and the exact sums) or .csv")
+    p.add_argument("--first-order-bin-width", metavar="BW", type=int, default=25,
+                   help="Fixed bin width of the Entropy and Uniformity of --first-order in HU, a positive integer "
+                        "(default 25)")
+    p.add_argument("--first-order-shift", metavar="C", type=int, default=0,
+                   help="Integer added to every value for Energy, TotalEnergy and RootMeanSquared of --first-order "
+                        "(PyRadiomics' voxelArrayShift, default 0)")
     return p
 
 
@@ -106,6 +117,13 @@ def main(argv=None):
             sys.exit("--texture-classes: %s" % ex)
     if args.shape is not None:
         check_table_path(args.shape, "shape")
+    if args.first_order is not None:
+        check_table_path(args.first_order, "first_order")
+        from .texture import check_arguments as check_bin_width
+        try:
+            check_bin_width(args.first_order_bin_width)
+        except ValueError as ex:
+            sys.exit("--first-order-bin-width: %s" % ex)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -144,6 +162,10 @@ def main(argv=None):
     if args.shape is not None:
         logger.info(f"Save shape features to: {args.shape}")
         save_shape(args.shape, inferer.shape(result, image=image))
+    if args.first_order is not None:
+        logger.info(f"Save first-order features to: {args.first_order}")
+        save_first_order(args.first_order, inferer.first_order(image, result, bin_width=args.first_order_bin_width,
+                                                               voxel_array_shift=args.first_order_shift))
 
 
 if __name__ == "__main__":

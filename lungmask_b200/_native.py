@@ -60,6 +60,8 @@ def lib():
         "lm_neighbour_counts_dev": ([vp, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_shape_sums_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_max_diameters_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp], i32),
+        "lm_first_order_sums_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32] + [vp] * 12, i32),
+        "lm_first_order_splits_dev": ([vp, vp, i32, u8p, i32, i32, i32] + [vp] * 11, i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -90,7 +92,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -410,6 +412,46 @@ class Engine:
         _check(lib().lm_max_diameters_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, int(row), _ptr(sp), _ptr(d2),
                                           C.c_void_p(int(stream)) if stream else None))
         return d2
+
+    # ---- first-order sums (lm_first_order_sums_dev, lm_first_order_splits_dev)
+    @staticmethod
+    def _rows(values, dtype):
+        """A per-row input of the first-order calls: 257 values (row 0 unused) as a C-contiguous host array."""
+        a = np.ascontiguousarray(values, dtype=dtype).reshape(-1)
+        if a.size != 257:
+            raise ValueError("first-order row inputs need 257 values (rows 0..256), got %d" % a.size)
+        return a
+
+    def first_order_sums_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, bin_width, mode, low, n_levels, base, centre,
+                             band_lo, band_hi, stream=0):
+        """lm_first_order_sums_dev (pass A) on device memory of this engine's device (`stream` as for apply_dev); every row
+        input has 257 entries -> dict: "histogram" int64 (257, 256), "int_sums" uint64 (257, 10) (S1..S4, S_B as (low,
+        high) word pairs of exact rows), "band_count" int64 [257], "float_sums" float64 (257, 5) (float rows)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ins = [self._rows(mode, np.int32), self._rows(low, np.int64), self._rows(n_levels, np.int32),
+               self._rows(base, np.int64), self._rows(centre, np.float64), self._rows(band_lo, np.float64),
+               self._rows(band_hi, np.float64)]
+        res = {"histogram": np.zeros((257, 256), np.int64), "int_sums": np.zeros((257, 10), np.uint64),
+               "band_count": np.zeros(257, np.int64), "float_sums": np.zeros((257, 5), np.float64)}
+        _check(lib().lm_first_order_sums_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), C.c_void_p(d_mask_ptr), n0, n1,
+                                             n2, int(bin_width), *[_ptr(a) for a in ins],
+                                             *[_ptr(res[k]) for k in ("histogram", "int_sums", "band_count", "float_sums")],
+                                             C.c_void_p(int(stream)) if stream else None))
+        return res
+
+    def first_order_splits_dev(self, d_vol_ptr, dtype_code, d_mask_ptr, shape, mode, base, split, split_band, centre,
+                               centre_band, band_lo, band_hi, stream=0):
+        """lm_first_order_splits_dev (pass B), row inputs as for first_order_sums_dev -> dict: "below" int64 (257, 4)
+        (n_lo, L, n_lo_B, L_B of exact rows), "abs_dev" float64 (257, 2) (float rows)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ins = [self._rows(mode, np.int32), self._rows(base, np.int64), self._rows(split, np.int64),
+               self._rows(split_band, np.int64), self._rows(centre, np.float64), self._rows(centre_band, np.float64),
+               self._rows(band_lo, np.float64), self._rows(band_hi, np.float64)]
+        res = {"below": np.zeros((257, 4), np.int64), "abs_dev": np.zeros((257, 2), np.float64)}
+        _check(lib().lm_first_order_splits_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), C.c_void_p(d_mask_ptr), n0,
+                                               n1, n2, *[_ptr(a) for a in ins], _ptr(res["below"]), _ptr(res["abs_dev"]),
+                                               C.c_void_p(int(stream)) if stream else None))
+        return res
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

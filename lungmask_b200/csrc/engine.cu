@@ -22,6 +22,7 @@
 #include "regions.cuh"
 #include "texture.cuh"
 #include "shape.cuh"
+#include "first_order.cuh"
 
 using namespace lm;
 
@@ -199,6 +200,7 @@ struct lm_engine {
   TextureWork texture;    // lm_texture_levels_dev, lm_glcm_dev, lm_glrlm_dev, lm_neighbour_counts_dev: error flag, counters
                           // (lm_zone_sizes_dev uses `clusters`)
   ShapeWork shape;        // lm_shape_sums_dev, lm_max_diameters_dev: sums, line tables, diameter candidates
+  FirstOrderWork first_order;   // lm_first_order_sums_dev, lm_first_order_splits_dev: row table, histograms, sums
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -925,6 +927,7 @@ void lm_destroy(lm_engine* e) {
   e->regions.release();
   e->texture.release();
   e->shape.release();
+  e->first_order.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1315,6 +1318,80 @@ int lm_max_diameters_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, in
     if (!(spacing[k] > 0.0 && spacing[k] < INFINITY)) return fail(-1, "%s: spacing[%d] = %g is not finite and positive", fn, k, spacing[k]);
   RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}}));
   RC(max_diameters(e->shape, d_mask, n0, n1, n2, row, spacing, d2, e->num_sms, e->st, &e->launches));
+  return 0;
+}
+
+// The row arguments the two first-order calls share: modes, the band and the exact rows' base; `pass` 0 (sums) also
+// checks the levels, 1 (splits) the split points and the float rows' centres.
+static int check_first_order_rows(const char* fn, int dtype, const FirstOrderRows& r, int pass) {
+  const bool int_dtype = dtype == LM_DTYPE_U8 || dtype == LM_DTYPE_I8 || dtype == LM_DTYPE_I16 || dtype == LM_DTYPE_I32 ||
+                         dtype == LM_DTYPE_I64;
+  if (r.mode[0] != kFoSkip) return fail(-1, "%s: row 0 (background) has mode %d, it is never a row", fn, r.mode[0]);
+  bool labels = false;
+  for (int i = 1; i < kFoRows; ++i) {
+    const int m = r.mode[i];
+    if (m != kFoSkip && m != kFoFloat && m != kFoExact) return fail(-1, "%s: row %d: mode %d is not 0, 1 or 2", fn, i, m);
+    if (m == kFoSkip) continue;
+    labels |= i < 256;
+    if (m == kFoExact && !int_dtype) return fail(-1, "%s: row %d: the exact mode needs an integer volume (dtype %d)", fn, i, dtype);
+    if (!(r.band_lo[i] <= r.band_hi[i])) return fail(-1, "%s: row %d: band [%g, %g] is empty or NaN", fn, i, r.band_lo[i], r.band_hi[i]);
+    if (m == kFoExact && (r.base[i] < -((int64_t)1 << 53) || r.base[i] > ((int64_t)1 << 53)))
+      return fail(-1, "%s: row %d: base %lld beyond 2^53", fn, i, (long long)r.base[i]);
+    if (m == kFoFloat && !isfinite(r.centre[i])) return fail(-1, "%s: row %d: centre %g is not finite", fn, i, r.centre[i]);
+    if (pass == 0 && (r.n_levels[i] < 1 || r.n_levels[i] > kTextureMaxLevels))
+      return fail(-1, "%s: row %d: n_levels %d not in [1,%d]", fn, i, r.n_levels[i], kTextureMaxLevels);
+    if (pass == 1 && m == kFoExact) {
+      if (r.split[i] < 0 || r.split[i] >= kFoExactSpan || r.split_band[i] < 0 || r.split_band[i] >= kFoExactSpan)
+        return fail(-1, "%s: row %d: split %lld / %lld not in [0,2^20)", fn, i, (long long)r.split[i], (long long)r.split_band[i]);
+    }
+    if (pass == 1 && m == kFoFloat && !isfinite(r.centre_band[i]))
+      return fail(-1, "%s: row %d: centre_band %g is not finite", fn, i, r.centre_band[i]);
+  }
+  if (labels && r.mode[256] == kFoSkip) return fail(-1, "%s: a label row needs the union row 256", fn);
+  return 0;
+}
+
+static int first_order_device_error(const char* fn, int rc) {
+  if (rc == kFoRange) return fail(rc, "%s: a value outside its row's exact span or level range", fn);
+  return rc;
+}
+
+int lm_first_order_sums_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                            int bin_width, const int* mode, const int64_t* low, const int* n_levels, const int64_t* base,
+                            const double* centre, const double* band_lo, const double* band_hi, int64_t* histogram,
+                            uint64_t* int_sums, int64_t* band_count, double* float_sums, void* stream) {
+  static const char* fn = "lm_first_order_sums_dev";
+  if (!e || !d_vol || !d_mask || !mode || !low || !n_levels || !base || !centre || !band_lo || !band_hi || !histogram ||
+      !int_sums || !band_count || !float_sums)
+    return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (bin_width < 1) return fail(-1, "%s: bin_width %d is not positive", fn, bin_width);
+  const FirstOrderRows rows{mode, low, n_levels, base, centre, nullptr, band_lo, band_hi, nullptr, nullptr};
+  RC(check_first_order_rows(fn, dtype, rows, 0));
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_mask", d_mask}}));
+  const int rc = first_order_sums(e->first_order, d_vol, dtype, d_mask, (size_t)n0 * n1 * n2, bin_width, rows, histogram,
+                                  int_sums, band_count, float_sums, e->num_sms, e->st, &e->launches);
+  if (rc) return first_order_device_error(fn, rc);
+  return 0;
+}
+
+int lm_first_order_splits_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                              const int* mode, const int64_t* base, const int64_t* split, const int64_t* split_band,
+                              const double* centre, const double* centre_band, const double* band_lo,
+                              const double* band_hi, int64_t* below, double* abs_dev, void* stream) {
+  static const char* fn = "lm_first_order_splits_dev";
+  if (!e || !d_vol || !d_mask || !mode || !base || !split || !split_band || !centre || !centre_band || !band_lo ||
+      !band_hi || !below || !abs_dev)
+    return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  const FirstOrderRows rows{mode, nullptr, nullptr, base, centre, centre_band, band_lo, band_hi, split, split_band};
+  RC(check_first_order_rows(fn, dtype, rows, 1));
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_mask", d_mask}}));
+  const int rc = first_order_splits(e->first_order, d_vol, dtype, d_mask, (size_t)n0 * n1 * n2, rows, below, abs_dev,
+                                    e->num_sms, e->st, &e->launches);
+  if (rc) return first_order_device_error(fn, rc);
   return 0;
 }
 

@@ -409,7 +409,8 @@ def save_probabilities(path, probs, like=None):
 
 def check_table_path(path, kind):
     """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
-    ("clusters"), save_regional_statistics ("regions"), save_texture ("texture") or save_shape ("shape") cannot write."""
+    ("clusters"), save_regional_statistics ("regions"), save_texture ("texture"), save_shape ("shape") or
+    save_first_order ("first_order") cannot write."""
     if not path.lower().endswith((".json", ".csv")):
         raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
 
@@ -521,6 +522,23 @@ def save_shape(path, shape):
     lines = [",".join(list(ShapeRow.SUMMARY) + list(SHAPE_FEATURES))]
     for r in shape.rows:
         cells = [getattr(r, k) for k in ShapeRow.SUMMARY] + [r.features[k] for k in SHAPE_FEATURES]
+        lines.append(",".join(_csv_cell(v) for v in cells))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def save_first_order(path, first_order):
+    """Writes the FirstOrderFeatures of LMInferer.first_order: .json (spacing, bin_width, voxel_array_shift and one object
+    per row with its features, level histogram, percentiles and exact power / split sums, NaN as null) or .csv (a header,
+    then one line per row: label, name, voxels, exact, low, bin_width, n_levels, then the 18 features of
+    first_order.FIRST_ORDER_FEATURES; an unknown value is an empty cell, NaN is "nan")."""
+    check_table_path(path, "first_order")
+    if path.lower().endswith(".json"):
+        return _save_json(path, first_order)
+    from .first_order import FIRST_ORDER_FEATURES, FirstOrderRow
+    lines = [",".join(list(FirstOrderRow.SUMMARY) + list(FIRST_ORDER_FEATURES))]
+    for r in first_order.rows:
+        cells = [getattr(r, k) for k in FirstOrderRow.SUMMARY] + [r.features[k] for k in FIRST_ORDER_FEATURES]
         lines.append(",".join(_csv_cell(v) for v in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")

@@ -543,6 +543,84 @@ class LMInferer:
             out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones, classes, runs, neighbours))
         return tx.TextureFeatures(s.spacing, bw, out, classes, alpha)
 
+    def first_order(self, image, mask, bin_width=25, spacing=None, voxel_array_shift=0):
+        """PyRadiomics' 18 default first-order features of `image` under `mask` -> lungmask_b200.first_order.
+        FirstOrderFeatures, with the rows of `statistics`: every label value in the mask and every label 1..K-1 of the
+        model (absent ones with 0 voxels and NaN features), then "lung" (mask > 0).  A row's ROI is its voxels with a
+        non-NaN value, read in the volume's dtype (float16 / bfloat16 as float32); a non-finite value in an ROI is a
+        ValueError.
+
+        The features (first_order.FIRST_ORDER_FEATURES) are the percentiles, Minimum, Maximum and Range of numpy.percentile
+        (bit-identical; Median is the 50th percentile), Mean, Variance, Skewness and Kurtosis (m4 / m2^2, not excess; both
+        0 when m2 = 0), MeanAbsoluteDeviation, RobustMeanAbsoluteDeviation (over P10 <= x <= P90), Energy = sum (x + c)^2
+        with c = `voxel_array_shift` (an integer, PyRadiomics' voxelArrayShift), TotalEnergy = Energy x the voxel volume
+        in mm^3 (NaN without a spacing), RootMeanSquared, and Entropy and Uniformity of the level histogram of the
+        fixed `bin_width` discretisation of `texture` (more than 255 levels in any row is a ValueError before any
+        first-order kernel runs).  Integer rows that span fewer than 2^20 values are summed exactly: their features are
+        reproducible bit for bit (`exact` on the row).  Each row keeps the level histogram, the power and split sums and
+        the percentiles its features come from.
+
+        `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the
+        spacing), CPU tensors, or CUDA tensors on the engine's device read in place after the work queued on the current
+        stream; both are left unchanged."""
+        from . import first_order as fo
+        from . import texture as tx
+        from .statistics import label_name
+        bw = tx.check_arguments(bin_width)
+        shift = fo.check_shift(voxel_array_shift)
+        s = self._stage("first_order", image, mask, spacing)
+        shape = tuple(s.mask.shape)
+        st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, fo.PERCENTILES, (),
+                                         stream=s.stream)
+        present = set(int(x) for x in np.nonzero(st["voxels"][1:256])[0] + 1)
+        rows = sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]
+        names = {r: fo.UNION if r == 256 else label_name(self.modelname, r) for r in rows}
+        integer = s.dtype in (_native.DTYPE_U8, _native.DTYPE_I8, _native.DTYPE_I16, _native.DTYPE_I32, _native.DTYPE_I64)
+        plan = {}   # every row's plan first: a refused row stops the call before any first-order kernel
+        for r in rows:
+            n = int(st["voxels"][r] - st["nan_voxels"][r])
+            if n:
+                m = st["moments"][r]
+                plan[r] = fo.plan_row(n, float(m[2]), float(m[3]), float(m[0]), st["percentile"][r], bw, integer,
+                                      "row %s (%s)" % ("lung" if r == 256 else r, names[r]))
+        if not plan:
+            return fo.FirstOrderFeatures(s.spacing, bw, shift, [fo.build_row(r, names[r], bw) for r in rows])
+        mode = np.zeros(257, np.int32)
+        low, base, split, split_b = (np.zeros(257, np.int64) for _ in range(4))
+        n_levels = np.zeros(257, np.int32)
+        centre, centre_b, band_lo, band_hi = (np.zeros(257, np.float64) for _ in range(4))
+        for r, p in plan.items():
+            mode[r] = fo.MODE_EXACT if p.exact else fo.MODE_FLOAT
+            low[r], n_levels[r], base[r], centre[r] = p.low, p.n_levels, p.base, p.mean
+            band_lo[r], band_hi[r] = p.percentiles[0], p.percentiles[4]
+        a = self.engine.first_order_sums_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, bw, mode, low, n_levels, base,
+                                             centre, band_lo, band_hi, stream=s.stream)
+        sums = {}
+        for r, p in plan.items():
+            if p.exact:
+                w = fo.int_sums_from_words(a["int_sums"][r])
+                sums[r] = (w[:4], int(a["band_count"][r]), w[4])
+            else:
+                f = [float(x) for x in a["float_sums"][r]]
+                sums[r] = (f[:4], int(a["band_count"][r]), f[4])
+            t, tb = fo.split_points(p, *sums[r])
+            if p.exact:
+                split[r], split_b[r] = t, tb
+            else:
+                centre[r], centre_b[r] = t, tb
+        b = self.engine.first_order_splits_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, mode, base, split, split_b,
+                                               centre, centre_b, band_lo, band_hi, stream=s.stream)
+        out = []
+        for r in rows:
+            if r not in plan:
+                out.append(fo.build_row(r, names[r], bw))
+                continue
+            p = plan[r]
+            splits = [int(x) for x in b["below"][r]] if p.exact else [float(x) for x in b["abs_dev"][r]]
+            ps, nb, sb = sums[r]
+            out.append(fo.build_row(r, names[r], bw, p, a["histogram"][r][1:], ps, nb, sb, splits, s.spacing, shift))
+        return fo.FirstOrderFeatures(s.spacing, bw, shift, out)
+
     def shape(self, mask, spacing=None, image=None):
         """Mesh shape features of every row of `statistics` -> lungmask_b200.shape.ShapeFeatures: every label value in the
         mask and every label 1..K-1 of the model (absent ones with 0 voxels and NaN features), then "lung" (mask != 0).
