@@ -318,6 +318,26 @@ LM_API int lm_first_order_splits_dev(lm_engine* e, const void* d_vol, int dtype,
                                      const double* band_lo, const double* band_hi, int64_t* below, double* abs_dev,
                                      void* stream);
 
+/* Wavelet decomposition (no counterpart in the reference; DESIGN §4.12): one band of PyRadiomics' getWaveletImage with
+ * its defaults (pywt.swtn, level 1, start_level 0), so that LMInferer.wavelet_features can run the first-order and
+ * texture calls on every decomposition.
+ * lm_wavelet_dev writes band `band` (0..7 = 4 h_x + 2 h_y + h_z, h = 1 for the high-pass filter along that axis:
+ *   1 LLH, 2 LHL, 3 LHH, 4 HLL, 5 HLH, 6 HHL, 7 HHH, 0 LLL) of the (n0,n1,n2) volume d_vol (every LM_DTYPE_* code; bool
+ *   as LM_DTYPE_U8; converted to float64 first) to the float64 (n0,n1,n2) d_out.  The passes run along array axis 2 (x),
+ *   then 1 (y), then 0 (z): out[o] = sum_{j=0..F-1} f[j] in[(o + F/2 - j) mod N'], summed from +0.0 with j ascending, each
+ *   product and each sum rounded to float64 with no fused multiply-add; an odd axis of N voxels is wrapped to
+ *   N' = N + 1 (index N holds index 0) and the result trimmed back to N.  Filters: PyWavelets' dec_lo of `wavelet` and
+ *   dec_hi[k] = (-1)^(k+1) dec_lo[F-1-k]; coif1 (F = 6) or haar (F = 2).  Every padded extent N' must be at least F and
+ *   the volume must hold fewer than 2^32 voxels; d_out must not overlap d_vol.  Device memory of the engine's device, the
+ *   caller's cudaStream_t with the event-wait rule of lm_apply_dev; every argument is checked before any kernel runs and
+ *   the call returns after the engine's stream has synchronised.  A NaN or +-inf anywhere in the volume returns
+ *   LM_ERR_NONFINITE (d_out is then not a band).  Work area: one flag; no full-volume intermediate. */
+#define LM_WAVELET_COIF1 0
+#define LM_WAVELET_HAAR 1
+#define LM_ERR_NONFINITE (-41)   /* lm_wavelet_dev: the volume holds a NaN or +-inf */
+LM_API int lm_wavelet_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, int wavelet, int band,
+                          double* d_out, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

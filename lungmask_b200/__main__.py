@@ -11,14 +11,17 @@ label and the whole lung (GLCM and GLSZM by default, `--texture-classes` adds GL
 LMInferer.texture), `--shape PATH` the mesh shape features
 (surface area, mesh volume, sphericity, maximum diameters, principal axes) of every label and the whole lung (.json /
 .csv, LMInferer.shape), and `--first-order PATH` PyRadiomics' first-order features (percentiles, moments, mean absolute
-deviations, energy, entropy, uniformity) of every label and the whole lung (.json / .csv, LMInferer.first_order).
+deviations, energy, entropy, uniformity) of every label and the whole lung (.json / .csv, LMInferer.first_order), and
+`--wavelet PATH` the first-order and texture features of the 8 coif1 (or haar) wavelet decompositions (.json / .csv,
+LMInferer.wavelet_features).
 """
 import argparse
 import os
 import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_first_order, save_mask,
-                 save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture)
+                 save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
+                 save_wavelet_features)
 from .logger import logger
 from .mask import LMInferer
 
@@ -84,6 +87,17 @@ def build_parser():
     p.add_argument("--first-order-shift", metavar="C", type=int, default=0,
                    help="Integer added to every value for Energy, TotalEnergy and RootMeanSquared of --first-order "
                         "(PyRadiomics' voxelArrayShift, default 0)")
+    p.add_argument("--wavelet", metavar="PATH", type=str, default=None,
+                   help="Also write the first-order and texture features of the 8 wavelet decompositions (PyRadiomics' "
+                        "Wavelet image type, keys such as wavelet-LLH_firstorder_Mean) of every label and the whole lung: "
+                        ".json (with the exact sums and matrices) or .csv")
+    p.add_argument("--wavelet-name", choices=["coif1", "haar"], default="coif1", help="Wavelet of --wavelet (default coif1)")
+    p.add_argument("--wavelet-bin-width", metavar="SPEC", type=str, default="25",
+                   help="Fixed bin width of --wavelet in HU: one positive integer, or a default followed by "
+                        "per-decomposition overrides such as 25,LLL=50 (default 25)")
+    p.add_argument("--wavelet-classes", metavar="NAMES", type=str, default="firstorder,glcm,glszm,glrlm,gldm,ngtdm",
+                   help="Comma-separated feature classes of --wavelet: any of firstorder, glcm, glszm, glrlm, gldm, ngtdm "
+                        "(default all)")
     return p
 
 
@@ -124,6 +138,18 @@ def main(argv=None):
             check_bin_width(args.first_order_bin_width)
         except ValueError as ex:
             sys.exit("--first-order-bin-width: %s" % ex)
+    if args.wavelet is not None:
+        check_table_path(args.wavelet, "wavelet")
+        from .wavelet import check_classes as check_wavelet_classes, parse_bin_widths
+        try:
+            wavelet_bin_width = parse_bin_widths(args.wavelet_bin_width)
+        except (TypeError, ValueError) as ex:
+            sys.exit("--wavelet-bin-width: %s" % ex)
+        wavelet_classes = [c.strip() for c in args.wavelet_classes.split(",") if c.strip()]
+        try:
+            check_wavelet_classes(wavelet_classes)
+        except ValueError as ex:
+            sys.exit("--wavelet-classes: %s" % ex)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -166,6 +192,10 @@ def main(argv=None):
         logger.info(f"Save first-order features to: {args.first_order}")
         save_first_order(args.first_order, inferer.first_order(image, result, bin_width=args.first_order_bin_width,
                                                                voxel_array_shift=args.first_order_shift))
+    if args.wavelet is not None:
+        logger.info(f"Save wavelet features to: {args.wavelet}")
+        save_wavelet_features(args.wavelet, inferer.wavelet_features(image, result, wavelet=args.wavelet_name,
+                                                                     bin_width=wavelet_bin_width, classes=wavelet_classes))
 
 
 if __name__ == "__main__":

@@ -11,6 +11,8 @@ NET_RES = 256
 FLAG_NO_POSTPROCESS = 1
 DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2   # LM_DTYPE_* of lm_apply_volume_probs
 DTYPE_U8, DTYPE_I8, DTYPE_I32, DTYPE_I64, DTYPE_F16, DTYPE_BF16 = 3, 4, 5, 6, 7, 8   # lm_apply_dev only (U8 also bool)
+WAVELET_CODES = {"coif1": 0, "haar": 1}   # LM_WAVELET_* of lm_wavelet_dev
+ERR_NONFINITE = -41                       # LM_ERR_NONFINITE
 
 _lib = None
 
@@ -62,6 +64,7 @@ def lib():
         "lm_max_diameters_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp], i32),
         "lm_first_order_sums_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32] + [vp] * 12, i32),
         "lm_first_order_splits_dev": ([vp, vp, i32, u8p, i32, i32, i32] + [vp] * 11, i32),
+        "lm_wavelet_dev": ([vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -92,7 +95,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_wavelet_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -452,6 +455,20 @@ class Engine:
                                                n1, n2, *[_ptr(a) for a in ins], _ptr(res["below"]), _ptr(res["abs_dev"]),
                                                C.c_void_p(int(stream)) if stream else None))
         return res
+
+    # ---- wavelet decomposition (lm_wavelet_dev)
+    def wavelet_dev(self, d_vol_ptr, dtype_code, shape, wavelet, band, d_out_ptr, stream=0):
+        """Writes band `band` (0..7 = 4 h_x + 2 h_y + h_z) of the `wavelet` ("coif1" or "haar") decomposition of a
+        C-contiguous `shape` device volume of element type `dtype_code` to the float64 `shape` device buffer `d_out_ptr`
+        (`stream` as for apply_dev).  ValueError when the volume holds a NaN or +-inf; NativeError for the other failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        if wavelet not in WAVELET_CODES:
+            raise ValueError("wavelet_dev: unknown wavelet %r (known: %s)" % (wavelet, ", ".join(WAVELET_CODES)))
+        rc = lib().lm_wavelet_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2, WAVELET_CODES[wavelet],
+                                  int(band), C.c_void_p(d_out_ptr), C.c_void_p(int(stream)) if stream else None)
+        if rc == ERR_NONFINITE:
+            raise ValueError("wavelet: " + lib().lm_last_error().decode().split(": ", 1)[1])
+        _check(rc)
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

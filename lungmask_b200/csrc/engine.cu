@@ -23,6 +23,7 @@
 #include "texture.cuh"
 #include "shape.cuh"
 #include "first_order.cuh"
+#include "wavelet.cuh"
 
 using namespace lm;
 
@@ -201,6 +202,7 @@ struct lm_engine {
                           // (lm_zone_sizes_dev uses `clusters`)
   ShapeWork shape;        // lm_shape_sums_dev, lm_max_diameters_dev: sums, line tables, diameter candidates
   FirstOrderWork first_order;   // lm_first_order_sums_dev, lm_first_order_splits_dev: row table, histograms, sums
+  WaveletWork wavelet;          // lm_wavelet_dev: the non-finite flag
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -928,6 +930,7 @@ void lm_destroy(lm_engine* e) {
   e->texture.release();
   e->shape.release();
   e->first_order.release();
+  e->wavelet.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1393,6 +1396,30 @@ int lm_first_order_splits_dev(lm_engine* e, const void* d_vol, int dtype, const 
                                     e->num_sms, e->st, &e->launches);
   if (rc) return first_order_device_error(fn, rc);
   return 0;
+}
+
+int lm_wavelet_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, int wavelet, int band, double* d_out,
+                   void* stream) {
+  static const char* fn = "lm_wavelet_dev";
+  if (!e || !d_vol || !d_out) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the wavelet call takes fewer than 2^32", fn, n);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  const int taps = wavelet_taps(wavelet);
+  if (!taps) return fail(-1, "%s: unknown wavelet code %d", fn, wavelet);
+  if (band < 0 || band >= kWaveletBands) return fail(-1, "%s: band %d not in [0,%d)", fn, band, kWaveletBands);
+  const int dims[3] = {n0, n1, n2};
+  for (int a = 0; a < 3; ++a)
+    if (dims[a] + (dims[a] & 1) < taps)
+      return fail(-1, "%s: axis %d has %d voxels (padded %d), the filter needs at least %d", fn, a, dims[a],
+                  dims[a] + (dims[a] & 1), taps);
+  const uintptr_t v0 = reinterpret_cast<uintptr_t>(d_vol), o0 = reinterpret_cast<uintptr_t>(d_out);
+  if (v0 < o0 + n * sizeof(double) && o0 < v0 + n * dtype_bytes(dtype)) return fail(-1, "%s: d_out overlaps d_vol", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_out", d_out}}));
+  const int rc = wavelet_band(e->wavelet, d_vol, dtype, n0, n1, n2, wavelet, band, d_out, e->st, &e->launches);
+  if (rc == LM_ERR_NONFINITE) return fail(rc, "%s: the volume holds a NaN or +-inf", fn);
+  return rc;
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

@@ -409,8 +409,8 @@ def save_probabilities(path, probs, like=None):
 
 def check_table_path(path, kind):
     """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
-    ("clusters"), save_regional_statistics ("regions"), save_texture ("texture"), save_shape ("shape") or
-    save_first_order ("first_order") cannot write."""
+    ("clusters"), save_regional_statistics ("regions"), save_texture ("texture"), save_shape ("shape"),
+    save_first_order ("first_order") or save_wavelet_features ("wavelet") cannot write."""
     if not path.lower().endswith((".json", ".csv")):
         raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
 
@@ -540,5 +540,26 @@ def save_first_order(path, first_order):
     for r in first_order.rows:
         cells = [getattr(r, k) for k in FirstOrderRow.SUMMARY] + [r.features[k] for k in FIRST_ORDER_FEATURES]
         lines.append(",".join(_csv_cell(v) for v in cells))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def save_wavelet_features(path, features):
+    """Writes the WaveletFeatures of LMInferer.wavelet_features: .json (the wavelet, the classes and, per decomposition,
+    its bin width and the to_dict() of its first-order and texture features with their exact histograms, sums and
+    matrices, NaN as null) or .csv (a header, then one line per row: label, name, voxels, then the row's flat vector
+    WaveletFeatures.vector with PyRadiomics' keys such as wavelet-LLH_firstorder_Mean; NaN is "nan")."""
+    check_table_path(path, "wavelet")
+    if path.lower().endswith(".json"):
+        return _save_json(path, features)
+    labels = features.labels
+    d = features.decompositions[0]
+    names = {r.label: r.name for r in (d.first_order or d.texture).rows}
+    keys = list(features.vector(labels[0]))
+    lines = [",".join(["label", "name", "voxels"] + keys)]
+    for label in labels:
+        v = features.vector(label)
+        cells = [label, names[label], features.voxels(label)] + [v[k] for k in keys]
+        lines.append(",".join(_csv_cell(c) for c in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")

@@ -667,14 +667,111 @@ class LMInferer:
                                              stream=stream)["voxels"]
         return set(int(x) for x in np.nonzero(voxels[1:256])[0] + 1)
 
-    def _stage(self, what, image, mask, spacing=None, mask_only=False):
+    def wavelet(self, image, wavelet="coif1", decompositions=None):
+        """PyRadiomics' wavelet decompositions of `image` (getWaveletImage with its defaults: pywt.swtn, one level, start
+        level 0) -> {name: float64 band of the image's shape}, in PyRadiomics' order: wavelet-LLH, -LHL, -LHH, -HLL,
+        -HLH, -HHL, -HHH, then -LLL.  The letters are the filters along (x, y, z) = array axes (2, 1, 0) of the (S, H, W)
+        array as given (no reorientation, as PyRadiomics filters sitk.GetArrayFromImage(image)).
+
+        The values are converted to float64 and filtered along axis 2, then 1, then 0 by the periodic stationary
+        transform: out[o] = sum_j f[j] in[(o + F/2 - j) mod N'], every product and sum rounded to float64, an odd axis
+        wrapped to N' = N + 1 (index N holds index 0) and trimmed back; bit-identical to wavelet.swt_host.  `wavelet`:
+        "coif1" (F = 6: every axis needs at least 5 voxels) or "haar" (F = 2).  `decompositions`: None for all 8, or a
+        collection of names ("wavelet-LLL" or "LLL"); all 8 of a 300 x 512 x 512 volume take 5 GB.  A NaN or +-inf in
+        the volume is a ValueError.
+
+        `image`: a numpy array, a Volume or SimpleITK image (its array; numpy bands come back), a CPU tensor (CPU tensors
+        come back), or a CUDA tensor on the engine's device, read in place after the work queued on the current stream
+        (CUDA float64 tensors on that device come back).  The input is left unchanged."""
+        import torch
+        from . import wavelet as wv
+        wavelet = wv.check_wavelet(wavelet)
+        names = wv.check_decompositions(decompositions)
+        s = self._stage("wavelet", image, None, image_only=True)
+        shape = wv.check_shape(s.vol.shape, wavelet)
+        in_place = _is_tensor(image) and image.is_cuda
+        out = {}
+        band = None
+        for n in names:
+            if band is None or in_place:   # host results are copied out of one device band; CUDA results are the bands
+                band = torch.empty(shape, dtype=torch.float64, device=s.vol.device)
+            self.engine.wavelet_dev(s.vol.data_ptr(), s.dtype, shape, wavelet, wv.band_code(n), band.data_ptr(),
+                                    stream=s.stream)
+            out[n] = s.back(band)
+        return out
+
+    def wavelet_features(self, image, mask, wavelet="coif1", bin_width=25,
+                         classes=("firstorder", "glcm", "glszm", "glrlm", "gldm", "ngtdm"), gldm_alpha=0, spacing=None,
+                         voxel_array_shift=0):
+        """The first-order and texture features of every wavelet decomposition of `image` under `mask` ->
+        lungmask_b200.wavelet.WaveletFeatures: for each of the 8 decompositions of `wavelet` (see `wavelet`), in
+        PyRadiomics' order, the FirstOrderFeatures of `first_order` and the TextureFeatures of `texture` run on that
+        band with the rows of `statistics`.  `vector(label)` gives a row's flat vector with PyRadiomics' keys such as
+        wavelet-LLH_firstorder_Mean.
+
+        `classes`: a non-empty collection of "firstorder", "glcm", "glszm", "glrlm", "gldm" and "ngtdm".  `bin_width`: a
+        positive integer, or a dict giving one for every decomposition name ("wavelet-LLL" or "LLL"): wavelet-LLL scales
+        values by about 2.8, so it may need a wider bin.  Every decomposition's rows are discretised before any
+        first-order or texture kernel runs; a row with more than 255 levels is a ValueError naming the decomposition, the
+        row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`: as for `texture` and
+        `first_order`.  Bad arguments raise before any kernel runs.
+
+        `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the
+        spacing), CPU tensors, or CUDA tensors on the engine's device read in place after the work queued on the current
+        stream; both are left unchanged.  One float64 band of the volume's size is held on the device at a time."""
+        import torch
+        from . import first_order as fo
+        from . import texture as tx
+        from . import wavelet as wv
+        from .statistics import label_name
+        wavelet = wv.check_wavelet(wavelet)
+        widths = wv.check_bin_widths(bin_width)
+        first, texture_classes = wv.check_classes(classes)
+        alpha = tx.check_alpha(gldm_alpha)
+        shift = fo.check_shift(voxel_array_shift)
+        s = self._stage("wavelet_features", image, mask, spacing)
+        shape = wv.check_shape(s.vol.shape, wavelet)
+        band = torch.empty(shape, dtype=torch.float64, device=s.mask.device)
+
+        def compute(name):
+            self.engine.wavelet_dev(s.vol.data_ptr(), s.dtype, shape, wavelet, wv.band_code(name), band.data_ptr(),
+                                    stream=s.stream)
+
+        for name in wv.NAMES:   # every decomposition's discretisation first: a refusal stops the call before any feature kernel
+            compute(name)
+            st = self.engine.label_stats_dev(band.data_ptr(), _native.DTYPE_F64, s.mask.data_ptr(), shape, (), (),
+                                             stream=s.stream)
+            present = set(int(x) for x in np.nonzero(st["voxels"][1:256])[0] + 1)
+            for r in sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]:
+                if st["voxels"][r] - st["nan_voxels"][r]:
+                    row = "%s row %s" % (name, "lung" if r == 256 else "%d (%s)" % (r, label_name(self.modelname, r)))
+                    try:
+                        tx.discretisation(float(st["moments"][r][2]), float(st["moments"][r][3]), widths[name], row)
+                    except ValueError as ex:
+                        raise ValueError("wavelet_features: " + str(ex).split(": ", 1)[1]) from None
+        out = []
+        for name in wv.NAMES:
+            compute(name)
+            d = wv.WaveletDecomposition(name, widths[name])
+            if first:
+                d.first_order = self.first_order(band, s.mask, widths[name], s.spacing, shift)
+            if texture_classes:
+                d.texture = self.texture(band, s.mask, widths[name], s.spacing, texture_classes, alpha)
+            out.append(d)
+        computed = (("firstorder",) if first else ()) + texture_classes
+        return wv.WaveletFeatures(wavelet, computed, s.spacing, shift, alpha, out)
+
+    def _stage(self, what, image, mask, spacing=None, mask_only=False, image_only=False):
         """The inputs of an analysis call as contiguous tensors on the engine's device -> _Staged.  CUDA tensors must be on
         the engine's device and are read in place; a CUDA volume needs a CUDA mask and the reverse.  Everything else is
         uploaded: numpy arrays, CPU tensors as their numpy arrays (bfloat16 widened to float32), a Volume or SimpleITK
         image, which also supplies the orientation and, unless `spacing` is given, the spacing.  The mask is uint8 or bool
-        of the volume's shape.  mask_only: `image` is not used and the volume and its dtype code are None.  Neither input
-        is modified."""
+        of the volume's shape.  mask_only: `image` is not used and the volume and its dtype code are None.  image_only:
+        `mask` is not used, the mask is None and back(t) gives a result of the volume's shape in the type the volume came
+        as.  Neither input is modified."""
         import torch
+        if image_only:
+            return self._stage_image(what, image)
         device = torch.device("cuda", self.engine.device)
         inputs = {"mask": mask} if mask_only else {"volume": image, "mask": mask}
         on_cuda = [_is_tensor(x) and x.is_cuda for x in inputs.values()]
@@ -729,6 +826,34 @@ class LMInferer:
         if m.dtype == torch.bool:
             m = m.view(torch.uint8)
         return _Staged(vol, dtype, m, torch.cuda.current_stream(device).cuda_stream, spacing, code, back)
+
+    def _stage_image(self, what, image):
+        """_stage's image_only mode: the volume alone, read in place as a CUDA tensor on the engine's device or uploaded
+        (numpy arrays, CPU tensors as their numpy arrays with bfloat16 widened to float32, a Volume's or SimpleITK image's
+        array as given, without reorientation).  The orientation is "LPS" and the spacing None."""
+        import torch
+        device = torch.device("cuda", self.engine.device)
+        if _is_tensor(image) and image.is_cuda:
+            if image.device.index != self.engine.device:
+                raise ValueError("%s: the volume tensor is on %s, the engine on cuda:%d" % (what, image.device, self.engine.device))
+            if image.dim() != 3:
+                raise ValueError("%s: expected a (slices, H, W) volume, got shape %s" % (what, tuple(image.shape)))
+            vol = image.detach().contiguous()
+            dtype, back = _tensor_dtype_code(vol), (lambda t: t)
+        else:
+            if _is_tensor(image):
+                image = image.detach()
+                vol, back = (image.float() if image.dtype == torch.bfloat16 else image).numpy(), (lambda t: t.cpu())
+            else:
+                vol, back = self._array_and_orientation(image, what)[0], (lambda t: t.cpu().numpy())
+            vol = np.asarray(vol)
+            if vol.ndim != 3:
+                raise ValueError("%s: expected a (slices, H, W) volume, got shape %s" % (what, tuple(vol.shape)))
+            vol, dtype = _host_volume(vol, what)
+            with warnings.catch_warnings():   # read-only arrays: the host tensor is only copied from
+                warnings.simplefilter("ignore", UserWarning)
+                vol = torch.from_numpy(vol).to(device)
+        return _Staged(vol, dtype, None, torch.cuda.current_stream(device).cuda_stream, None, "LPS", back)
 
 
 def apply(image, model=None, force_cpu=False, batch_size=20, volume_postprocessing=True, tqdm_disable=False):
