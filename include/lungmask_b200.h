@@ -338,6 +338,39 @@ LM_API int lm_first_order_splits_dev(lm_engine* e, const void* d_vol, int dtype,
 LM_API int lm_wavelet_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, int wavelet, int band,
                           double* d_out, void* stream);
 
+/* Image filters (no counterpart in the reference; DESIGN §4.13): PyRadiomics' Square, SquareRoot, Logarithm, Exponential
+ * and Gradient image types with their defaults, so that LMInferer.filtered_features can run the first-order and texture
+ * calls on them.  All three calls take the (n0,n1,n2) volume d_vol (every LM_DTYPE_* code; bool as LM_DTYPE_U8; each
+ * voxel converted to float64), fewer than 2^32 voxels, device memory of the engine's device and the caller's
+ * cudaStream_t with the event-wait rule of lm_apply_dev; every argument is checked before any kernel runs, the call
+ * returns after the engine's stream has synchronised, and a NaN or +-inf anywhere in the volume returns
+ * LM_ERR_NONFINITE (the outputs are then not an image).  Work area: a flag and 24 KB of range partials.
+ * lm_image_range_dev writes the volume's min and max (as float64) to the host out[2].
+ * lm_image_filter_dev writes image type `type` (LM_FILTER_*) to the float64 (n0,n1,n2) d_out, which must not overlap
+ *   d_vol or the table.  With d_table NULL it computes, with c = params[0] formed by the caller in float64 from
+ *   m = max|x|: SQUARE t = c x, t t (c = 1/sqrt(m)); SQUAREROOT x > 0: sqrt(x c), x < 0: -sqrt(-x c), else x (c = m);
+ *   LOGARITHM x > 0: log(x + 1), x < 0: -log(-(x - 1)), else x, then times c (c = m / log(m + 1)); EXPONENTIAL
+ *   exp(c x) (c = log(m) / m); each product, sum and square root rounded to float64 with no fused multiply-add, log and
+ *   exp CUDA's (within 1 ulp).  With d_table (integer dtypes only; device float64 [table_len], 1 <= table_len <= 2^20)
+ *   it writes d_table[x - table_min]; a voxel outside [table_min, table_min + table_len) returns LM_ERR_TABLE_RANGE.
+ * lm_gradient_dev writes ITK's GradientMagnitudeImageFilter to the float64 (n0,n1,n2) d_out (not overlapping d_vol):
+ *   per axis i (x = array axis 2, y = 1, z = 0) g_i = ((0 + k0 f[-1]) + k1 f[0]) + k2 f[+1] with (k0, k1, k2) =
+ *   (-0.5, 0, 0.5) * (1.0 / spacing_xyz[i]) and neighbours outside the array clamped to the edge voxel, then
+ *   sqrt(((0 + g_x^2) + g_y^2) + g_z^2), each product, sum and the square root rounded to float64.  spacing_xyz: 3
+ *   finite positive sizes in mm (x, y, z). */
+#define LM_FILTER_SQUARE 0
+#define LM_FILTER_SQUAREROOT 1
+#define LM_FILTER_LOGARITHM 2
+#define LM_FILTER_EXPONENTIAL 3
+#define LM_ERR_TABLE_RANGE (-42)   /* lm_image_filter_dev: a voxel lies outside the table */
+LM_API int lm_image_range_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, double* out,
+                              void* stream);
+LM_API int lm_image_filter_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, int type,
+                               const double* params, const double* d_table, int64_t table_min, int64_t table_len,
+                               double* d_out, void* stream);
+LM_API int lm_gradient_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, const double* spacing_xyz,
+                           double* d_out, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -13,7 +13,8 @@ LMInferer.texture), `--shape PATH` the mesh shape features
 .csv, LMInferer.shape), and `--first-order PATH` PyRadiomics' first-order features (percentiles, moments, mean absolute
 deviations, energy, entropy, uniformity) of every label and the whole lung (.json / .csv, LMInferer.first_order), and
 `--wavelet PATH` the first-order and texture features of the 8 coif1 (or haar) wavelet decompositions (.json / .csv,
-LMInferer.wavelet_features).
+LMInferer.wavelet_features), and `--filtered PATH` those of the Square, SquareRoot, Logarithm, Exponential and Gradient
+image types (.json / .csv, LMInferer.filtered_features).
 """
 import argparse
 import os
@@ -21,7 +22,7 @@ import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_first_order, save_mask,
                  save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
-                 save_wavelet_features)
+                 save_filtered_features, save_wavelet_features)
 from .logger import logger
 from .mask import LMInferer
 
@@ -98,6 +99,20 @@ def build_parser():
     p.add_argument("--wavelet-classes", metavar="NAMES", type=str, default="firstorder,glcm,glszm,glrlm,gldm,ngtdm",
                    help="Comma-separated feature classes of --wavelet: any of firstorder, glcm, glszm, glrlm, gldm, ngtdm "
                         "(default all)")
+    p.add_argument("--filtered", metavar="PATH", type=str, default=None,
+                   help="Also write the first-order and texture features of PyRadiomics' Square, SquareRoot, Logarithm, "
+                        "Exponential and Gradient image types (keys such as square_firstorder_Mean) of every label and the "
+                        "whole lung: .json (with the exact sums and matrices) or .csv")
+    p.add_argument("--filtered-types", metavar="NAMES", type=str,
+                   default="square,squareroot,logarithm,exponential,gradient",
+                   help="Comma-separated image types of --filtered: any of square, squareroot, logarithm, exponential, "
+                        "gradient (default all)")
+    p.add_argument("--filtered-bin-width", metavar="SPEC", type=str, default="25",
+                   help="Fixed bin width of --filtered: one positive integer, or a default followed by per-type overrides "
+                        "such as 25,gradient=10 (default 25)")
+    p.add_argument("--filtered-classes", metavar="NAMES", type=str, default="firstorder,glcm,glszm,glrlm,gldm,ngtdm",
+                   help="Comma-separated feature classes of --filtered: any of firstorder, glcm, glszm, glrlm, gldm, "
+                        "ngtdm (default all)")
     return p
 
 
@@ -150,6 +165,23 @@ def main(argv=None):
             check_wavelet_classes(wavelet_classes)
         except ValueError as ex:
             sys.exit("--wavelet-classes: %s" % ex)
+    if args.filtered is not None:
+        check_table_path(args.filtered, "filtered")
+        from . import filters
+        filtered_types = [c.strip() for c in args.filtered_types.split(",") if c.strip()]
+        try:
+            filtered_types = filters.check_image_types(filtered_types)
+        except ValueError as ex:
+            sys.exit("--filtered-types: %s" % ex)
+        try:
+            filtered_bin_width = filters.check_bin_widths(filters.parse_bin_widths(args.filtered_bin_width), filtered_types)
+        except (TypeError, ValueError) as ex:
+            sys.exit("--filtered-bin-width: %s" % ex)
+        filtered_classes = [c.strip() for c in args.filtered_classes.split(",") if c.strip()]
+        try:
+            filters.check_classes(filtered_classes)
+        except ValueError as ex:
+            sys.exit("--filtered-classes: %s" % ex)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -196,6 +228,11 @@ def main(argv=None):
         logger.info(f"Save wavelet features to: {args.wavelet}")
         save_wavelet_features(args.wavelet, inferer.wavelet_features(image, result, wavelet=args.wavelet_name,
                                                                      bin_width=wavelet_bin_width, classes=wavelet_classes))
+    if args.filtered is not None:
+        logger.info(f"Save filtered-image features to: {args.filtered}")
+        save_filtered_features(args.filtered, inferer.filtered_features(image, result, image_types=filtered_types,
+                                                                        bin_width=filtered_bin_width,
+                                                                        classes=filtered_classes))
 
 
 if __name__ == "__main__":

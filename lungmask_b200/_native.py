@@ -13,6 +13,8 @@ DTYPE_I16, DTYPE_F32, DTYPE_F64 = 0, 1, 2   # LM_DTYPE_* of lm_apply_volume_prob
 DTYPE_U8, DTYPE_I8, DTYPE_I32, DTYPE_I64, DTYPE_F16, DTYPE_BF16 = 3, 4, 5, 6, 7, 8   # lm_apply_dev only (U8 also bool)
 WAVELET_CODES = {"coif1": 0, "haar": 1}   # LM_WAVELET_* of lm_wavelet_dev
 ERR_NONFINITE = -41                       # LM_ERR_NONFINITE
+FILTER_CODES = {"square": 0, "squareroot": 1, "logarithm": 2, "exponential": 3}   # LM_FILTER_* of lm_image_filter_dev
+ERR_TABLE_RANGE = -42                     # LM_ERR_TABLE_RANGE
 
 _lib = None
 
@@ -65,6 +67,9 @@ def lib():
         "lm_first_order_sums_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32] + [vp] * 12, i32),
         "lm_first_order_splits_dev": ([vp, vp, i32, u8p, i32, i32, i32] + [vp] * 11, i32),
         "lm_wavelet_dev": ([vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
+        "lm_image_range_dev": ([vp, vp, i32, i32, i32, i32, vp, vp], i32),
+        "lm_image_filter_dev": ([vp, vp, i32, i32, i32, i32, i32, vp, vp, C.c_int64, C.c_int64, vp, vp], i32),
+        "lm_gradient_dev": ([vp, vp, i32, i32, i32, i32, vp, vp, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -95,7 +100,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_wavelet_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -111,6 +116,13 @@ def _ptr(a):
 def _check(rc):
     if rc != 0:
         raise NativeError("lungmask_b200 native call failed (%d): %s" % (rc, lib().lm_last_error().decode()))
+
+
+def _filter_check(rc, what):
+    """_check for the filter calls, with a non-finite volume as ValueError."""
+    if rc == ERR_NONFINITE:
+        raise ValueError("%s: %s" % (what, lib().lm_last_error().decode().split(": ", 1)[1]))
+    _check(rc)
 
 
 def _as(a, dtype, ndim=None):
@@ -469,6 +481,44 @@ class Engine:
         if rc == ERR_NONFINITE:
             raise ValueError("wavelet: " + lib().lm_last_error().decode().split(": ", 1)[1])
         _check(rc)
+
+    # ---- image filters (lm_image_range_dev, lm_image_filter_dev, lm_gradient_dev)
+    def image_range_dev(self, d_vol_ptr, dtype_code, shape, stream=0):
+        """(min, max) of a C-contiguous `shape` device volume of element type `dtype_code`, every voxel as float64
+        (`stream` as for apply_dev).  ValueError when the volume holds a NaN or +-inf; NativeError for the other
+        failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        out = np.zeros(2, np.float64)
+        rc = lib().lm_image_range_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2, _ptr(out),
+                                      C.c_void_p(int(stream)) if stream else None)
+        _filter_check(rc, "image range")
+        return float(out[0]), float(out[1])
+
+    def image_filter_dev(self, d_vol_ptr, dtype_code, shape, image_type, param, d_out_ptr, table=None, stream=0):
+        """Writes the elementwise image type `image_type` ("square", "squareroot", "logarithm", "exponential") of a
+        C-contiguous `shape` device volume to the float64 `shape` device buffer `d_out_ptr`: with the host scalar
+        `param`, or, when `table` = (device pointer of a float64 table, its first value, its length) is given, as
+        table[x - first value].  ValueError when the volume holds a NaN or +-inf; NativeError for the other failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        if image_type not in FILTER_CODES:
+            raise ValueError("image_filter_dev: unknown image type %r (known: %s)" % (image_type, ", ".join(FILTER_CODES)))
+        params = np.array([param], np.float64)
+        d_table, table_min, table_len = table if table is not None else (0, 0, 0)
+        rc = lib().lm_image_filter_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2,
+                                       FILTER_CODES[image_type], _ptr(params), C.c_void_p(d_table or None),
+                                       int(table_min), int(table_len), C.c_void_p(d_out_ptr),
+                                       C.c_void_p(int(stream)) if stream else None)
+        _filter_check(rc, image_type)
+
+    def gradient_dev(self, d_vol_ptr, dtype_code, shape, spacing_xyz, d_out_ptr, stream=0):
+        """Writes the gradient magnitude (ITK's GradientMagnitudeImageFilter, spacing (x, y, z) in mm) of a
+        C-contiguous `shape` device volume to the float64 `shape` device buffer `d_out_ptr`.  ValueError when the volume
+        holds a NaN or +-inf; NativeError for the other failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        sp = np.array([float(s) for s in spacing_xyz], np.float64)
+        rc = lib().lm_gradient_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2, _ptr(sp),
+                                   C.c_void_p(d_out_ptr), C.c_void_p(int(stream)) if stream else None)
+        _filter_check(rc, "gradient")
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

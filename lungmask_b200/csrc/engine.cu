@@ -24,6 +24,7 @@
 #include "shape.cuh"
 #include "first_order.cuh"
 #include "wavelet.cuh"
+#include "filters.cuh"
 
 using namespace lm;
 
@@ -203,6 +204,7 @@ struct lm_engine {
   ShapeWork shape;        // lm_shape_sums_dev, lm_max_diameters_dev: sums, line tables, diameter candidates
   FirstOrderWork first_order;   // lm_first_order_sums_dev, lm_first_order_splits_dev: row table, histograms, sums
   WaveletWork wavelet;          // lm_wavelet_dev: the non-finite flag
+  FilterWork filters;           // lm_image_range_dev, lm_image_filter_dev, lm_gradient_dev: a flag, the range partials
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -931,6 +933,7 @@ void lm_destroy(lm_engine* e) {
   e->shape.release();
   e->first_order.release();
   e->wavelet.release();
+  e->filters.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1420,6 +1423,82 @@ int lm_wavelet_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, i
   const int rc = wavelet_band(e->wavelet, d_vol, dtype, n0, n1, n2, wavelet, band, d_out, e->st, &e->launches);
   if (rc == LM_ERR_NONFINITE) return fail(rc, "%s: the volume holds a NaN or +-inf", fn);
   return rc;
+}
+
+// The volume arguments shared by the filter calls: the engine, the volume pointer, its extents and dtype code.
+static int filter_volume_args(const char* fn, lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2) {
+  if (!e || !d_vol) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (n >= ((size_t)1 << 32)) return fail(-1, "%s: %zu voxels, the filter calls take fewer than 2^32", fn, n);
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  return 0;
+}
+
+static bool overlaps(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+  const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+  return a0 < b0 + b_bytes && b0 < a0 + a_bytes;
+}
+
+static int filter_result(const char* fn, int rc) {
+  if (rc == LM_ERR_NONFINITE) return fail(rc, "%s: the volume holds a NaN or +-inf", fn);
+  if (rc == LM_ERR_TABLE_RANGE) return fail(rc, "%s: a voxel lies outside the table", fn);
+  return rc;
+}
+
+int lm_image_range_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, double* out, void* stream) {
+  static const char* fn = "lm_image_range_dev";
+  RC(filter_volume_args(fn, e, d_vol, dtype, n0, n1, n2));
+  if (!out) return fail(-1, "%s: NULL argument", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}}));
+  return filter_result(fn, image_range(e->filters, d_vol, dtype, (size_t)n0 * n1 * n2, out, e->num_sms, e->st,
+                                       &e->launches));
+}
+
+int lm_image_filter_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, int type, const double* params,
+                        const double* d_table, int64_t table_min, int64_t table_len, double* d_out, void* stream) {
+  static const char* fn = "lm_image_filter_dev";
+  RC(filter_volume_args(fn, e, d_vol, dtype, n0, n1, n2));
+  if (!d_out) return fail(-1, "%s: NULL argument", fn);
+  if (type < LM_FILTER_SQUARE || type > LM_FILTER_EXPONENTIAL) return fail(-1, "%s: unknown image type code %d", fn, type);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (overlaps(d_vol, n * dtype_bytes(dtype), d_out, n * sizeof(double))) return fail(-1, "%s: d_out overlaps d_vol", fn);
+  double param = 0.0;
+  if (d_table) {
+    const bool integer = dtype == LM_DTYPE_U8 || dtype == LM_DTYPE_I8 || dtype == LM_DTYPE_I16 || dtype == LM_DTYPE_I32 ||
+                         dtype == LM_DTYPE_I64;
+    if (!integer) return fail(-1, "%s: a table needs an integer volume, got dtype code %d", fn, dtype);
+    if (table_len < 1 || table_len > ((int64_t)1 << 20))
+      return fail(-1, "%s: table length %lld not in [1, 2^20]", fn, (long long)table_len);
+    if (table_min > INT64_MAX - table_len) return fail(-1, "%s: table [%lld, +%lld) overflows int64", fn,
+                                                       (long long)table_min, (long long)table_len);
+    if (overlaps(d_table, (size_t)table_len * sizeof(double), d_out, n * sizeof(double)))
+      return fail(-1, "%s: d_out overlaps d_table", fn);
+  } else {
+    if (!params) return fail(-1, "%s: NULL params without a table", fn);
+    param = params[0];
+    if (!isfinite(param)) return fail(-1, "%s: params[0] = %g is not finite", fn, param);
+  }
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_out", d_out}, {"d_table", d_table}}));
+  return filter_result(fn, image_filter(e->filters, d_vol, dtype, n, type, param, d_table, table_min, table_len, d_out,
+                                        e->num_sms, e->st, &e->launches));
+}
+
+int lm_gradient_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, const double* spacing_xyz,
+                    double* d_out, void* stream) {
+  static const char* fn = "lm_gradient_dev";
+  RC(filter_volume_args(fn, e, d_vol, dtype, n0, n1, n2));
+  if (!d_out || !spacing_xyz) return fail(-1, "%s: NULL argument", fn);
+  double inv[3];
+  for (int a = 0; a < 3; ++a) {
+    if (!(isfinite(spacing_xyz[a]) && spacing_xyz[a] > 0.0))
+      return fail(-1, "%s: spacing %g along %c is not a finite positive size", fn, spacing_xyz[a], "xyz"[a]);
+    inv[a] = 1.0 / spacing_xyz[a];
+  }
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (overlaps(d_vol, n * dtype_bytes(dtype), d_out, n * sizeof(double))) return fail(-1, "%s: d_out overlaps d_vol", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_out", d_out}}));
+  return filter_result(fn, gradient_magnitude(e->filters, d_vol, dtype, n0, n1, n2, inv, d_out, e->st, &e->launches));
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

@@ -410,7 +410,8 @@ def save_probabilities(path, probs, like=None):
 def check_table_path(path, kind):
     """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
     ("clusters"), save_regional_statistics ("regions"), save_texture ("texture"), save_shape ("shape"),
-    save_first_order ("first_order") or save_wavelet_features ("wavelet") cannot write."""
+    save_first_order ("first_order"), save_wavelet_features ("wavelet") or save_filtered_features ("filtered") cannot
+    write."""
     if not path.lower().endswith((".json", ".csv")):
         raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
 
@@ -554,6 +555,27 @@ def save_wavelet_features(path, features):
         return _save_json(path, features)
     labels = features.labels
     d = features.decompositions[0]
+    names = {r.label: r.name for r in (d.first_order or d.texture).rows}
+    keys = list(features.vector(labels[0]))
+    lines = [",".join(["label", "name", "voxels"] + keys)]
+    for label in labels:
+        v = features.vector(label)
+        cells = [label, names[label], features.voxels(label)] + [v[k] for k in keys]
+        lines.append(",".join(_csv_cell(c) for c in cells))
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def save_filtered_features(path, features):
+    """Writes the FilteredFeatures of LMInferer.filtered_features: .json (the classes and, per image type, its bin width
+    and the to_dict() of its first-order and texture features with their exact histograms, sums and matrices, NaN as
+    null) or .csv (a header, then one line per row: label, name, voxels, then the row's flat vector
+    FilteredFeatures.vector with PyRadiomics' keys such as square_firstorder_Mean; NaN is "nan")."""
+    check_table_path(path, "filtered")
+    if path.lower().endswith(".json"):
+        return _save_json(path, features)
+    labels = features.labels
+    d = features.images[0]
     names = {r.label: r.name for r in (d.first_order or d.texture).rows}
     keys = list(features.vector(labels[0]))
     lines = [",".join(["label", "name", "voxels"] + keys)]

@@ -723,7 +723,6 @@ class LMInferer:
         from . import first_order as fo
         from . import texture as tx
         from . import wavelet as wv
-        from .statistics import label_name
         wavelet = wv.check_wavelet(wavelet)
         widths = wv.check_bin_widths(bin_width)
         first, texture_classes = wv.check_classes(classes)
@@ -737,9 +736,25 @@ class LMInferer:
             self.engine.wavelet_dev(s.vol.data_ptr(), s.dtype, shape, wavelet, wv.band_code(name), band.data_ptr(),
                                     stream=s.stream)
 
-        for name in wv.NAMES:   # every decomposition's discretisation first: a refusal stops the call before any feature kernel
+        out = self._image_features("wavelet_features", s, band, wv.NAMES, compute, widths, first, texture_classes, shift,
+                                   alpha)
+        computed = (("firstorder",) if first else ()) + texture_classes
+        return wv.WaveletFeatures(wavelet, computed, s.spacing, shift, alpha, out)
+
+    def _image_features(self, what, s, image, names, compute, widths, first, texture_classes, shift, alpha):
+        """The feature loop of wavelet_features and filtered_features over the derived images `names`: compute(name)
+        writes image `name` to the float64 device tensor `image` of the staged volume's shape.  Every image's rows
+        (those of `statistics`) are discretised first with §4.9's rule, so that a row with more than 255 levels is a
+        ValueError naming the image, the row and a sufficient bin width before any first-order or texture kernel runs;
+        then each image is recomputed and `first_order` (when `first`) and `texture` (on `texture_classes`) run on it
+        with the staged mask.  -> [wavelet.ImageFeatures] in the order of `names`."""
+        from . import texture as tx
+        from . import wavelet as wv
+        from .statistics import label_name
+        shape = tuple(image.shape)
+        for name in names:   # every image's discretisation first: a refusal stops the call before any feature kernel
             compute(name)
-            st = self.engine.label_stats_dev(band.data_ptr(), _native.DTYPE_F64, s.mask.data_ptr(), shape, (), (),
+            st = self.engine.label_stats_dev(image.data_ptr(), _native.DTYPE_F64, s.mask.data_ptr(), shape, (), (),
                                              stream=s.stream)
             present = set(int(x) for x in np.nonzero(st["voxels"][1:256])[0] + 1)
             for r in sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]:
@@ -748,18 +763,118 @@ class LMInferer:
                     try:
                         tx.discretisation(float(st["moments"][r][2]), float(st["moments"][r][3]), widths[name], row)
                     except ValueError as ex:
-                        raise ValueError("wavelet_features: " + str(ex).split(": ", 1)[1]) from None
+                        raise ValueError(what + ": " + str(ex).split(": ", 1)[1]) from None
         out = []
-        for name in wv.NAMES:
+        for name in names:
             compute(name)
-            d = wv.WaveletDecomposition(name, widths[name])
+            d = wv.ImageFeatures(name, widths[name])
             if first:
-                d.first_order = self.first_order(band, s.mask, widths[name], s.spacing, shift)
+                d.first_order = self.first_order(image, s.mask, widths[name], s.spacing, shift)
             if texture_classes:
-                d.texture = self.texture(band, s.mask, widths[name], s.spacing, texture_classes, alpha)
+                d.texture = self.texture(image, s.mask, widths[name], s.spacing, texture_classes, alpha)
             out.append(d)
+        return out
+
+    def _filter_plan(self, s, names, spacing, use_spacing):
+        """Checks the image types `names` against the staged volume before any image is written -> compute(name, out):
+        writes image type `name` of the volume to the float64 device tensor `out`.  The range pass runs once (a NaN or
+        +-inf is a ValueError), an all-zero volume is refused for square, logarithm and exponential, and the gradient
+        needs its spacing.  Integer volumes within lungmask_b200.filters.table_span get each elementwise type as a
+        device table of the numpy statement, built on first use."""
+        import torch
+        from . import filters as flt
+        shape = flt.check_shape(s.vol.shape)
+        grad_spacing = flt.gradient_spacing(spacing, use_spacing) if "gradient" in names else None
+        elementwise = [n for n in names if n != "gradient"]
+        lo = hi = 0.0
+        if elementwise:
+            lo, hi = self.engine.image_range_dev(s.vol.data_ptr(), s.dtype, shape, stream=s.stream)
+            for n in elementwise:
+                flt.check_range(n, lo, hi)
+        span = flt.table_span(s.dtype, lo, hi) if elementwise else None
+        tables = {}
+
+        def compute(name, out):
+            if name == "gradient":
+                self.engine.gradient_dev(s.vol.data_ptr(), s.dtype, shape, grad_spacing, out.data_ptr(), stream=s.stream)
+                return
+            if span is None:
+                self.engine.image_filter_dev(s.vol.data_ptr(), s.dtype, shape, name, flt.scalar(name, max(abs(lo), abs(hi))),
+                                             out.data_ptr(), stream=s.stream)
+                return
+            if name not in tables:   # uploaded on the current stream, the one the call runs on
+                tables[name] = torch.from_numpy(flt.table(name, *span)).to(out.device)
+            self.engine.image_filter_dev(s.vol.data_ptr(), s.dtype, shape, name, 0.0, out.data_ptr(),
+                                         table=(tables[name].data_ptr(), span[0], span[1]), stream=s.stream)
+
+        return compute
+
+    def filtered(self, image, image_types=None, spacing=None, gradient_use_spacing=True):
+        """PyRadiomics' Square, SquareRoot, Logarithm, Exponential and Gradient image types of `image` (get<Type>Image
+        with its defaults) -> {name: float64 image of the image's shape}, in that order: "square", "squareroot",
+        "logarithm", "exponential", "gradient".  The (S, H, W) array is taken as given (no reorientation), converted to
+        float64, with m = max|x| over the whole volume; lungmask_b200.filters.filter_host is the numpy statement.
+        Integer volumes whose max - min is below 2^20 are bit-identical to it (a table of the statement); float and
+        wider integer volumes are bit-identical for square, squareroot and gradient, and within DESIGN §4.13's ulp bound
+        for logarithm and exponential (CUDA's log and exp).  `image_types`: None for all 5, or a collection of names.
+        The gradient uses `spacing` (x, y, z) mm, or a Volume's or SimpleITK image's, unless gradient_use_spacing is
+        False (spacing 1).  A NaN or +-inf in the volume, or an all-zero volume for square, logarithm or exponential, is
+        a ValueError before any image is written.
+
+        `image`: a numpy array, a Volume or SimpleITK image (numpy images come back), a CPU tensor (CPU tensors come
+        back), or a CUDA tensor on the engine's device, read in place after the work queued on the current stream (CUDA
+        float64 tensors on that device come back).  The input is left unchanged."""
+        import torch
+        from . import filters as flt
+        names = flt.check_image_types(image_types)
+        if spacing is None and not isinstance(image, np.ndarray) and not _is_tensor(image):
+            spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
+        s = self._stage("filtered", image, None, image_only=True)
+        compute = self._filter_plan(s, names, spacing, gradient_use_spacing)
+        in_place = _is_tensor(image) and image.is_cuda
+        out = {}
+        buf = None
+        for n in names:
+            if buf is None or in_place:   # host results are copied out of one device image; CUDA results are the images
+                buf = torch.empty(tuple(s.vol.shape), dtype=torch.float64, device=s.vol.device)
+            compute(n, buf)
+            out[n] = s.back(buf)
+        return out
+
+    def filtered_features(self, image, mask, image_types=None, bin_width=25,
+                          classes=("firstorder", "glcm", "glszm", "glrlm", "gldm", "ngtdm"), gldm_alpha=0, spacing=None,
+                          voxel_array_shift=0, gradient_use_spacing=True):
+        """The first-order and texture features of PyRadiomics' Square, SquareRoot, Logarithm, Exponential and Gradient
+        image types of `image` under `mask` -> lungmask_b200.filters.FilteredFeatures: for each image type of
+        `image_types` (None for all 5; see `filtered`), in PyRadiomics' order, the FirstOrderFeatures of `first_order`
+        and the TextureFeatures of `texture` run on that image with the rows of `statistics`.  `vector(label)` gives a
+        row's flat vector with PyRadiomics' keys such as square_firstorder_Mean or gradient_glcm_Contrast.
+
+        `classes`: a non-empty collection of "firstorder", "glcm", "glszm", "glrlm", "gldm" and "ngtdm".  `bin_width`: a
+        positive integer, or a dict giving one for every requested image type.  Every image's rows are discretised
+        before any first-order or texture kernel runs; a row with more than 255 levels is a ValueError naming the image
+        type, the row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`: as for `texture` and
+        `first_order`; the spacing is also the gradient's (see `filtered`).  Bad arguments raise before any kernel runs.
+
+        `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the
+        spacing), CPU tensors, or CUDA tensors on the engine's device read in place after the work queued on the current
+        stream; both are left unchanged.  One float64 image of the volume's size is held on the device at a time."""
+        import torch
+        from . import filters as flt
+        from . import first_order as fo
+        from . import texture as tx
+        names = flt.check_image_types(image_types)
+        widths = flt.check_bin_widths(bin_width, names)
+        first, texture_classes = flt.check_classes(classes)
+        alpha = tx.check_alpha(gldm_alpha)
+        shift = fo.check_shift(voxel_array_shift)
+        s = self._stage("filtered_features", image, mask, spacing)
+        compute = self._filter_plan(s, names, s.spacing, gradient_use_spacing)
+        image_buf = torch.empty(tuple(s.vol.shape), dtype=torch.float64, device=s.mask.device)
+        out = self._image_features("filtered_features", s, image_buf, names, lambda n: compute(n, image_buf), widths,
+                                   first, texture_classes, shift, alpha)
         computed = (("firstorder",) if first else ()) + texture_classes
-        return wv.WaveletFeatures(wavelet, computed, s.spacing, shift, alpha, out)
+        return flt.FilteredFeatures(computed, s.spacing, shift, alpha, bool(gradient_use_spacing), out)
 
     def _stage(self, what, image, mask, spacing=None, mask_only=False, image_only=False):
         """The inputs of an analysis call as contiguous tensors on the engine's device -> _Staged.  CUDA tensors must be on

@@ -196,7 +196,8 @@ def swt_host(volume, wavelet="coif1", decompositions=None):
 
 
 @dataclass
-class WaveletDecomposition:
+class ImageFeatures:
+    """The features of one derived image: a wavelet decomposition here, an image type of lungmask_b200.filters."""
     name: str
     bin_width: int
     first_order: Optional[object] = None   # first_order.FirstOrderFeatures, None without "firstorder"
@@ -206,6 +207,25 @@ class WaveletDecomposition:
         return {"bin_width": self.bin_width,
                 "firstorder": self.first_order.to_dict() if self.first_order is not None else None,
                 "texture": self.texture.to_dict() if self.texture is not None else None}
+
+
+WaveletDecomposition = ImageFeatures
+
+
+def image_vector(images, classes, label):
+    """The flat feature vector of a row over a list of ImageFeatures, with PyRadiomics' keys <image>_<class>_<feature>,
+    in image, class (`classes`, in the order of FEATURE_CLASSES) and feature order."""
+    from .first_order import FIRST_ORDER_FEATURES
+    from .texture import GLCM_FEATURES, GLDM_FEATURES, GLRLM_FEATURES, GLSZM_FEATURES, NGTDM_FEATURES
+    names = dict(zip(FEATURE_CLASSES, (FIRST_ORDER_FEATURES, GLCM_FEATURES, GLSZM_FEATURES, GLRLM_FEATURES,
+                                       GLDM_FEATURES, NGTDM_FEATURES)))
+    out = {}
+    for d in images:
+        for c in classes:
+            f = d.first_order[label].features if c == "firstorder" else getattr(d.texture[label], c)
+            for k in names[c]:
+                out["%s_%s_%s" % (d.name, c, k)] = f[k]
+    return out
 
 
 @dataclass
@@ -238,17 +258,7 @@ class WaveletFeatures:
     def vector(self, label):
         """The flat feature vector of a row with PyRadiomics' keys, such as wavelet-LLH_firstorder_Mean or
         wavelet-LLL_glcm_Contrast, in decomposition, class and feature order."""
-        from .first_order import FIRST_ORDER_FEATURES
-        from .texture import GLCM_FEATURES, GLDM_FEATURES, GLRLM_FEATURES, GLSZM_FEATURES, NGTDM_FEATURES
-        names = dict(zip(FEATURE_CLASSES, (FIRST_ORDER_FEATURES, GLCM_FEATURES, GLSZM_FEATURES, GLRLM_FEATURES,
-                                           GLDM_FEATURES, NGTDM_FEATURES)))
-        out = {}
-        for d in self.decompositions:
-            for c in self.classes:
-                f = d.first_order[label].features if c == "firstorder" else getattr(d.texture[label], c)
-                for k in names[c]:
-                    out["%s_%s_%s" % (d.name, c, k)] = f[k]
-        return out
+        return image_vector(self.decompositions, self.classes, label)
 
     def to_dict(self):
         """JSON-ready: the to_dict() of every decomposition's FirstOrderFeatures and TextureFeatures (NaN as None)."""
