@@ -282,6 +282,38 @@ LM_API int lm_shape_sums_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1
 LM_API int lm_max_diameters_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const double* spacing,
                                 double* d2, void* stream);
 
+/* Surface meshes (no counterpart in the reference; DESIGN §4.14): the marching-cubes mesh of one row that
+ * lm_shape_sums_dev's SurfaceArea and MeshVolume describe, so that LMInferer.mesh can return it and io.save_mesh write it
+ * as STL, OBJ or PLY.  Both take device memory of the engine's device and the caller's cudaStream_t with the event-wait
+ * rule of lm_apply_dev, check every argument before any kernel runs and return after the engine's stream has
+ * synchronised; the mask is never written.  mask (n0,n1,n2) uint8 and row (1..256) as lm_max_diameters_dev, on the mask
+ * padded with one voxel of outside (grid points q with q_k in -1..n_k).
+ *   Vertices: one per crossing edge, the edge from grid point q to q + e_m (m = 0, 1, 2 an array axis) whose ends differ
+ *   in membership; ordered by q in the padded grid's linear order (axis 0 slowest), then m.
+ *   Triangles: each cube (lowest corner p) gets the triangles of its configuration from the caller's table, ordered by
+ *   cube in the padded linear order, then table order.  tri_offsets [257] (host int32, non-decreasing from 0, at most
+ *   16 triangles per configuration, none for configurations 0 and 255): configuration c owns triangles
+ *   [tri_offsets[c], tri_offsets[c + 1]); tri_codes [3 tri_offsets[256]] (host uint8): per triangle vertex the code
+ *   (a << 2) | m of the cube edge from corner a (0..7, as lm_shape_sums_dev numbers them, with bit 2 - m clear) to corner
+ *   a + e_m, which must cross in that configuration.  The edge names the vertex owned by (p + corner a, m).
+ * lm_mesh_counts_dev: *n_vertices = V, *n_triangles = T (host int64).
+ * lm_mesh_emit_dev: n_vertices and n_triangles must equal V and T (the call recounts them), each at most 2^31 - 1.
+ *   d_index2 (V,3) int32: the doubled array-axis coordinates 2q + e_m of every vertex (exact).
+ *   d_vertices (V,3) float64: with (x, y, z) = (u2, u1, u0) / 2 of u = index2, o = geometry[0..2] (mm), D = geometry[3..11]
+ *     (row-major 3x3, columns = array axes 2, 1, 0) and s = geometry[12..14] (spacing x, y, z in mm, positive), p_c =
+ *     ((o_c + D[c][0] (s_x x)) + D[c][1] (s_y y)) + D[c][2] (s_z z), every product and sum rounded on its own (no fused
+ *     multiply-add); LM_MESH_RAS negates p_0 and p_1.
+ *   d_triangles (T,3) int32: vertex indices; the last two are swapped when det D < 0, so that the normals point out of
+ *     the row in patient space as the table's do in (x, y, z).
+ *   Work area: the table and 16 bytes per line of the padded grid along axis 2 ((n0 + 1) (n1 + 1) lines), kept by the
+ *   engine. */
+#define LM_MESH_RAS 1
+LM_API int lm_mesh_counts_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const int32_t* tri_offsets,
+                              const uint8_t* tri_codes, int64_t* n_vertices, int64_t* n_triangles, void* stream);
+LM_API int lm_mesh_emit_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const int32_t* tri_offsets,
+                            const uint8_t* tri_codes, const double* geometry, int flags, int64_t n_vertices,
+                            int64_t n_triangles, int32_t* d_index2, double* d_vertices, int32_t* d_triangles, void* stream);
+
 /* First-order (histogram) sums (no counterpart in the reference; DESIGN §4.11): LMInferer.first_order computes
  * PyRadiomics' 18 default firstorder features of every row of lm_label_stats_dev from these two passes.  Both take
  * device memory of the engine's device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev, check

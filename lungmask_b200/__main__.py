@@ -14,14 +14,16 @@ LMInferer.texture), `--shape PATH` the mesh shape features
 deviations, energy, entropy, uniformity) of every label and the whole lung (.json / .csv, LMInferer.first_order), and
 `--wavelet PATH` the first-order and texture features of the 8 coif1 (or haar) wavelet decompositions (.json / .csv,
 LMInferer.wavelet_features), and `--filtered PATH` those of the Square, SquareRoot, Logarithm, Exponential and Gradient
-image types (.json / .csv, LMInferer.filtered_features).
+image types (.json / .csv, LMInferer.filtered_features), and `--mesh DIR` the marching-cubes surface of every present
+label and of the whole lung, one file per row (`--mesh-format` stl, obj or ply, `--mesh-space` lps or ras;
+LMInferer.mesh with the input's geometry).
 """
 import argparse
 import os
 import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_first_order, save_mask,
-                 save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
+                 save_mesh, save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
                  save_filtered_features, save_wavelet_features)
 from .logger import logger
 from .mask import LMInferer
@@ -113,7 +115,19 @@ def build_parser():
     p.add_argument("--filtered-classes", metavar="NAMES", type=str, default="firstorder,glcm,glszm,glrlm,gldm,ngtdm",
                    help="Comma-separated feature classes of --filtered: any of firstorder, glcm, glszm, glrlm, gldm, "
                         "ngtdm (default all)")
+    p.add_argument("--mesh", metavar="DIR", type=str, default=None,
+                   help="Also write the marching-cubes surface (the mesh of --shape, in patient space) of every present "
+                        "label and of the whole lung to DIR, one file per row named after it (right_lung.stl, lung.stl)")
+    p.add_argument("--mesh-format", choices=["stl", "obj", "ply"], default="stl",
+                   help="File format of --mesh: binary STL (default), ASCII OBJ or binary PLY")
+    p.add_argument("--mesh-space", choices=["lps", "ras"], default="lps",
+                   help="Frame of the --mesh positions: LPS (DICOM / ITK, default) or RAS (3D Slicer, NIfTI)")
     return p
+
+
+def mesh_file_name(mesh, fmt):
+    """The file --mesh writes a row's mesh to: its name with spaces as underscores."""
+    return "%s.%s" % (str(mesh.name).replace(" ", "_"), fmt)
 
 
 def main(argv=None):
@@ -182,6 +196,12 @@ def main(argv=None):
             filters.check_classes(filtered_classes)
         except ValueError as ex:
             sys.exit("--filtered-classes: %s" % ex)
+    if args.mesh is not None:
+        if os.path.exists(args.mesh) and not os.path.isdir(args.mesh):
+            sys.exit("--mesh: %s exists and is not a directory" % args.mesh)
+        parent = os.path.dirname(os.path.abspath(args.mesh))
+        if not os.path.isdir(parent):
+            sys.exit("--mesh: the parent directory of %s does not exist" % args.mesh)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -233,6 +253,12 @@ def main(argv=None):
         save_filtered_features(args.filtered, inferer.filtered_features(image, result, image_types=filtered_types,
                                                                         bin_width=filtered_bin_width,
                                                                         classes=filtered_classes))
+    if args.mesh is not None:
+        logger.info(f"Save meshes to: {args.mesh}")
+        os.makedirs(args.mesh, exist_ok=True)
+        for m in inferer.mesh(result, image=image, space=args.mesh_space):
+            if m.n_triangles or m.label == "lung":
+                save_mesh(os.path.join(args.mesh, mesh_file_name(m, args.mesh_format)), m)
 
 
 if __name__ == "__main__":

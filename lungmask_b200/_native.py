@@ -15,6 +15,7 @@ WAVELET_CODES = {"coif1": 0, "haar": 1}   # LM_WAVELET_* of lm_wavelet_dev
 ERR_NONFINITE = -41                       # LM_ERR_NONFINITE
 FILTER_CODES = {"square": 0, "squareroot": 1, "logarithm": 2, "exponential": 3}   # LM_FILTER_* of lm_image_filter_dev
 ERR_TABLE_RANGE = -42                     # LM_ERR_TABLE_RANGE
+MESH_RAS = 1                              # LM_MESH_RAS of lm_mesh_emit_dev
 
 _lib = None
 
@@ -64,6 +65,8 @@ def lib():
         "lm_neighbour_counts_dev": ([vp, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_shape_sums_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_max_diameters_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp], i32),
+        "lm_mesh_counts_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp, vp, vp], i32),
+        "lm_mesh_emit_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp, i32, C.c_int64, C.c_int64, vp, vp, vp, vp], i32),
         "lm_first_order_sums_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32] + [vp] * 12, i32),
         "lm_first_order_splits_dev": ([vp, vp, i32, u8p, i32, i32, i32] + [vp] * 11, i32),
         "lm_wavelet_dev": ([vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
@@ -100,7 +103,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -427,6 +430,33 @@ class Engine:
         _check(lib().lm_max_diameters_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, int(row), _ptr(sp), _ptr(d2),
                                           C.c_void_p(int(stream)) if stream else None))
         return d2
+
+    # ---- surface meshes (lm_mesh_counts_dev, lm_mesh_emit_dev)
+    def mesh_counts_dev(self, d_mask_ptr, shape, row, tri_offsets, tri_codes, stream=0):
+        """-> (V, T): the vertices and triangles of the marching-cubes mesh of `row` (1..255, or 256 for mask != 0) of a
+        (n0,n1,n2) uint8 device mask padded with outside, for the table (tri_offsets int32 [257], tri_codes uint8
+        [3 tri_offsets[256]] of (corner << 2) | axis codes; `stream` as for apply_dev)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        off, codes = _as(tri_offsets, np.int32, 1), _as(tri_codes, np.uint8, 1)
+        nv, nt = C.c_int64(0), C.c_int64(0)
+        _check(lib().lm_mesh_counts_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, int(row), _ptr(off), _ptr(codes),
+                                        C.byref(nv), C.byref(nt), C.c_void_p(int(stream)) if stream else None))
+        return int(nv.value), int(nt.value)
+
+    def mesh_emit_dev(self, d_mask_ptr, shape, row, tri_offsets, tri_codes, geometry, n_vertices, n_triangles, d_index2_ptr,
+                      d_vertices_ptr, d_triangles_ptr, ras=False, stream=0):
+        """Writes the mesh of `row` (counts from mesh_counts_dev): int32 (V,3) doubled coordinates, float64 (V,3) positions
+        and int32 (T,3) vertex indices to the device pointers.  `geometry`: 15 float64, origin (3), direction (9, row-major)
+        and spacing (x, y, z); `ras` negates the first two components."""
+        n0, n1, n2 = (int(x) for x in shape)
+        off, codes = _as(tri_offsets, np.int32, 1), _as(tri_codes, np.uint8, 1)
+        geo = np.ascontiguousarray(geometry, dtype=np.float64).reshape(-1)
+        if geo.size != 15:
+            raise ValueError("mesh_emit_dev: geometry needs 15 values, got %d" % geo.size)
+        _check(lib().lm_mesh_emit_dev(self._h, C.c_void_p(d_mask_ptr), n0, n1, n2, int(row), _ptr(off), _ptr(codes), _ptr(geo),
+                                      MESH_RAS if ras else 0, int(n_vertices), int(n_triangles),
+                                      C.c_void_p(d_index2_ptr or None), C.c_void_p(d_vertices_ptr or None),
+                                      C.c_void_p(d_triangles_ptr or None), C.c_void_p(int(stream)) if stream else None))
 
     # ---- first-order sums (lm_first_order_sums_dev, lm_first_order_splits_dev)
     @staticmethod

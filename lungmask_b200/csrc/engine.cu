@@ -25,6 +25,7 @@
 #include "first_order.cuh"
 #include "wavelet.cuh"
 #include "filters.cuh"
+#include "mesh.cuh"
 
 using namespace lm;
 
@@ -205,6 +206,7 @@ struct lm_engine {
   FirstOrderWork first_order;   // lm_first_order_sums_dev, lm_first_order_splits_dev: row table, histograms, sums
   WaveletWork wavelet;          // lm_wavelet_dev: the non-finite flag
   FilterWork filters;           // lm_image_range_dev, lm_image_filter_dev, lm_gradient_dev: a flag, the range partials
+  MeshWork mesh;                // lm_mesh_counts_dev, lm_mesh_emit_dev: the triangle table, per-line counts and offsets
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -934,6 +936,7 @@ void lm_destroy(lm_engine* e) {
   e->first_order.release();
   e->wavelet.release();
   e->filters.release();
+  e->mesh.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1325,6 +1328,75 @@ int lm_max_diameters_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, in
   RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}}));
   RC(max_diameters(e->shape, d_mask, n0, n1, n2, row, spacing, d2, e->num_sms, e->st, &e->launches));
   return 0;
+}
+
+// The arguments the two mesh calls share: the shape and row as the shape calls, and the triangle table (see
+// lm_mesh_counts_dev): offsets non-decreasing from 0, at most kMeshMaxTriangles per configuration, and every code an edge
+// from corner a along axis m that crosses in its configuration.
+static int check_mesh_args(const char* fn, int n0, int n1, int n2, int row, const int32_t* off, const uint8_t* codes) {
+  RC(check_shape_volume(fn, n0, n1, n2));
+  if (row < 1 || row > 256) return fail(-1, "%s: row %d not in [1,256]", fn, row);
+  if (off[0] != 0) return fail(-1, "%s: tri_offsets[0] = %d, expected 0", fn, off[0]);
+  for (int c = 0; c < kMeshConfigs; ++c) {
+    const int nt = off[c + 1] - off[c];
+    if (nt < 0 || nt > kMeshMaxTriangles)
+      return fail(-1, "%s: configuration %d has %d triangles, the table allows 0..%d", fn, c, nt, kMeshMaxTriangles);
+    if ((c == 0 || c == kMeshConfigs - 1) && nt) return fail(-1, "%s: configuration %d cannot have triangles", fn, c);
+    for (int i = 3 * off[c]; i < 3 * off[c + 1]; ++i) {
+      const int a = codes[i] >> 2, m = codes[i] & 3;
+      if (a > 7 || m > 2 || (a & (4 >> m)))
+        return fail(-1, "%s: configuration %d: code %d is not an edge (corner << 2 | axis)", fn, c, codes[i]);
+      if (((c >> a) & 1) == ((c >> (a | (4 >> m))) & 1))
+        return fail(-1, "%s: configuration %d: the edge of code %d does not cross", fn, c, codes[i]);
+    }
+  }
+  return 0;
+}
+
+int lm_mesh_counts_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const int32_t* tri_offsets,
+                       const uint8_t* tri_codes, int64_t* n_vertices, int64_t* n_triangles, void* stream) {
+  static const char* fn = "lm_mesh_counts_dev";
+  if (!e || !d_mask || !tri_offsets || !tri_codes || !n_vertices || !n_triangles) return fail(-1, "%s: NULL argument", fn);
+  RC(check_mesh_args(fn, n0, n1, n2, row, tri_offsets, tri_codes));
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}}));
+  RC(mesh_counts(e->mesh, d_mask, n0, n1, n2, row, MeshTable{tri_offsets, tri_codes}, n_vertices, n_triangles, e->num_sms,
+                 e->st, &e->launches));
+  return 0;
+}
+
+int lm_mesh_emit_dev(lm_engine* e, const uint8_t* d_mask, int n0, int n1, int n2, int row, const int32_t* tri_offsets,
+                     const uint8_t* tri_codes, const double* geometry, int flags, int64_t n_vertices, int64_t n_triangles,
+                     int32_t* d_index2, double* d_vertices, int32_t* d_triangles, void* stream) {
+  static const char* fn = "lm_mesh_emit_dev";
+  if (!e || !d_mask || !tri_offsets || !tri_codes || !geometry) return fail(-1, "%s: NULL argument", fn);
+  RC(check_mesh_args(fn, n0, n1, n2, row, tri_offsets, tri_codes));
+  if (flags & ~LM_MESH_RAS) return fail(-1, "%s: unknown flags 0x%x", fn, flags);
+  if (n_vertices < 0 || n_vertices > INT32_MAX || n_triangles < 0 || n_triangles > INT32_MAX)
+    return fail(-1, "%s: %lld vertices / %lld triangles, int32 indices take at most 2^31 - 1", fn, (long long)n_vertices,
+                (long long)n_triangles);
+  if ((n_vertices && (!d_index2 || !d_vertices)) || (n_triangles && !d_triangles)) return fail(-1, "%s: NULL output", fn);
+  MeshPlacement P{};
+  for (int k = 0; k < 15; ++k)
+    if (!isfinite(geometry[k])) return fail(-1, "%s: geometry[%d] = %g is not finite", fn, k, geometry[k]);
+  for (int k = 0; k < 3; ++k) {
+    P.o[k] = geometry[k];
+    P.s[k] = geometry[12 + k];
+    if (!(P.s[k] > 0.0)) return fail(-1, "%s: spacing %g along %c is not positive", fn, P.s[k], "xyz"[k]);
+  }
+  for (int k = 0; k < 9; ++k) P.d[k] = geometry[3 + k];
+  const double* D = P.d;
+  const double det = D[0] * (D[4] * D[8] - D[5] * D[7]) - D[1] * (D[3] * D[8] - D[5] * D[6]) + D[2] * (D[3] * D[7] - D[4] * D[6]);
+  if (det == 0.0) return fail(-1, "%s: the direction matrix is singular", fn);
+  P.ras = flags & LM_MESH_RAS;
+  P.reverse = det < 0.0;
+  const size_t nv = (size_t)n_vertices, nt = (size_t)n_triangles;
+  RC(analysis_inputs(e, fn, stream, {{"d_mask", d_mask}, {"d_index2", nv ? d_index2 : nullptr},
+                                     {"d_vertices", nv ? d_vertices : nullptr}, {"d_triangles", nt ? d_triangles : nullptr}}));
+  const int rc = mesh_emit(e->mesh, d_mask, n0, n1, n2, row, MeshTable{tri_offsets, tri_codes}, P, n_vertices, n_triangles,
+                           d_index2, d_vertices, d_triangles, e->num_sms, e->st, &e->launches);
+  if (rc == -2) return fail(-1, "%s: n_vertices / n_triangles (%lld / %lld) are not the row's counts", fn,
+                            (long long)n_vertices, (long long)n_triangles);
+  return rc;
 }
 
 // The row arguments the two first-order calls share: modes, the band and the exact rows' base; `pass` 0 (sums) also

@@ -585,3 +585,50 @@ def save_filtered_features(path, features):
         lines.append(",".join(_csv_cell(c) for c in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")
+
+
+MESH_FORMATS = ("stl", "obj", "ply")
+
+
+def mesh_format(path):
+    """The format save_mesh writes to `path` (from its extension); refuses, before any work is done, one it cannot."""
+    ext = os.path.splitext(path)[1].lower().lstrip(".")
+    if ext not in MESH_FORMATS:
+        raise SystemExit("unsupported mesh output format (use .stl, .obj or .ply): %s" % path)
+    return ext
+
+
+def save_mesh(path, mesh):
+    """Writes one lungmask_b200.mesh.Mesh of LMInferer.mesh (numpy or CUDA arrays), the format following the extension:
+    .stl binary STL (float32 positions, each triangle's unit normal from its float64 positions, a zero normal for a
+    degenerate triangle), .obj ASCII Wavefront (positions as %.17g, 1-based faces) or .ply binary little-endian PLY
+    (float64 positions, int32 faces)."""
+    fmt = mesh_format(path)
+    m = mesh.numpy()
+    V = np.ascontiguousarray(m.vertices, dtype=np.float64).reshape(-1, 3)
+    T = np.ascontiguousarray(m.triangles, dtype=np.int32).reshape(-1, 3)
+    if fmt == "stl":
+        a, b, c = V[T[:, 0]], V[T[:, 1]], V[T[:, 2]]
+        n = np.cross(b - a, c - a)
+        length = np.sqrt(np.einsum("ij,ij->i", n, n))
+        n = np.divide(n, length[:, None], out=np.zeros_like(n), where=length[:, None] > 0)
+        rec = np.zeros(len(T), np.dtype([("n", "<f4", 3), ("v", "<f4", (3, 3)), ("attr", "<u2")]))
+        rec["n"] = n
+        rec["v"] = np.stack([a, b, c], axis=1)
+        header = ("lungmask_b200 mesh %s (%s)" % (m.name, m.space)).encode("ascii", "replace")[:80].ljust(80, b" ")
+        with open(path, "wb") as f:
+            f.write(header + struct.pack("<I", len(T)) + rec.tobytes())
+    elif fmt == "obj":
+        with open(path, "w") as f:
+            f.write("# lungmask_b200 mesh %s (%s)\n" % (m.name, m.space))
+            np.savetxt(f, V, fmt="v %.17g %.17g %.17g")
+            np.savetxt(f, T.astype(np.int64) + 1, fmt="f %d %d %d")
+    else:
+        header = ("ply\nformat binary_little_endian 1.0\ncomment lungmask_b200 mesh %s (%s)\nelement vertex %d\n"
+                  "property double x\nproperty double y\nproperty double z\nelement face %d\n"
+                  "property list uchar int vertex_indices\nend_header\n") % (m.name, m.space, len(V), len(T))
+        faces = np.zeros(len(T), np.dtype([("n", "u1"), ("i", "<i4", 3)]))
+        faces["n"] = 3
+        faces["i"] = T
+        with open(path, "wb") as f:
+            f.write(header.encode("ascii", "replace") + V.astype("<f8").tobytes() + faces.tobytes())

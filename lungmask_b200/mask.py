@@ -660,6 +660,51 @@ class LMInferer:
                                     geometry))
         return sh.ShapeFeatures(spacing, out)
 
+    def mesh(self, mask, spacing=None, image=None, rows=None, space="lps"):
+        """The marching-cubes surface of every row of `shape` -> lungmask_b200.mesh.MeshSet: every label value in the mask
+        and every label 1..K-1 of the model (absent ones as empty meshes), then "lung" (mask != 0); or the rows named by
+        `rows` (label values and / or "lung"), in that order.  Each is the mesh whose area and volume `shape` reports
+        (DESIGN §4.14): vertices at cube-edge midpoints of the mask padded with one voxel of outside, triangles from
+        shape.triangle_table(), closed and with normals pointing out of the row; not smoothed or decimated.
+
+        Each Mesh holds `vertices` (float64 (V, 3), mm), `index2` (int32 (V, 3), the exact doubled array-axis coordinates)
+        and `triangles` (int32 (T, 3)).  The positions are placed with the origin, direction and spacing of `image` (a
+        Volume or SimpleITK image; `spacing` overrides its spacing), or with `spacing` (x, y, z) alone (origin 0, identity
+        direction).  `space` "lps" (the frame of Volume and SimpleITK) or "ras" (the first two components negated).
+        `mask`: (S, H, W) uint8 or bool, numpy or a CPU tensor (numpy arrays back), or a CUDA tensor on the engine's device
+        read in place after the work queued on the current stream (tensors on that device back, with no host copy).  Bad
+        spacing, rows, space or direction raise a ValueError before any kernel runs."""
+        import torch
+        from . import mesh as me
+        from .statistics import label_name
+        spacing, origin, direction = me.geometry(spacing, image)
+        space = me.check_space(space)
+        want = None if rows is None else me.check_rows(rows)
+        s = self._stage("mesh", None, mask, mask_only=True)
+        on_device = _is_tensor(mask) and mask.is_cuda
+        shape, dev = tuple(s.mask.shape), s.mask.device
+        present = self._mask_labels(s.mask, s.stream)
+        order = want if want is not None else sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]
+        geo = me.geometry_vector(spacing, origin, direction)
+        out = []
+        for r in order:
+            label = me.UNION if r == 256 else r
+            nv = nt = 0
+            if r in present or r == 256 and present:
+                nv, nt = self.engine.mesh_counts_dev(s.mask.data_ptr(), shape, r, me.TABLE_OFFSETS, me.TABLE_CODES,
+                                                     stream=s.stream)
+                me.check_counts(label, nv, nt)
+            index2 = torch.empty((nv, 3), dtype=torch.int32, device=dev)
+            verts = torch.empty((nv, 3), dtype=torch.float64, device=dev)
+            tris = torch.empty((nt, 3), dtype=torch.int32, device=dev)
+            if nv or nt:
+                self.engine.mesh_emit_dev(s.mask.data_ptr(), shape, r, me.TABLE_OFFSETS, me.TABLE_CODES, geo, nv, nt,
+                                          index2.data_ptr(), verts.data_ptr(), tris.data_ptr(), ras=space == "ras",
+                                          stream=s.stream)
+            m = me.Mesh(label, me.UNION if r == 256 else label_name(self.modelname, r), verts, index2, tris, space)
+            out.append(m if on_device else m.numpy())
+        return me.MeshSet(spacing, origin, direction, space, out)
+
     def _mask_labels(self, mask, stream):
         """The non-zero label values of a (S,H,W) uint8 CUDA mask tensor.  lm_label_stats_dev with the mask as its own uint8
         volume and no percentiles or thresholds: its count and histogram passes over the mask bytes."""
