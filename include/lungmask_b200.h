@@ -403,6 +403,29 @@ LM_API int lm_image_filter_dev(lm_engine* e, const void* d_vol, int dtype, int n
 LM_API int lm_gradient_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, const double* spacing_xyz,
                            double* d_out, void* stream);
 
+/* Voxel-based first-order feature maps (no counterpart in the reference; DESIGN §4.15): PyRadiomics' voxel-based
+ * firstorder extraction of one row, for LMInferer.first_order_maps.  Device memory of the engine's device and the
+ * caller's cudaStream_t with the event-wait rule of lm_apply_dev; every argument is checked before any kernel runs and
+ * the call returns after the engine's stream has synchronised.  d_vol (n0,n1,n2) of any LM_DTYPE_* code and d_mask
+ * (n0,n1,n2) uint8, fewer than 2^32 voxels, never written.  row 1..255 (mask == row) or 256 (mask > 0); the ROI is the
+ * row's voxels with a non-NaN value.  radius 1..3: the window of voxel c is the (2 radius + 1)^3 cube about c clipped at
+ * the array border; its candidates are the window's ROI voxels (masked 1) or its non-NaN voxels (masked 0).
+ * bin_width >= 1, low and n_levels (1..255) the fixed-bin-width discretisation of the host's region; mode
+ * LM_FOM_FLOAT, or LM_FOM_EXACT (integer dtypes; every candidate within [base, base + 2^20), |base| <= 2^53);
+ * shift: voxelArrayShift, |shift| < 2^58 and, exact, |base + shift| < 2^58.  voxel_volume: the TotalEnergy factor
+ * (NaN for none).  feature_bits: a non-empty subset of the 18 bits LM_FOM_* (bit k = first_order.FIRST_ORDER_FEATURES[k]).
+ * d_entropy_table: device float64, table_len = K (K + 1) / 2 with K = (2 radius + 1)^3 (see first_order_maps.
+ * entropy_table).  d_out: popcount(feature_bits) float64 (n0,n1,n2) planes in bit order, not overlapping the inputs:
+ * ROI voxels get their window's features in the sequence of DESIGN §4.15, every other voxel init_value.  A +-inf
+ * candidate returns LM_ERR_NONFINITE.  Work area: one flag; each thread holds its window in local memory. */
+#define LM_FOM_FLOAT 1
+#define LM_FOM_EXACT 2
+LM_API int lm_first_order_maps_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                                   int row, int radius, int masked, int bin_width, int64_t low, int n_levels, int mode,
+                                   int64_t base, int64_t shift, double voxel_volume, double init_value,
+                                   uint32_t feature_bits, const double* d_entropy_table, int64_t table_len, double* d_out,
+                                   void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -16,14 +16,15 @@ deviations, energy, entropy, uniformity) of every label and the whole lung (.jso
 LMInferer.wavelet_features), and `--filtered PATH` those of the Square, SquareRoot, Logarithm, Exponential and Gradient
 image types (.json / .csv, LMInferer.filtered_features), and `--mesh DIR` the marching-cubes surface of every present
 label and of the whole lung, one file per row (`--mesh-format` stl, obj or ply, `--mesh-space` lps or ras;
-LMInferer.mesh with the input's geometry).
+LMInferer.mesh with the input's geometry), and `--first-order-maps DIR` the voxel-based first-order feature maps of one
+row, one image per feature with the input's geometry (LMInferer.first_order_maps).
 """
 import argparse
 import os
 import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_first_order, save_mask,
-                 save_mesh, save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
+                 save_feature_maps, save_mesh, save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
                  save_filtered_features, save_wavelet_features)
 from .logger import logger
 from .mask import LMInferer
@@ -122,7 +123,49 @@ def build_parser():
                    help="File format of --mesh: binary STL (default), ASCII OBJ or binary PLY")
     p.add_argument("--mesh-space", choices=["lps", "ras"], default="lps",
                    help="Frame of the --mesh positions: LPS (DICOM / ITK, default) or RAS (3D Slicer, NIfTI)")
+    p.add_argument("--first-order-maps", metavar="DIR", type=str, default=None,
+                   help="Also write voxel-based first-order feature maps (PyRadiomics' voxelBased extraction) of one row "
+                        "to DIR, one float64 image per feature named <row>_<Feature> (lung_Entropy.nii.gz); uses "
+                        "--first-order-bin-width and --first-order-shift")
+    p.add_argument("--first-order-maps-radius", type=int, choices=[1, 2, 3], default=1,
+                   help="Kernel radius of --first-order-maps: the window is the (2r+1)^3 cube about each voxel (default 1)")
+    p.add_argument("--first-order-maps-features", metavar="NAMES", type=str, default=None,
+                   help="Comma-separated features of --first-order-maps, PyRadiomics names such as Mean,Entropy "
+                        "(default all 18)")
+    p.add_argument("--first-order-maps-label", metavar="ROW", type=str, default="lung",
+                   help='Row of --first-order-maps: "lung" (every label, default) or one label value 1..255')
+    p.add_argument("--first-order-maps-unmasked", action="store_true",
+                   help="Windows of --first-order-maps take every non-NaN voxel, not only the row's (PyRadiomics' "
+                        "maskedKernel=False)")
+    p.add_argument("--first-order-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
+                   help="File format of --first-order-maps (default nii.gz)")
     return p
+
+
+def first_order_maps_arguments(args):
+    """-> (label, features) of --first-order-maps; exits with a message naming the flag for a bad value."""
+    from . import first_order_maps as fm
+    from .texture import check_arguments as check_bin_width
+    if os.path.exists(args.first_order_maps) and not os.path.isdir(args.first_order_maps):
+        sys.exit("--first-order-maps: %s exists and is not a directory" % args.first_order_maps)
+    if not os.path.isdir(os.path.dirname(os.path.abspath(args.first_order_maps))):
+        sys.exit("--first-order-maps: the parent directory of %s does not exist" % args.first_order_maps)
+    try:
+        check_bin_width(args.first_order_bin_width)
+    except ValueError as ex:
+        sys.exit("--first-order-bin-width: %s" % ex)
+    label = args.first_order_maps_label.strip()
+    try:
+        label = fm.check_label(label if label == "lung" else int(label))
+    except ValueError as ex:
+        sys.exit("--first-order-maps-label: %s" % ex)
+    features = None
+    if args.first_order_maps_features is not None:
+        try:
+            features = fm.check_features([c.strip() for c in args.first_order_maps_features.split(",") if c.strip()])
+        except ValueError as ex:
+            sys.exit("--first-order-maps-features: %s" % ex)
+    return label, features
 
 
 def mesh_file_name(mesh, fmt):
@@ -202,6 +245,8 @@ def main(argv=None):
         parent = os.path.dirname(os.path.abspath(args.mesh))
         if not os.path.isdir(parent):
             sys.exit("--mesh: the parent directory of %s does not exist" % args.mesh)
+    if args.first_order_maps is not None:
+        maps_label, maps_features = first_order_maps_arguments(args)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -259,6 +304,16 @@ def main(argv=None):
         for m in inferer.mesh(result, image=image, space=args.mesh_space):
             if m.n_triangles or m.label == "lung":
                 save_mesh(os.path.join(args.mesh, mesh_file_name(m, args.mesh_format)), m)
+
+    if args.first_order_maps is not None:
+        logger.info(f"Save first-order maps to: {args.first_order_maps}")
+        save_feature_maps(args.first_order_maps,
+                          inferer.first_order_maps(image, result, label=maps_label, features=maps_features,
+                                                   kernel_radius=args.first_order_maps_radius,
+                                                   masked_kernel=not args.first_order_maps_unmasked,
+                                                   bin_width=args.first_order_bin_width,
+                                                   voxel_array_shift=args.first_order_shift),
+                          image, args.first_order_maps_format)
 
 
 if __name__ == "__main__":

@@ -26,6 +26,7 @@
 #include "wavelet.cuh"
 #include "filters.cuh"
 #include "mesh.cuh"
+#include "first_order_maps.cuh"
 
 using namespace lm;
 
@@ -207,6 +208,7 @@ struct lm_engine {
   WaveletWork wavelet;          // lm_wavelet_dev: the non-finite flag
   FilterWork filters;           // lm_image_range_dev, lm_image_filter_dev, lm_gradient_dev: a flag, the range partials
   MeshWork mesh;                // lm_mesh_counts_dev, lm_mesh_emit_dev: the triangle table, per-line counts and offsets
+  FomWork fo_maps;              // lm_first_order_maps_dev: the error flag
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -937,6 +939,7 @@ void lm_destroy(lm_engine* e) {
   e->wavelet.release();
   e->filters.release();
   e->mesh.release();
+  e->fo_maps.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1571,6 +1574,50 @@ int lm_gradient_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, 
   if (overlaps(d_vol, n * dtype_bytes(dtype), d_out, n * sizeof(double))) return fail(-1, "%s: d_out overlaps d_vol", fn);
   RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_out", d_out}}));
   return filter_result(fn, gradient_magnitude(e->filters, d_vol, dtype, n0, n1, n2, inv, d_out, e->st, &e->launches));
+}
+
+int lm_first_order_maps_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,
+                            int row, int radius, int masked, int bin_width, int64_t low, int n_levels, int mode,
+                            int64_t base, int64_t shift, double voxel_volume, double init_value, uint32_t feature_bits,
+                            const double* d_entropy_table, int64_t table_len, double* d_out, void* stream) {
+  static const char* fn = "lm_first_order_maps_dev";
+  if (!e || !d_vol || !d_mask || !d_entropy_table || !d_out) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (dtype < LM_DTYPE_I16 || dtype > LM_DTYPE_BF16) return fail(-1, "%s: unknown dtype code %d", fn, dtype);
+  if (row < 1 || row > 256) return fail(-1, "%s: row %d not in [1,256]", fn, row);
+  if (radius < 1 || radius > kFomMaxRadius) return fail(-1, "%s: radius %d not in [1,%d]", fn, radius, kFomMaxRadius);
+  if (masked != 0 && masked != 1) return fail(-1, "%s: masked %d is not 0 or 1", fn, masked);
+  if (bin_width < 1) return fail(-1, "%s: bin_width %d is not positive", fn, bin_width);
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  const bool integer = dtype == LM_DTYPE_U8 || dtype == LM_DTYPE_I8 || dtype == LM_DTYPE_I16 || dtype == LM_DTYPE_I32 ||
+                       dtype == LM_DTYPE_I64;
+  if (mode != LM_FOM_FLOAT && mode != LM_FOM_EXACT) return fail(-1, "%s: mode %d is not LM_FOM_FLOAT or LM_FOM_EXACT", fn, mode);
+  if (mode == LM_FOM_EXACT && !integer) return fail(-1, "%s: the exact mode needs an integer volume (dtype %d)", fn, dtype);
+  const int64_t lim53 = (int64_t)1 << 53, lim58 = (int64_t)1 << 58, lim62 = (int64_t)1 << 62;
+  if (mode == LM_FOM_EXACT && (base < -lim53 || base > lim53)) return fail(-1, "%s: base %lld beyond 2^53", fn, (long long)base);
+  if (low <= -lim62 || low >= lim62) return fail(-1, "%s: low %lld beyond 2^62", fn, (long long)low);
+  if (shift <= -lim58 || shift >= lim58 || (mode == LM_FOM_EXACT && (base + shift <= -lim58 || base + shift >= lim58)))
+    return fail(-1, "%s: shift %lld: |shift| and |base + shift| must stay below 2^58", fn, (long long)shift);
+  if (!(isnan(voxel_volume) || (isfinite(voxel_volume) && voxel_volume > 0.0)))
+    return fail(-1, "%s: voxel_volume %g is neither NaN nor finite and positive", fn, voxel_volume);
+  if (feature_bits == 0 || (feature_bits >> kFomFeatures))
+    return fail(-1, "%s: feature_bits 0x%x: set one or more of the %d feature bits and no other", fn, feature_bits, kFomFeatures);
+  const int64_t K = (int64_t)(2 * radius + 1) * (2 * radius + 1) * (2 * radius + 1);
+  if (table_len != K * (K + 1) / 2)
+    return fail(-1, "%s: table_len %lld, radius %d needs %lld", fn, (long long)table_len, radius, (long long)(K * (K + 1) / 2));
+  const size_t n = (size_t)n0 * n1 * n2, out_bytes = (size_t)__builtin_popcount(feature_bits) * n * sizeof(double);
+  if (overlaps(d_vol, n * dtype_bytes(dtype), d_out, out_bytes)) return fail(-1, "%s: d_out overlaps d_vol", fn);
+  if (overlaps(d_mask, n, d_out, out_bytes)) return fail(-1, "%s: d_out overlaps d_mask", fn);
+  if (overlaps(d_entropy_table, (size_t)table_len * sizeof(double), d_out, out_bytes))
+    return fail(-1, "%s: d_out overlaps d_entropy_table", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_mask", d_mask}, {"d_entropy_table", d_entropy_table},
+                                     {"d_out", d_out}}));
+  const FomArgs a{row, radius, masked, bin_width, n_levels, mode == LM_FOM_EXACT, (long long)low, (long long)base,
+                  (long long)shift, voxel_volume, init_value, feature_bits, d_entropy_table};
+  const int rc = first_order_maps(e->fo_maps, d_vol, dtype, d_mask, n0, n1, n2, a, d_out, e->num_sms, e->st, &e->launches);
+  if (rc == LM_ERR_NONFINITE) return fail(rc, "%s: a window holds a +-inf value", fn);
+  if (rc == kFomRange) return fail(rc, "%s: a value outside the exact span or a level outside 1..%d", fn, n_levels);
+  return rc;
 }
 
 int lm_shard_init(lm_engine* e, int rank, int world, int max_slices) {

@@ -632,3 +632,26 @@ def save_mesh(path, mesh):
         faces["i"] = T
         with open(path, "wb") as f:
             f.write(header.encode("ascii", "replace") + V.astype("<f8").tobytes() + faces.tobytes())
+
+
+FEATURE_MAP_FORMATS = ("nii.gz", "nii", "mha", "npy")
+
+
+def feature_map_file(label, feature, fmt):
+    """The file name of one map of LMInferer.first_order_maps: <row name>_<Feature>.<ext> (lung_Entropy.nii.gz)."""
+    return "%s_%s.%s" % (str(label).replace(" ", "_"), feature, fmt)
+
+
+def save_feature_maps(directory, maps, like=None, fmt="nii.gz"):
+    """Writes every map of a lungmask_b200.first_order_maps.FirstOrderMaps (numpy or CUDA) to `directory` (created when
+    missing) as float64 images with the geometry of `like` (a Volume, or None for unit spacing), one file per feature
+    named by feature_map_file.  -> the paths written."""
+    if fmt not in FEATURE_MAP_FORMATS:
+        raise ValueError("feature map format %r is not one of %s" % (fmt, ", ".join(FEATURE_MAP_FORMATS)))
+    os.makedirs(directory, exist_ok=True)
+    paths = []
+    for feature, m in maps.numpy().maps.items():
+        path = os.path.join(directory, feature_map_file(maps.label, feature, fmt))
+        save_mask(path, np.ascontiguousarray(m, dtype=np.float64), like)
+        paths.append(path)
+    return paths

@@ -621,6 +621,67 @@ class LMInferer:
             out.append(fo.build_row(r, names[r], bw, p, a["histogram"][r][1:], ps, nb, sb, splits, s.spacing, shift))
         return fo.FirstOrderFeatures(s.spacing, bw, shift, out)
 
+    def first_order_maps(self, image, mask, label="lung", features=None, kernel_radius=1, masked_kernel=True, bin_width=25,
+                         voxel_array_shift=0, init_value=0.0, spacing=None):
+        """PyRadiomics' voxel-based first-order extraction of one row -> lungmask_b200.first_order_maps.FirstOrderMaps:
+        one float64 map of the volume's shape per feature of first_order.FIRST_ORDER_FEATURES (or of `features`, a
+        subset, in that order), indexed by name (`fm["Entropy"]`).  `label`: a label value 1..255 or "lung" (mask > 0);
+        the ROI is the row's voxels with a non-NaN value.  Each ROI voxel gets the features of the candidates of its
+        window, the (2 kernel_radius + 1)^3 cube about it clipped at the array border (kernel_radius 1, 2 or 3): the
+        window's ROI voxels (masked_kernel) or its non-NaN voxels.  Every other voxel holds `init_value`.  The levels of
+        Entropy and Uniformity come from the fixed `bin_width` discretisation of the ROI (masked) or of the non-NaN voxels
+        of its bounding box padded by kernel_radius (unmasked); more than 255 levels or a +-inf there is a ValueError
+        before any map kernel runs.  The features and `voxel_array_shift`, `spacing` are those of `first_order`, formed
+        per window in the sequence of DESIGN §4.15 (bit-identical to first_order_maps.maps_host).
+
+        `image`, `mask` and `spacing` as for `first_order`.  CUDA inputs give CUDA float64 tensors on their device with no
+        host copy, CPU tensors CPU tensors and everything else numpy arrays.  Each map takes 8 bytes per voxel (629 MB at
+        300 x 512 x 512, 11.3 GB for all 18), allocated for the requested features only."""
+        import torch
+        from . import first_order as fo
+        from . import first_order_maps as fm
+        from . import texture as tx
+        row = fm.check_label(label)
+        feats = fm.check_features(features)
+        r = fm.check_radius(kernel_radius)
+        bw = tx.check_arguments(bin_width)
+        shift = fo.check_shift(voxel_array_shift)
+        s = self._stage("first_order_maps", image, mask, spacing)
+        shape = tuple(s.mask.shape)
+        code = 256 if row == fm.UNION else row
+        integer = s.dtype in (_native.DTYPE_U8, _native.DTYPE_I8, _native.DTYPE_I16, _native.DTYPE_I32, _native.DTYPE_I64)
+        st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, (), (), stream=s.stream)
+        n_roi = int(st["voxels"][code] - st["nan_voxels"][code])
+        d_row, region = code, s.mask
+        if n_roi and not masked_kernel:   # D: the non-NaN voxels of the ROI's bounding box padded by r
+            roi = s.mask > 0 if code == 256 else s.mask == code
+            if not integer:
+                roi &= ~torch.isnan(s.vol)
+            box = []
+            for ax in range(3):
+                idx = torch.nonzero(roi.any(dim=[a for a in range(3) if a != ax])).reshape(-1)
+                box.append(slice(max(int(idx[0]) - r, 0), int(idx[-1]) + r + 1))
+            region = torch.zeros_like(s.mask)
+            region[tuple(box)] = 1
+            d_row = 1
+            st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, region.data_ptr(), shape, (), (), stream=s.stream)
+        n_d = int(st["voxels"][d_row] - st["nan_voxels"][d_row])
+        plan = fm.plan_maps(n_d, float(st["moments"][d_row][2]), float(st["moments"][d_row][3]), bw, integer, shift, n_roi,
+                            "first_order_maps: row %s" % label)
+        del region
+        vv = float("nan") if s.spacing is None else (s.spacing[0] * s.spacing[1]) * s.spacing[2]
+        K = (2 * r + 1) ** 3
+        table = torch.from_numpy(fm.entropy_table(K)).to(s.mask.device)
+        out = torch.empty((len(feats),) + shape, dtype=torch.float64, device=s.mask.device)
+        # an empty ROI: the kernel writes init_value everywhere (no voxel reads the discretisation)
+        self.engine.first_order_maps_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, code, r, masked_kernel, bw,
+                                         plan.low or 0, plan.n_levels or 1, plan.exact, plan.base, shift, vv,
+                                         float(init_value), fm.feature_bits(feats), table.data_ptr(), table.numel(),
+                                         out.data_ptr(), stream=s.stream)
+        maps = collections.OrderedDict((f, s.back(out[j])) for j, f in enumerate(feats))
+        return fm.FirstOrderMaps(row, r, bool(masked_kernel), bw, shift, float(init_value), plan.low, plan.n_levels,
+                                 plan.exact, n_roi, s.spacing, maps)
+
     def shape(self, mask, spacing=None, image=None):
         """Mesh shape features of every row of `statistics` -> lungmask_b200.shape.ShapeFeatures: every label value in the
         mask and every label 1..K-1 of the model (absent ones with 0 voxels and NaN features), then "lung" (mask != 0).
