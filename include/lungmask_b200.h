@@ -426,6 +426,23 @@ LM_API int lm_first_order_maps_dev(lm_engine* e, const void* d_vol, int dtype, c
                                    uint32_t feature_bits, const double* d_entropy_table, int64_t table_len, double* d_out,
                                    void* stream);
 
+/* Voxel-based GLCM feature maps (no counterpart in the reference; DESIGN §4.16): PyRadiomics' voxel-based glcm extraction
+ * of one row, for LMInferer.glcm_maps.  Device memory of the engine's device and the caller's cudaStream_t with the
+ * event-wait rule of lm_apply_dev; every argument is checked before any kernel runs and the call returns after the
+ * engine's stream has synchronised.  d_levels (n0,n1,n2) uint8, the level map of lm_texture_levels_dev over the
+ * discretisation region (0 outside it), and d_mask (n0,n1,n2) uint8, fewer than 2^32 voxels, never written.  A voxel is
+ * a candidate when its level is not 0, and a centre when it is a candidate with mask == row (row 1..255) or mask > 0
+ * (row 256).  radius 1..3: the window of a centre is the (2 radius + 1)^3 cube about it clipped at the array border.
+ * n_levels 1..255 (Ng of Idmn and Idn); a level above it returns an error and no map.  feature_bits: a non-empty subset
+ * of the 22 bits, bit k = texture.GLCM_FEATURES[k].  d_entropy_table: device float64, table_len = M (M + 1) / 2 with
+ * M = 2 (2 radius + 1)^2 (2 radius) (see first_order_maps.entropy_table).  d_out: popcount(feature_bits) float64
+ * (n0,n1,n2) planes in bit order, not overlapping the inputs: centres get their window's features in the sequence of
+ * DESIGN §4.16 (NaN without a pair in any direction), every other voxel init_value.  Work area: one flag; each thread
+ * holds its window, pair keys and count tables in local memory. */
+LM_API int lm_glcm_maps_dev(lm_engine* e, const uint8_t* d_levels, const uint8_t* d_mask, int n0, int n1, int n2, int row,
+                            int radius, int n_levels, double init_value, uint32_t feature_bits,
+                            const double* d_entropy_table, int64_t table_len, double* d_out, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

@@ -17,7 +17,8 @@ LMInferer.wavelet_features), and `--filtered PATH` those of the Square, SquareRo
 image types (.json / .csv, LMInferer.filtered_features), and `--mesh DIR` the marching-cubes surface of every present
 label and of the whole lung, one file per row (`--mesh-format` stl, obj or ply, `--mesh-space` lps or ras;
 LMInferer.mesh with the input's geometry), and `--first-order-maps DIR` the voxel-based first-order feature maps of one
-row, one image per feature with the input's geometry (LMInferer.first_order_maps).
+row, one image per feature with the input's geometry (LMInferer.first_order_maps), and `--glcm-maps DIR` its voxel-based
+GLCM feature maps the same way (LMInferer.glcm_maps).
 """
 import argparse
 import os
@@ -139,6 +140,22 @@ def build_parser():
                         "maskedKernel=False)")
     p.add_argument("--first-order-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
                    help="File format of --first-order-maps (default nii.gz)")
+    p.add_argument("--glcm-maps", metavar="DIR", type=str, default=None,
+                   help="Also write voxel-based GLCM feature maps (PyRadiomics' voxelBased extraction) of one row to DIR, "
+                        "one float64 image per feature named <row>_glcm_<Feature> (lung_glcm_Contrast.nii.gz); uses "
+                        "--texture-bin-width")
+    p.add_argument("--glcm-maps-radius", type=int, choices=[1, 2, 3], default=1,
+                   help="Kernel radius of --glcm-maps: the window is the (2r+1)^3 cube about each voxel (default 1)")
+    p.add_argument("--glcm-maps-features", metavar="NAMES", type=str, default=None,
+                   help="Comma-separated features of --glcm-maps, PyRadiomics names such as Contrast,JointEntropy,Idm "
+                        "(default all 22)")
+    p.add_argument("--glcm-maps-label", metavar="ROW", type=str, default="lung",
+                   help='Row of --glcm-maps: "lung" (every label, default) or one label value 1..255')
+    p.add_argument("--glcm-maps-unmasked", action="store_true",
+                   help="Windows of --glcm-maps take every non-NaN voxel, not only the row's (PyRadiomics' "
+                        "maskedKernel=False)")
+    p.add_argument("--glcm-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
+                   help="File format of --glcm-maps (default nii.gz)")
     return p
 
 
@@ -165,6 +182,33 @@ def first_order_maps_arguments(args):
             features = fm.check_features([c.strip() for c in args.first_order_maps_features.split(",") if c.strip()])
         except ValueError as ex:
             sys.exit("--first-order-maps-features: %s" % ex)
+    return label, features
+
+
+def glcm_maps_arguments(args):
+    """-> (label, features) of --glcm-maps; exits with a message naming the flag for a bad value."""
+    from . import first_order_maps as fm
+    from . import glcm_maps as gm
+    from .texture import check_arguments as check_bin_width
+    if os.path.exists(args.glcm_maps) and not os.path.isdir(args.glcm_maps):
+        sys.exit("--glcm-maps: %s exists and is not a directory" % args.glcm_maps)
+    if not os.path.isdir(os.path.dirname(os.path.abspath(args.glcm_maps))):
+        sys.exit("--glcm-maps: the parent directory of %s does not exist" % args.glcm_maps)
+    try:
+        check_bin_width(args.texture_bin_width)
+    except (TypeError, ValueError) as ex:
+        sys.exit("--texture-bin-width: %s" % ex)
+    label = args.glcm_maps_label.strip()
+    try:
+        label = fm.check_label(label if label == "lung" else int(label))
+    except ValueError as ex:
+        sys.exit("--glcm-maps-label: %s" % ex)
+    features = None
+    if args.glcm_maps_features is not None:
+        try:
+            features = gm.check_features([c.strip() for c in args.glcm_maps_features.split(",") if c.strip()])
+        except ValueError as ex:
+            sys.exit("--glcm-maps-features: %s" % ex)
     return label, features
 
 
@@ -247,6 +291,8 @@ def main(argv=None):
             sys.exit("--mesh: the parent directory of %s does not exist" % args.mesh)
     if args.first_order_maps is not None:
         maps_label, maps_features = first_order_maps_arguments(args)
+    if args.glcm_maps is not None:
+        glcm_label, glcm_features = glcm_maps_arguments(args)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -314,6 +360,14 @@ def main(argv=None):
                                                    bin_width=args.first_order_bin_width,
                                                    voxel_array_shift=args.first_order_shift),
                           image, args.first_order_maps_format)
+
+    if args.glcm_maps is not None:
+        logger.info(f"Save GLCM maps to: {args.glcm_maps}")
+        save_feature_maps(args.glcm_maps,
+                          inferer.glcm_maps(image, result, label=glcm_label, features=glcm_features,
+                                            kernel_radius=args.glcm_maps_radius, masked_kernel=not args.glcm_maps_unmasked,
+                                            bin_width=args.texture_bin_width),
+                          image, args.glcm_maps_format)
 
 
 if __name__ == "__main__":

@@ -637,21 +637,25 @@ def save_mesh(path, mesh):
 FEATURE_MAP_FORMATS = ("nii.gz", "nii", "mha", "npy")
 
 
-def feature_map_file(label, feature, fmt):
-    """The file name of one map of LMInferer.first_order_maps: <row name>_<Feature>.<ext> (lung_Entropy.nii.gz)."""
-    return "%s_%s.%s" % (str(label).replace(" ", "_"), feature, fmt)
+def feature_map_file(label, feature, fmt, feature_class=None):
+    """The file name of one feature map: <row name>_<Feature>.<ext> for LMInferer.first_order_maps (lung_Entropy.nii.gz),
+    <row name>_<class>_<Feature>.<ext> for a texture class (lung_glcm_Contrast.nii.gz)."""
+    row = str(label).replace(" ", "_")
+    if feature_class:
+        return "%s_%s_%s.%s" % (row, feature_class, feature, fmt)
+    return "%s_%s.%s" % (row, feature, fmt)
 
 
 def save_feature_maps(directory, maps, like=None, fmt="nii.gz"):
-    """Writes every map of a lungmask_b200.first_order_maps.FirstOrderMaps (numpy or CUDA) to `directory` (created when
-    missing) as float64 images with the geometry of `like` (a Volume, or None for unit spacing), one file per feature
-    named by feature_map_file.  -> the paths written."""
+    """Writes every map of a lungmask_b200.first_order_maps.FirstOrderMaps or glcm_maps.GLCMMaps (numpy or CUDA) to
+    `directory` (created when missing) as float64 images with the geometry of `like` (a Volume, or None for unit
+    spacing), one file per feature named by feature_map_file.  -> the paths written."""
     if fmt not in FEATURE_MAP_FORMATS:
         raise ValueError("feature map format %r is not one of %s" % (fmt, ", ".join(FEATURE_MAP_FORMATS)))
     os.makedirs(directory, exist_ok=True)
     paths = []
     for feature, m in maps.numpy().maps.items():
-        path = os.path.join(directory, feature_map_file(maps.label, feature, fmt))
+        path = os.path.join(directory, feature_map_file(maps.label, feature, fmt, getattr(maps, "FEATURE_CLASS", None)))
         save_mask(path, np.ascontiguousarray(m, dtype=np.float64), like)
         paths.append(path)
     return paths

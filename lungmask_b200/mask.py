@@ -650,6 +650,29 @@ class LMInferer:
         shape = tuple(s.mask.shape)
         code = 256 if row == fm.UNION else row
         integer = s.dtype in (_native.DTYPE_U8, _native.DTYPE_I8, _native.DTYPE_I16, _native.DTYPE_I32, _native.DTYPE_I64)
+        n_roi, n_d, vmin, vmax, region, d_row = self._maps_region(s, code, r, masked_kernel, integer)
+        plan = fm.plan_maps(n_d, vmin, vmax, bw, integer, shift, n_roi, "first_order_maps: row %s" % label)
+        del region
+        vv = float("nan") if s.spacing is None else (s.spacing[0] * s.spacing[1]) * s.spacing[2]
+        K = (2 * r + 1) ** 3
+        table = torch.from_numpy(fm.entropy_table(K)).to(s.mask.device)
+        out = torch.empty((len(feats),) + shape, dtype=torch.float64, device=s.mask.device)
+        # an empty ROI: the kernel writes init_value everywhere (no voxel reads the discretisation)
+        self.engine.first_order_maps_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, code, r, masked_kernel, bw,
+                                         plan.low or 0, plan.n_levels or 1, plan.exact, plan.base, shift, vv,
+                                         float(init_value), fm.feature_bits(feats), table.data_ptr(), table.numel(),
+                                         out.data_ptr(), stream=s.stream)
+        maps = collections.OrderedDict((f, s.back(out[j])) for j, f in enumerate(feats))
+        return fm.FirstOrderMaps(row, r, bool(masked_kernel), bw, shift, float(init_value), plan.low, plan.n_levels,
+                                 plan.exact, n_roi, s.spacing, maps)
+
+    def _maps_region(self, s, code, r, masked_kernel, integer):
+        """The ROI count of row `code` (1..255, or 256 for mask > 0) of a staged feature-map call and its discretisation
+        region D (DESIGN §4.15): the ROI (masked_kernel) or the non-NaN voxels of the ROI's bounding box padded by r.
+        -> (n_roi, n_d, vmin, vmax, region, d_row): D is the voxels of the uint8 tensor `region` equal to d_row with a
+        non-NaN value, n_d of them spanning [vmin, vmax]."""
+        import torch
+        shape = tuple(s.mask.shape)
         st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, (), (), stream=s.stream)
         n_roi = int(st["voxels"][code] - st["nan_voxels"][code])
         d_row, region = code, s.mask
@@ -666,21 +689,51 @@ class LMInferer:
             d_row = 1
             st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, region.data_ptr(), shape, (), (), stream=s.stream)
         n_d = int(st["voxels"][d_row] - st["nan_voxels"][d_row])
-        plan = fm.plan_maps(n_d, float(st["moments"][d_row][2]), float(st["moments"][d_row][3]), bw, integer, shift, n_roi,
-                            "first_order_maps: row %s" % label)
+        return n_roi, n_d, float(st["moments"][d_row][2]), float(st["moments"][d_row][3]), region, d_row
+
+    def glcm_maps(self, image, mask, label="lung", features=None, kernel_radius=1, masked_kernel=True, bin_width=25,
+                  init_value=0.0):
+        """PyRadiomics' voxel-based GLCM extraction of one row -> lungmask_b200.glcm_maps.GLCMMaps: one float64 map of
+        the volume's shape per feature of texture.GLCM_FEATURES (or of `features`, a subset, in that order), indexed by
+        name (`gm["Contrast"]`).  `label`, `kernel_radius` (1, 2 or 3), `masked_kernel` and the window are those of
+        `first_order_maps`.  The discretisation region D (the ROI, or the non-NaN voxels of its bounding box padded by
+        kernel_radius) is discretised with the fixed `bin_width` as `texture` does; more than 255 levels or a +-inf there
+        is a ValueError before any map kernel runs.  For each of the 13 directions, a window's pairs are the voxel pairs
+        (v, v + d) with both voxels among its candidates; the features of each direction with pairs follow the sequence
+        of DESIGN §4.16 and are averaged over those directions (bit-identical to glcm_maps.maps_host).  An ROI voxel
+        whose window has no pair gets NaN, every other voxel `init_value`.
+
+        `image` and `mask` as for `texture` (a wavelet band or filtered image works as input).  CUDA inputs give CUDA
+        float64 tensors on their device with no host copy, CPU tensors CPU tensors and everything else numpy arrays.  Each
+        map takes 8 bytes per voxel (629 MB at 300 x 512 x 512, 13.8 GB for all 22), allocated for the requested features
+        only."""
+        import torch
+        from . import first_order_maps as fm
+        from . import glcm_maps as gm
+        from . import texture as tx
+        row = fm.check_label(label)
+        feats = gm.check_features(features)
+        r = fm.check_radius(kernel_radius)
+        bw = tx.check_arguments(bin_width)
+        s = self._stage("glcm_maps", image, mask)
+        shape = tuple(s.mask.shape)
+        code = 256 if row == fm.UNION else row
+        integer = s.dtype in (_native.DTYPE_U8, _native.DTYPE_I8, _native.DTYPE_I16, _native.DTYPE_I32, _native.DTYPE_I64)
+        n_roi, n_d, vmin, vmax, region, d_row = self._maps_region(s, code, r, masked_kernel, integer)
+        low, ng = None, 0
+        levels = torch.zeros(shape, dtype=torch.uint8, device=s.mask.device)
+        if n_roi:
+            low, ng = tx.discretisation(vmin, vmax, bw, "glcm_maps: row %s" % label)
+            self.engine.texture_levels_dev(s.vol.data_ptr(), s.dtype, region.data_ptr(), shape, d_row, low, bw, ng,
+                                           levels.data_ptr(), stream=s.stream)
         del region
-        vv = float("nan") if s.spacing is None else (s.spacing[0] * s.spacing[1]) * s.spacing[2]
-        K = (2 * r + 1) ** 3
-        table = torch.from_numpy(fm.entropy_table(K)).to(s.mask.device)
+        table = torch.from_numpy(fm.entropy_table(gm.max_pairs_n(r))).to(s.mask.device)
         out = torch.empty((len(feats),) + shape, dtype=torch.float64, device=s.mask.device)
-        # an empty ROI: the kernel writes init_value everywhere (no voxel reads the discretisation)
-        self.engine.first_order_maps_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, code, r, masked_kernel, bw,
-                                         plan.low or 0, plan.n_levels or 1, plan.exact, plan.base, shift, vv,
-                                         float(init_value), fm.feature_bits(feats), table.data_ptr(), table.numel(),
-                                         out.data_ptr(), stream=s.stream)
+        # an empty ROI: the level map is all 0, so every voxel gets init_value
+        self.engine.glcm_maps_dev(levels.data_ptr(), s.mask.data_ptr(), shape, code, r, ng or 1, float(init_value),
+                                  gm.feature_bits(feats), table.data_ptr(), table.numel(), out.data_ptr(), stream=s.stream)
         maps = collections.OrderedDict((f, s.back(out[j])) for j, f in enumerate(feats))
-        return fm.FirstOrderMaps(row, r, bool(masked_kernel), bw, shift, float(init_value), plan.low, plan.n_levels,
-                                 plan.exact, n_roi, s.spacing, maps)
+        return gm.GLCMMaps(row, r, bool(masked_kernel), bw, float(init_value), low, ng, n_roi, maps)
 
     def shape(self, mask, spacing=None, image=None):
         """Mesh shape features of every row of `statistics` -> lungmask_b200.shape.ShapeFeatures: every label value in the
