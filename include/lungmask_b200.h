@@ -443,6 +443,26 @@ LM_API int lm_glcm_maps_dev(lm_engine* e, const uint8_t* d_levels, const uint8_t
                             int radius, int n_levels, double init_value, uint32_t feature_bits,
                             const double* d_entropy_table, int64_t table_len, double* d_out, void* stream);
 
+/* Voxel-based GLSZM, GLRLM, GLDM and NGTDM feature maps (no counterpart in the reference; DESIGN §4.17): PyRadiomics'
+ * voxel-based extraction of one texture class of one row, for LMInferer.texture_maps.  Device memory, stream rule,
+ * checks, synchronisation, d_levels, d_mask, row, radius and n_levels as for lm_glcm_maps_dev.  A neighbour, run step or
+ * zone link counts only when both voxels are candidates of the window.  cls: LM_TEXMAP_GLSZM (zones: 26-connected
+ * components of equal level), LM_TEXMAP_GLRLM (runs along the 13 directions, features averaged over them), LM_TEXMAP_GLDM
+ * (dependence: neighbours within alpha levels, alpha >= 0; ignored by the other classes) or LM_TEXMAP_NGTDM.
+ * feature_bits: a non-empty subset of the class's 16, 16, 14 or 5 bits, bit k = the k-th name of texture.GLSZM_FEATURES,
+ * GLRLM_FEATURES, GLDM_FEATURES or NGTDM_FEATURES.  d_entropy_table: device float64, table_len = K (K + 1) / 2 with
+ * K = (2 radius + 1)^3 (first_order_maps.entropy_table).  d_out: popcount(feature_bits) float64 (n0,n1,n2) planes in bit
+ * order, not overlapping the inputs: centres get their window's features in the sequence of DESIGN §4.17 (NGTDM NaN when
+ * no candidate has a neighbour), every other voxel init_value.  Work area: one flag; each thread holds its window, item
+ * keys and union-find or per-level tables in local memory. */
+#define LM_TEXMAP_GLSZM 1
+#define LM_TEXMAP_GLRLM 2
+#define LM_TEXMAP_GLDM 3
+#define LM_TEXMAP_NGTDM 4
+LM_API int lm_texture_maps_dev(lm_engine* e, const uint8_t* d_levels, const uint8_t* d_mask, int n0, int n1, int n2, int row,
+                               int radius, int n_levels, int cls, int alpha, double init_value, uint32_t feature_bits,
+                               const double* d_entropy_table, int64_t table_len, double* d_out, void* stream);
+
 /* ---- one volume over several GPUs (SURVEY.md 8e; the reference is single-device, mask.py:118-121) ----------------
  * One process and one engine per GPU.  Slices are independent up to the 3-D post-processing (utils.py:48-51,
  * mask.py:173-187,196-202 vs utils.py:293-358): rank r of `world` runs pre-processing and the network on the contiguous

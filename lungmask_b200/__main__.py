@@ -18,7 +18,8 @@ image types (.json / .csv, LMInferer.filtered_features), and `--mesh DIR` the ma
 label and of the whole lung, one file per row (`--mesh-format` stl, obj or ply, `--mesh-space` lps or ras;
 LMInferer.mesh with the input's geometry), and `--first-order-maps DIR` the voxel-based first-order feature maps of one
 row, one image per feature with the input's geometry (LMInferer.first_order_maps), and `--glcm-maps DIR` its voxel-based
-GLCM feature maps the same way (LMInferer.glcm_maps).
+GLCM feature maps the same way (LMInferer.glcm_maps), and `--texture-maps DIR` its voxel-based GLSZM, GLRLM, GLDM and
+NGTDM feature maps (LMInferer.texture_maps).
 """
 import argparse
 import os
@@ -156,6 +157,25 @@ def build_parser():
                         "maskedKernel=False)")
     p.add_argument("--glcm-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
                    help="File format of --glcm-maps (default nii.gz)")
+    p.add_argument("--texture-maps", metavar="DIR", type=str, default=None,
+                   help="Also write voxel-based GLSZM, GLRLM, GLDM and NGTDM feature maps (PyRadiomics' voxelBased "
+                        "extraction) of one row to DIR, one float64 image per feature named <row>_<class>_<Feature> "
+                        "(lung_glszm_ZoneEntropy.nii.gz); uses --texture-bin-width")
+    p.add_argument("--texture-maps-classes", metavar="NAMES", type=str, default="glszm,glrlm,gldm,ngtdm",
+                   help="Comma-separated classes of --texture-maps: any of glszm, glrlm, gldm, ngtdm (default all; GLCM "
+                        "maps come from --glcm-maps)")
+    p.add_argument("--texture-maps-radius", type=int, choices=[1, 2, 3], default=1,
+                   help="Kernel radius of --texture-maps: the window is the (2r+1)^3 cube about each voxel (default 1)")
+    p.add_argument("--texture-maps-features", metavar="NAMES", type=str, default=None,
+                   help="Comma-separated features of --texture-maps, class-qualified PyRadiomics names such as "
+                        "glszm_ZoneEntropy,ngtdm_Contrast (default every feature of --texture-maps-classes)")
+    p.add_argument("--texture-maps-label", metavar="ROW", type=str, default="lung",
+                   help='Row of --texture-maps: "lung" (every label, default) or one label value 1..255')
+    p.add_argument("--texture-maps-unmasked", action="store_true",
+                   help="Windows of --texture-maps take every non-NaN voxel, not only the row's (PyRadiomics' "
+                        "maskedKernel=False)")
+    p.add_argument("--texture-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
+                   help="File format of --texture-maps (default nii.gz)")
     return p
 
 
@@ -210,6 +230,37 @@ def glcm_maps_arguments(args):
         except ValueError as ex:
             sys.exit("--glcm-maps-features: %s" % ex)
     return label, features
+
+
+def texture_maps_arguments(args):
+    """-> (label, classes, features) of --texture-maps; exits with a message naming the flag for a bad value."""
+    from . import first_order_maps as fm
+    from . import texture_maps as tm
+    from .texture import check_arguments as check_bin_width
+    if os.path.exists(args.texture_maps) and not os.path.isdir(args.texture_maps):
+        sys.exit("--texture-maps: %s exists and is not a directory" % args.texture_maps)
+    if not os.path.isdir(os.path.dirname(os.path.abspath(args.texture_maps))):
+        sys.exit("--texture-maps: the parent directory of %s does not exist" % args.texture_maps)
+    try:
+        check_bin_width(args.texture_bin_width)
+    except (TypeError, ValueError) as ex:
+        sys.exit("--texture-bin-width: %s" % ex)
+    label = args.texture_maps_label.strip()
+    try:
+        label = fm.check_label(label if label == "lung" else int(label))
+    except ValueError as ex:
+        sys.exit("--texture-maps-label: %s" % ex)
+    try:
+        classes = tm.check_classes([c.strip() for c in args.texture_maps_classes.split(",") if c.strip()])
+    except ValueError as ex:
+        sys.exit("--texture-maps-classes: %s" % ex)
+    features = None
+    if args.texture_maps_features is not None:
+        try:
+            features = tm.check_features([c.strip() for c in args.texture_maps_features.split(",") if c.strip()], classes)
+        except ValueError as ex:
+            sys.exit("--texture-maps-features: %s" % ex)
+    return label, classes, features
 
 
 def mesh_file_name(mesh, fmt):
@@ -293,6 +344,8 @@ def main(argv=None):
         maps_label, maps_features = first_order_maps_arguments(args)
     if args.glcm_maps is not None:
         glcm_label, glcm_features = glcm_maps_arguments(args)
+    if args.texture_maps is not None:
+        tmaps_label, tmaps_classes, tmaps_features = texture_maps_arguments(args)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -368,6 +421,15 @@ def main(argv=None):
                                             kernel_radius=args.glcm_maps_radius, masked_kernel=not args.glcm_maps_unmasked,
                                             bin_width=args.texture_bin_width),
                           image, args.glcm_maps_format)
+
+    if args.texture_maps is not None:
+        logger.info(f"Save texture maps to: {args.texture_maps}")
+        save_feature_maps(args.texture_maps,
+                          inferer.texture_maps(image, result, classes=tmaps_classes, label=tmaps_label,
+                                               features=tmaps_features, kernel_radius=args.texture_maps_radius,
+                                               masked_kernel=not args.texture_maps_unmasked,
+                                               bin_width=args.texture_bin_width),
+                          image, args.texture_maps_format)
 
 
 if __name__ == "__main__":

@@ -72,6 +72,8 @@ def lib():
                                      C.c_int64, C.c_double, C.c_double, C.c_uint32, vp, C.c_int64, vp, vp], i32),
         "lm_glcm_maps_dev": ([vp, u8p, u8p, i32, i32, i32, i32, i32, i32, C.c_double, C.c_uint32, vp, C.c_int64, vp, vp],
                              i32),
+        "lm_texture_maps_dev": ([vp, u8p, u8p, i32, i32, i32, i32, i32, i32, i32, i32, C.c_double, C.c_uint32, vp,
+                                 C.c_int64, vp, vp], i32),
         "lm_first_order_sums_dev": ([vp, vp, i32, u8p, i32, i32, i32, i32] + [vp] * 12, i32),
         "lm_first_order_splits_dev": ([vp, vp, i32, u8p, i32, i32, i32] + [vp] * 11, i32),
         "lm_wavelet_dev": ([vp, vp, i32, i32, i32, i32, i32, i32, vp, vp], i32),
@@ -108,7 +110,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -487,6 +489,17 @@ class Engine:
                                       int(radius), int(n_levels), float(init_value), int(feature_bits),
                                       C.c_void_p(d_table_ptr), int(table_len), C.c_void_p(d_out_ptr),
                                       C.c_void_p(int(stream)) if stream else None))
+
+    # ---- voxel-based GLSZM / GLRLM / GLDM / NGTDM maps (lm_texture_maps_dev)
+    def texture_maps_dev(self, d_levels_ptr, d_mask_ptr, shape, row, radius, n_levels, cls, alpha, init_value, feature_bits,
+                         d_table_ptr, table_len, d_out_ptr, stream=0):
+        """Writes the popcount(feature_bits) float64 maps of texture class `cls` (texture_maps.CLASS_CODES) of `row` (1..255, or 256 for
+        mask > 0) of a level map to d_out (device memory of this engine's device; `stream` as for apply_dev)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        _check(lib().lm_texture_maps_dev(self._h, C.c_void_p(d_levels_ptr), C.c_void_p(d_mask_ptr), n0, n1, n2, int(row),
+                                         int(radius), int(n_levels), int(cls), int(alpha), float(init_value),
+                                         int(feature_bits), C.c_void_p(d_table_ptr), int(table_len),
+                                         C.c_void_p(d_out_ptr), C.c_void_p(int(stream)) if stream else None))
 
     # ---- first-order sums (lm_first_order_sums_dev, lm_first_order_splits_dev)
     @staticmethod

@@ -28,6 +28,7 @@
 #include "mesh.cuh"
 #include "first_order_maps.cuh"
 #include "glcm_maps.cuh"
+#include "texture_maps.cuh"
 
 using namespace lm;
 
@@ -211,6 +212,7 @@ struct lm_engine {
   MeshWork mesh;                // lm_mesh_counts_dev, lm_mesh_emit_dev: the triangle table, per-line counts and offsets
   FomWork fo_maps;              // lm_first_order_maps_dev: the error flag
   GlcmMapsWork glcm_maps;       // lm_glcm_maps_dev: the error flag
+  TextureMapsWork texture_maps; // lm_texture_maps_dev: the error flag
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -943,6 +945,7 @@ void lm_destroy(lm_engine* e) {
   e->mesh.release();
   e->fo_maps.release();
   e->glcm_maps.release();
+  e->texture_maps.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1648,6 +1651,37 @@ int lm_glcm_maps_dev(lm_engine* e, const uint8_t* d_levels, const uint8_t* d_mas
   const GlcmMapsArgs a{row, radius, n_levels, init_value, feature_bits, d_entropy_table};
   const int rc = glcm_maps(e->glcm_maps, d_levels, d_mask, n0, n1, n2, a, d_out, e->num_sms, e->st, &e->launches);
   if (rc == kGlcmMapsRange) return fail(rc, "%s: a level above n_levels (%d) in a window", fn, n_levels);
+  return rc;
+}
+
+int lm_texture_maps_dev(lm_engine* e, const uint8_t* d_levels, const uint8_t* d_mask, int n0, int n1, int n2, int row,
+                        int radius, int n_levels, int cls, int alpha, double init_value, uint32_t feature_bits,
+                        const double* d_entropy_table, int64_t table_len, double* d_out, void* stream) {
+  static const char* fn = "lm_texture_maps_dev";
+  if (!e || !d_levels || !d_mask || !d_entropy_table || !d_out) return fail(-1, "%s: NULL argument", fn);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (cls < LM_TEXMAP_GLSZM || cls > LM_TEXMAP_NGTDM)
+    return fail(-1, "%s: class %d is not LM_TEXMAP_GLSZM, _GLRLM, _GLDM or _NGTDM", fn, cls);
+  if (row < 1 || row > 256) return fail(-1, "%s: row %d not in [1,256]", fn, row);
+  if (radius < 1 || radius > kTexMapsMaxRadius) return fail(-1, "%s: radius %d not in [1,%d]", fn, radius, kTexMapsMaxRadius);
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  if (alpha < 0) return fail(-1, "%s: alpha %d is negative", fn, alpha);
+  const int nf = texture_maps_features(cls);
+  if (feature_bits == 0 || (feature_bits >> nf))
+    return fail(-1, "%s: feature_bits 0x%x: set one or more of the class's %d feature bits and no other", fn, feature_bits, nf);
+  const int64_t K = (int64_t)(2 * radius + 1) * (2 * radius + 1) * (2 * radius + 1);
+  if (table_len != K * (K + 1) / 2)
+    return fail(-1, "%s: table_len %lld, radius %d needs %lld", fn, (long long)table_len, radius, (long long)(K * (K + 1) / 2));
+  const size_t n = (size_t)n0 * n1 * n2, out_bytes = (size_t)__builtin_popcount(feature_bits) * n * sizeof(double);
+  if (overlaps(d_levels, n, d_out, out_bytes)) return fail(-1, "%s: d_out overlaps d_levels", fn);
+  if (overlaps(d_mask, n, d_out, out_bytes)) return fail(-1, "%s: d_out overlaps d_mask", fn);
+  if (overlaps(d_entropy_table, (size_t)table_len * sizeof(double), d_out, out_bytes))
+    return fail(-1, "%s: d_out overlaps d_entropy_table", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}, {"d_mask", d_mask}, {"d_entropy_table", d_entropy_table},
+                                     {"d_out", d_out}}));
+  const TextureMapsArgs a{row, radius, n_levels, cls, alpha, init_value, feature_bits, d_entropy_table};
+  const int rc = texture_maps(e->texture_maps, d_levels, d_mask, n0, n1, n2, a, d_out, e->num_sms, e->st, &e->launches);
+  if (rc == kTexMapsRange) return fail(rc, "%s: a level above n_levels (%d) in a window", fn, n_levels);
   return rc;
 }
 

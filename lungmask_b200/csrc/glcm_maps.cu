@@ -13,13 +13,17 @@
 #include <algorithm>
 
 #include "glcm_maps.cuh"
+#include "map_common.cuh"
 
 namespace lm {
 namespace {
 
 constexpr int kThreads = 128;
 
-typedef unsigned __int128 u128;
+using maps::cvt_u128;
+using maps::insertion_sort;
+using maps::offset;
+using maps::u128;
 typedef __int128 i128;
 
 // Feature bits, in texture.GLCM_FEATURES order (only the ones that gate work are named).
@@ -70,44 +74,9 @@ __device__ __forceinline__ double exp_fixed(double y) {
   return __dmul_rn(p, __longlong_as_double(((long long)k + 1023) << 52));
 }
 
-// The correctly rounded float64 of a 128-bit integer: the top 64 significant bits with every shifted-out bit ORed into
-// bit 0 (a sticky bit below the rounding position), rounded to nearest even, scaled by 2^s exactly.
-__device__ __forceinline__ double cvt_u128(u128 m) {
-  const unsigned long long hi = (unsigned long long)(m >> 64), lo = (unsigned long long)m;
-  if (!hi) return __ull2double_rn(lo);
-  const int s = 64 - __clzll((long long)hi);
-  unsigned long long top = (unsigned long long)(m >> s);
-  if (s == 64 ? lo : (lo & ((1ull << s) - 1))) top |= 1ull;
-  return __dmul_rn(__ull2double_rn(top), __longlong_as_double((long long)(1023 + s) << 52));
-}
 __device__ __forceinline__ double cvt_i128(i128 v) { return v < 0 ? -cvt_u128((u128)0 - (u128)v) : cvt_u128((u128)v); }
 
 __device__ __forceinline__ double cvt(long long v) { return __ll2double_rn(v); }
-
-// The offset (dz, dy, dx) of direction d, in texture.OFFSETS order.
-__device__ __forceinline__ void offset(int d, int& dz, int& dy, int& dx) {
-  if (d < 4) {
-    dz = 0;
-    dy = d == 0 ? 0 : 1;
-    dx = d == 0 ? 1 : d - 2;
-  } else {
-    dz = 1;
-    dy = (d - 4) / 3 - 1;
-    dx = (d - 4) % 3 - 1;
-  }
-}
-
-__device__ __forceinline__ void insertion_sort(uint16_t* v, int n) {
-  for (int i = 1; i < n; ++i) {
-    const uint16_t k = v[i];
-    int j = i - 1;
-    while (j >= 0 && v[j] > k) {
-      v[j + 1] = v[j];
-      --j;
-    }
-    v[j + 1] = k;
-  }
-}
 
 template <int R>
 __global__ void __launch_bounds__(kThreads) glcm_maps_kernel(const uint8_t* __restrict__ levels, const uint8_t* __restrict__ mask,

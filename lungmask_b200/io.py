@@ -647,7 +647,8 @@ def feature_map_file(label, feature, fmt, feature_class=None):
 
 
 def save_feature_maps(directory, maps, like=None, fmt="nii.gz"):
-    """Writes every map of a lungmask_b200.first_order_maps.FirstOrderMaps or glcm_maps.GLCMMaps (numpy or CUDA) to
+    """Writes every map of a lungmask_b200.first_order_maps.FirstOrderMaps, glcm_maps.GLCMMaps or texture_maps.TextureMaps
+    (numpy or CUDA; the keys of TextureMaps are already class-qualified, so its files are <row>_<class>_<Feature>) to
     `directory` (created when missing) as float64 images with the geometry of `like` (a Volume, or None for unit
     spacing), one file per feature named by feature_map_file.  -> the paths written."""
     if fmt not in FEATURE_MAP_FORMATS:

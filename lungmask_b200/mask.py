@@ -735,6 +735,60 @@ class LMInferer:
         maps = collections.OrderedDict((f, s.back(out[j])) for j, f in enumerate(feats))
         return gm.GLCMMaps(row, r, bool(masked_kernel), bw, float(init_value), low, ng, n_roi, maps)
 
+    def texture_maps(self, image, mask, classes=("glszm", "glrlm", "gldm", "ngtdm"), label="lung", features=None,
+                     kernel_radius=1, masked_kernel=True, bin_width=25, gldm_alpha=0, init_value=0.0):
+        """PyRadiomics' voxel-based GLSZM, GLRLM, GLDM and NGTDM extraction of one row ->
+        lungmask_b200.texture_maps.TextureMaps: one float64 map of the volume's shape per feature of the `classes`,
+        keyed by class-qualified PyRadiomics names (`tm["glszm_SmallAreaEmphasis"]`, `tm["ngtdm_Contrast"]`), or of
+        `features`, a subset of those names, in class then feature order.  `classes` as for `texture`, without "glcm"
+        (glcm_maps gives those).  `label`, `kernel_radius` (1, 2 or 3), `masked_kernel`, the window, the discretisation
+        with the fixed `bin_width` and its refusals are those of `glcm_maps`.  Only voxels that are candidates of the window
+        link: zones (26-connected, equal level), runs along the 13 directions (features averaged over them), dependence
+        (neighbours within `gldm_alpha` levels, a non-negative int) and the NGTDM neighbourhoods.  Centres get their
+        window's features in the sequence of DESIGN §4.17 (bit-identical to texture_maps.maps_host); NGTDM gives NaN where
+        no candidate of the window has a neighbour.  Every other voxel holds `init_value`.
+
+        `image` and `mask` as for `texture` (a wavelet band or filtered image works as input).  CUDA inputs give CUDA
+        float64 tensors on their device with no host copy, CPU tensors CPU tensors and everything else numpy arrays.  The
+        level map is built once per call.  Each map takes 8 bytes per voxel (629 MB at 300 x 512 x 512, 32 GB for all 51),
+        allocated for the requested features only."""
+        import torch
+        from . import first_order_maps as fm
+        from . import texture as tx
+        from . import texture_maps as tm
+        row = fm.check_label(label)
+        cls = tm.check_classes(classes)
+        feats = tm.check_features(features, cls)
+        r = fm.check_radius(kernel_radius)
+        bw = tx.check_arguments(bin_width)
+        alpha = tx.check_alpha(gldm_alpha)
+        s = self._stage("texture_maps", image, mask)
+        shape = tuple(s.mask.shape)
+        code = 256 if row == fm.UNION else row
+        integer = s.dtype in (_native.DTYPE_U8, _native.DTYPE_I8, _native.DTYPE_I16, _native.DTYPE_I32, _native.DTYPE_I64)
+        n_roi, n_d, vmin, vmax, region, d_row = self._maps_region(s, code, r, masked_kernel, integer)
+        low, ng = None, 0
+        levels = torch.zeros(shape, dtype=torch.uint8, device=s.mask.device)
+        if n_roi:
+            low, ng = tx.discretisation(vmin, vmax, bw, "texture_maps: row %s" % label)
+            self.engine.texture_levels_dev(s.vol.data_ptr(), s.dtype, region.data_ptr(), shape, d_row, low, bw, ng,
+                                           levels.data_ptr(), stream=s.stream)
+        del region
+        table = torch.from_numpy(fm.entropy_table((2 * r + 1) ** 3)).to(s.mask.device)
+        out = torch.empty((len(feats),) + shape, dtype=torch.float64, device=s.mask.device)
+        # one launch per class into its planes; an empty ROI: the level map is all 0, so every voxel gets init_value
+        j = 0
+        for c in cls:
+            bits = tm.feature_bits(feats, c)
+            if not bits:
+                continue
+            self.engine.texture_maps_dev(levels.data_ptr(), s.mask.data_ptr(), shape, code, r, ng or 1, tm.CLASS_CODES[c],
+                                         alpha, float(init_value), bits, table.data_ptr(), table.numel(),
+                                         out[j].data_ptr(), stream=s.stream)
+            j += bin(bits).count("1")
+        maps = collections.OrderedDict((f, s.back(out[k])) for k, f in enumerate(feats))
+        return tm.TextureMaps(row, r, bool(masked_kernel), bw, float(init_value), low, ng, n_roi, cls, alpha, maps)
+
     def shape(self, mask, spacing=None, image=None):
         """Mesh shape features of every row of `statistics` -> lungmask_b200.shape.ShapeFeatures: every label value in the
         mask and every label 1..K-1 of the model (absent ones with 0 voxels and NaN features), then "lung" (mask != 0).
