@@ -257,6 +257,22 @@ LM_API int lm_glrlm_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, i
 LM_API int lm_neighbour_counts_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
                                    int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums, void* stream);
 
+/* Texture matrices over generalised neighbourhoods (DESIGN §4.18): PyRadiomics' distances and force2D settings, for
+ * LMInferer.texture.  Device memory, stream rule, checks, synchronisation and levels as for lm_glcm_dev.
+ * offsets (host): int8 [n_offsets][3] (dz, dy, dx) over array axes (0, 1, 2), 1 <= n_offsets <= 171, each with
+ *   components in -3..3, Chebyshev norm >= 1 and a positive first non-zero component, no two equal.
+ * lm_glcm_offsets_dev: U_o(i <= j) as lm_glcm_dev for each offset o in the given order: counts int64 [n_offsets][T].
+ * lm_neighbour_offsets_dev: lm_neighbour_counts_dev over the K = 2 n_offsets neighbours v +- o: dependence,
+ *   ngtdm_counts, ngtdm_sums int64 [n_levels][K + 1].
+ * lm_zone_sizes_plane_dev: lm_zone_sizes_dev with zones 8-connected within each plane normal to `axis` (0, 1 or 2). */
+LM_API int lm_glcm_offsets_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels,
+                               const int8_t* offsets, int n_offsets, int64_t* counts, void* stream);
+LM_API int lm_neighbour_offsets_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                                    const int8_t* offsets, int n_offsets, int64_t* dependence, int64_t* ngtdm_counts,
+                                    int64_t* ngtdm_sums, void* stream);
+LM_API int lm_zone_sizes_plane_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int axis, int64_t* n_pairs,
+                                   int64_t* sizes, int64_t* counts, size_t max_pairs, void* stream);
+
 /* Mesh shape support (no counterpart in the reference; DESIGN §4.10): LMInferer.shape computes PyRadiomics-style shape
  * features (surface area, mesh volume, sphericity, maximum diameters, principal axes) of every row of lm_label_stats_dev
  * from these.  Both take device memory of the engine's device and the caller's cudaStream_t with the event-wait rule of

@@ -19,7 +19,8 @@ label and of the whole lung, one file per row (`--mesh-format` stl, obj or ply, 
 LMInferer.mesh with the input's geometry), and `--first-order-maps DIR` the voxel-based first-order feature maps of one
 row, one image per feature with the input's geometry (LMInferer.first_order_maps), and `--glcm-maps DIR` its voxel-based
 GLCM feature maps the same way (LMInferer.glcm_maps), and `--texture-maps DIR` its voxel-based GLSZM, GLRLM, GLDM and
-NGTDM feature maps (LMInferer.texture_maps).
+NGTDM feature maps (LMInferer.texture_maps).  `--texture-distances`, `--texture-force2d` and `--texture-weighting-norm`
+set PyRadiomics' distances, force2D and weightingNorm for the texture matrices of --texture, --wavelet and --filtered.
 """
 import argparse
 import os
@@ -79,6 +80,16 @@ def build_parser():
     p.add_argument("--texture-classes", metavar="NAMES", type=str, default="glcm,glszm",
                    help="Comma-separated texture classes of --texture: any of glcm, glszm, glrlm, gldm, ngtdm "
                         "(default glcm,glszm)")
+    p.add_argument("--texture-distances", metavar="D", type=str, default=None,
+                   help="Comma-separated neighbour distances 1..3 of the GLCM, GLDM and NGTDM of --texture, --wavelet and "
+                        "--filtered, such as 1,2,3 (PyRadiomics' distances; default 1)")
+    p.add_argument("--texture-force2d", metavar="AXIS", type=int, choices=[0, 1, 2], default=None,
+                   help="Texture matrices of --texture, --wavelet and --filtered within the planes normal to array axis "
+                        "AXIS (0: axial slices; PyRadiomics' force2D / force2Ddimension; default 3-D)")
+    p.add_argument("--texture-weighting-norm", choices=["manhattan", "euclidean", "infinity", "no_weighting"], default=None,
+                   help="Merge the GLCM and GLRLM matrices of --texture, --wavelet and --filtered over directions with "
+                        "spacing-based weights before computing features (PyRadiomics' weightingNorm; default: features "
+                        "averaged over directions)")
     p.add_argument("--shape", metavar="PATH", type=str, default=None,
                    help="Also write the mesh shape features (PyRadiomics names: surface area, mesh volume, sphericity, "
                         "maximum 3-D and 2-D diameters, principal axis lengths) of every label and the whole lung: .json "
@@ -177,6 +188,21 @@ def build_parser():
     p.add_argument("--texture-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
                    help="File format of --texture-maps (default nii.gz)")
     return p
+
+
+def texture_settings_arguments(args):
+    """-> the keyword arguments distances, force2d, force2d_dimension, weighting_norm of the --texture-* settings;
+    exits with a message naming the flag for a bad value."""
+    from .texture import check_settings
+    distances = (1,)
+    if args.texture_distances is not None:
+        try:
+            distances = [int(c.strip()) for c in args.texture_distances.split(",") if c.strip()]
+            check_settings(distances)
+        except (TypeError, ValueError) as ex:
+            sys.exit("--texture-distances: %s" % ex)
+    return {"distances": tuple(distances), "force2d": args.texture_force2d is not None,
+            "force2d_dimension": args.texture_force2d or 0, "weighting_norm": args.texture_weighting_norm}
 
 
 def first_order_maps_arguments(args):
@@ -296,6 +322,7 @@ def main(argv=None):
             texture_classes = check_classes([c.strip() for c in args.texture_classes.split(",") if c.strip()])
         except ValueError as ex:
             sys.exit("--texture-classes: %s" % ex)
+    settings = texture_settings_arguments(args)
     if args.shape is not None:
         check_table_path(args.shape, "shape")
     if args.first_order is not None:
@@ -380,7 +407,8 @@ def main(argv=None):
         save_regional_statistics(args.regions, inferer.regional_statistics(image, result))
     if args.texture is not None:
         logger.info(f"Save texture features to: {args.texture}")
-        save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width, classes=texture_classes))
+        save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width, classes=texture_classes,
+                                                           **settings))
     if args.shape is not None:
         logger.info(f"Save shape features to: {args.shape}")
         save_shape(args.shape, inferer.shape(result, image=image))
@@ -391,12 +419,13 @@ def main(argv=None):
     if args.wavelet is not None:
         logger.info(f"Save wavelet features to: {args.wavelet}")
         save_wavelet_features(args.wavelet, inferer.wavelet_features(image, result, wavelet=args.wavelet_name,
-                                                                     bin_width=wavelet_bin_width, classes=wavelet_classes))
+                                                                     bin_width=wavelet_bin_width, classes=wavelet_classes,
+                                                                     **settings))
     if args.filtered is not None:
         logger.info(f"Save filtered-image features to: {args.filtered}")
         save_filtered_features(args.filtered, inferer.filtered_features(image, result, image_types=filtered_types,
                                                                         bin_width=filtered_bin_width,
-                                                                        classes=filtered_classes))
+                                                                        classes=filtered_classes, **settings))
     if args.mesh is not None:
         logger.info(f"Save meshes to: {args.mesh}")
         os.makedirs(args.mesh, exist_ok=True)

@@ -64,6 +64,9 @@ def lib():
         "lm_zone_sizes_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, C.c_size_t, vp], i32),
         "lm_glrlm_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp], i32),
         "lm_neighbour_counts_dev": ([vp, u8p, i32, i32, i32, i32, i32, vp, vp, vp, vp], i32),
+        "lm_glcm_offsets_dev": ([vp, u8p, i32, i32, i32, i32, vp, i32, vp, vp], i32),
+        "lm_neighbour_offsets_dev": ([vp, u8p, i32, i32, i32, i32, i32, vp, i32, vp, vp, vp, vp], i32),
+        "lm_zone_sizes_plane_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp, C.c_size_t, vp], i32),
         "lm_shape_sums_dev": ([vp, u8p, i32, i32, i32, vp, vp, vp, vp], i32),
         "lm_max_diameters_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp], i32),
         "lm_mesh_counts_dev": ([vp, u8p, i32, i32, i32, i32, vp, vp, vp, vp, vp], i32),
@@ -110,7 +113,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_glcm_offsets_dev", "lm_neighbour_offsets_dev", "lm_zone_sizes_plane_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -413,6 +416,41 @@ class Engine:
         _check(lib().lm_neighbour_counts_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, ng, int(alpha), _ptr(G), _ptr(N),
                                              _ptr(A), C.c_void_p(int(stream)) if stream else None))
         return G, N, A
+
+    # ---- generalised neighbourhoods (lm_glcm_offsets_dev, lm_neighbour_offsets_dev, lm_zone_sizes_plane_dev)
+    def glcm_offsets_dev(self, d_levels_ptr, shape, n_levels, offsets, stream=0):
+        """-> int64 (len(offsets), n_levels (n_levels + 1) / 2): the unordered pair counts U_o(i <= j) of a uint8 level
+        map for each (dz, dy, dx) of `offsets` (texture.offsets), in their order and the order of np.triu_indices."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ng = int(n_levels)
+        o = np.ascontiguousarray(offsets, dtype=np.int8).reshape(-1, 3)
+        counts = np.zeros((max(len(o), 1), max(ng * (ng + 1) // 2, 1)), np.int64)
+        _check(lib().lm_glcm_offsets_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, ng, _ptr(o), len(o), _ptr(counts),
+                                         C.c_void_p(int(stream)) if stream else None))
+        return counts
+
+    def neighbour_offsets_dev(self, d_levels_ptr, shape, n_levels, offsets, alpha=0, stream=0):
+        """-> (G, N, A), each int64 (n_levels, 2 len(offsets) + 1): neighbour_counts_dev over the neighbourhood
+        v +- o for o in `offsets`."""
+        n0, n1, n2 = (int(x) for x in shape)
+        ng = int(n_levels)
+        o = np.ascontiguousarray(offsets, dtype=np.int8).reshape(-1, 3)
+        G, N, A = (np.zeros((max(ng, 1), 2 * len(o) + 1), np.int64) for _ in range(3))
+        _check(lib().lm_neighbour_offsets_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, ng, int(alpha), _ptr(o), len(o),
+                                              _ptr(G), _ptr(N), _ptr(A), C.c_void_p(int(stream)) if stream else None))
+        return G, N, A
+
+    def zone_sizes_plane_dev(self, d_levels_ptr, shape, axis, stream=0):
+        """zone_sizes_dev with zones 8-connected within each plane normal to `axis` (0, 1 or 2)."""
+        n0, n1, n2 = (int(x) for x in shape)
+        cap = int(lib().lm_laa_max_pairs(max(n0, 0) * max(n1, 0) * max(n2, 0)))
+        n_pairs = np.zeros(256, np.int64)
+        sizes, counts = np.zeros(cap, np.int64), np.zeros(cap, np.int64)
+        _check(lib().lm_zone_sizes_plane_dev(self._h, C.c_void_p(d_levels_ptr), n0, n1, n2, int(axis), _ptr(n_pairs),
+                                             _ptr(sizes), _ptr(counts), cap, C.c_void_p(int(stream)) if stream else None))
+        offsets = np.concatenate([[0], np.cumsum(n_pairs)])
+        total = int(offsets[-1])
+        return {"n_pairs": n_pairs, "sizes": sizes[:total].copy(), "counts": counts[:total].copy(), "offsets": offsets}
 
     # ---- mesh shape support (lm_shape_sums_dev, lm_max_diameters_dev)
     def shape_sums_dev(self, d_mask_ptr, shape, stream=0):

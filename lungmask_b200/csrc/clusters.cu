@@ -14,7 +14,8 @@
 // Passes 2-4 run once for map_l and once for map_u.  The host then reads each row's dense extent, copies those bins and
 // the overflow list, and compacts them into (size, count) pairs: sorted overflow entries after the scanned dense bins.
 // zone_sizes (lm_zone_sizes_dev, DESIGN §4.9) runs passes 2-4 and the compaction once, 26-connected, on a caller's
-// texture level map: the size-zone matrix, row = level.
+// texture level map: the size-zone matrix, row = level; zone_sizes_plane (lm_zone_sizes_plane_dev, DESIGN §4.18) the same
+// 8-connected within the planes normal to an axis, on the map permuted so that those planes are slices.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -111,6 +112,20 @@ __global__ void __launch_bounds__(kThreads) cluster_hist_kernel(const uint32_t* 
     const int row = i / kSmallSizes, s = i % kSmallSizes;
     atomicAdd(&dense[(size_t)row * kClusterDense + s], s_small[i]);
     atomicMax(&row_max[row], (uint32_t)s);
+  }
+}
+
+// ---- in-plane zones --------------------------------------------------------------------------------------------------------
+// out = the (n0,n1,n2) map with `axis` (1 or 2) moved to the front: (n1,n0,n2) or (n2,n0,n1), so that the planes normal to
+// `axis` become slices.  Zone sizes do not change under the permutation.
+__global__ void __launch_bounds__(kThreads) plane_permute_kernel(const uint8_t* __restrict__ in, int n0, int n1, int n2, int axis,
+                                                                 uint8_t* __restrict__ out) {
+  const size_t n = (size_t)n0 * n1 * n2;
+  const uint32_t m1 = (uint32_t)n0, m2 = (uint32_t)(axis == 1 ? n2 : n1);
+  for (size_t t = blockIdx.x * (size_t)blockDim.x + threadIdx.x; t < n; t += (size_t)gridDim.x * blockDim.x) {
+    const uint32_t c = (uint32_t)(t % m2), r = (uint32_t)(t / m2), b = r % m1, a = r / m1;   // out[a][b][c]
+    const size_t src = axis == 1 ? ((size_t)b * n1 + a) * n2 + c : ((size_t)b * n1 + c) * n2 + a;
+    out[t] = in[src];
   }
 }
 
@@ -302,20 +317,44 @@ int laa_clusters(ClusterWork& w, const void* d_vol, int dtype, const uint8_t* d_
   return compact_histogram(g, out, st);
 }
 
-int zone_sizes(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
-               int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches) {
+namespace {
+// zone_sizes (axis < 0: 26-connected) and zone_sizes_plane (8-connected within the planes normal to axis; axes 1 and 2
+// label the permuted map in map_l).
+int zones_of(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int axis, int64_t* n_pairs, int64_t* sizes,
+             int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches) {
   const size_t n = (size_t)n0 * n1 * n2;
+  const bool permute = axis > 0;
   ClusterDev g;
-  SC((cudaError_t)w.reserve(layout(nullptr, n, false, &g)));
-  layout(static_cast<char*>(w.d), n, false, &g);
+  SC((cudaError_t)w.reserve(layout(nullptr, n, permute, &g)));
+  layout(static_cast<char*>(w.d), n, permute, &g);
   const int crc = clear_histogram(g, st);
   if (crc) return crc;
-  const int lrc = count_components(g, d_levels, n0, n1, n2, 26, 0, num_sms, st, launches);
+  const uint8_t* map = d_levels;
+  int m0 = n0, m1 = n1, m2 = n2;
+  if (permute) {
+    plane_permute_kernel<<<grid_for(plane_permute_kernel, 0, n, num_sms), kThreads, 0, st>>>(d_levels, n0, n1, n2, axis, g.map_l);
+    SC(cudaGetLastError());
+    ++*launches;
+    map = g.map_l;
+    m0 = axis == 1 ? n1 : n2, m1 = n0, m2 = axis == 1 ? n2 : n1;
+  }
+  const int lrc = count_components(g, map, m0, m1, m2, axis < 0 ? 26 : 8, 0, num_sms, st, launches);
   if (lrc) return lrc;
   int64_t voxels[kClusterRows], zones[kClusterRows], pairs[kClusterRows];
   const int rc = compact_histogram(g, {voxels, zones, pairs, sizes, counts, max_pairs}, st);
   for (int r = 0; r < 256; ++r) n_pairs[r] = pairs[r];   // row 256 (the union) stays empty: fixed_row is 0
   return rc;
+}
+}  // namespace
+
+int zone_sizes(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
+               int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches) {
+  return zones_of(w, d_levels, n0, n1, n2, -1, n_pairs, sizes, counts, max_pairs, num_sms, st, launches);
+}
+
+int zone_sizes_plane(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int axis, int64_t* n_pairs, int64_t* sizes,
+                     int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches) {
+  return zones_of(w, d_levels, n0, n1, n2, axis, n_pairs, sizes, counts, max_pairs, num_sms, st, launches);
 }
 
 }  // namespace lm

@@ -44,4 +44,9 @@ int laa_clusters(ClusterWork& w, const void* d_vol, int dtype, const uint8_t* d_
 int zone_sizes(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int64_t* n_pairs, int64_t* sizes,
                int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches);
 
+// zone_sizes with 8-connected zones within each plane normal to `axis` (0, 1 or 2).  Axes 1 and 2 permute the map into
+// the work area's first map first (1 B / voxel more).  The caller checks the arguments.
+int zone_sizes_plane(ClusterWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int axis, int64_t* n_pairs, int64_t* sizes,
+                     int64_t* counts, size_t max_pairs, int num_sms, cudaStream_t st, int64_t* launches);
+
 }  // namespace lm

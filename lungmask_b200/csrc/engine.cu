@@ -1307,6 +1307,70 @@ int lm_zone_sizes_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int
   return 0;
 }
 
+// The offset list of lm_glcm_offsets_dev / lm_neighbour_offsets_dev: 1..171 distinct offsets, components in -3..3,
+// Chebyshev norm >= 1, first non-zero component positive.
+static int check_offsets(const char* fn, const int8_t* offsets, int n_offsets) {
+  if (!offsets) return fail(-1, "%s: NULL offsets", fn);
+  if (n_offsets < 1 || n_offsets > kMaxOffsets) return fail(-1, "%s: n_offsets %d not in [1,%d]", fn, n_offsets, kMaxOffsets);
+  for (int k = 0; k < n_offsets; ++k) {
+    const int dz = offsets[3 * k], dy = offsets[3 * k + 1], dx = offsets[3 * k + 2];
+    if (dz < -3 || dz > 3 || dy < -3 || dy > 3 || dx < -3 || dx > 3)
+      return fail(-1, "%s: offset %d (%d,%d,%d) has a component outside -3..3", fn, k, dz, dy, dx);
+    const int first = dz ? dz : (dy ? dy : dx);
+    if (first == 0) return fail(-1, "%s: offset %d is (0,0,0)", fn, k);
+    if (first < 0) return fail(-1, "%s: offset %d (%d,%d,%d): the first non-zero component is negative", fn, k, dz, dy, dx);
+    for (int j = 0; j < k; ++j)
+      if (offsets[3 * j] == dz && offsets[3 * j + 1] == dy && offsets[3 * j + 2] == dx)
+        return fail(-1, "%s: offset %d (%d,%d,%d) repeats offset %d", fn, k, dz, dy, dx, j);
+  }
+  return 0;
+}
+
+int lm_glcm_offsets_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, const int8_t* offsets,
+                        int n_offsets, int64_t* counts, void* stream) {
+  static const char* fn = "lm_glcm_offsets_dev";
+  if (!e || !d_levels || !counts) return fail(-1, "%s: NULL argument", fn);
+  RC(check_offsets(fn, offsets, n_offsets));
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  const int rc = glcm_offsets(e->texture, d_levels, n0, n1, n2, n_levels, offsets, n_offsets, counts, e->num_sms, e->st,
+                              &e->launches);
+  if (rc) return texture_device_error(fn, rc, n_levels);
+  return 0;
+}
+
+int lm_neighbour_offsets_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                             const int8_t* offsets, int n_offsets, int64_t* dependence, int64_t* ngtdm_counts,
+                             int64_t* ngtdm_sums, void* stream) {
+  static const char* fn = "lm_neighbour_offsets_dev";
+  if (!e || !d_levels || !dependence || !ngtdm_counts || !ngtdm_sums) return fail(-1, "%s: NULL argument", fn);
+  RC(check_offsets(fn, offsets, n_offsets));
+  RC(check_texture_volume(fn, n0, n1, n2));
+  if (n_levels < 1 || n_levels > kTextureMaxLevels) return fail(-1, "%s: n_levels %d not in [1,%d]", fn, n_levels, kTextureMaxLevels);
+  if (alpha < 0) return fail(-1, "%s: alpha %d is negative", fn, alpha);
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  const int rc = neighbour_offsets(e->texture, d_levels, n0, n1, n2, n_levels, alpha, offsets, n_offsets, dependence,
+                                   ngtdm_counts, ngtdm_sums, e->num_sms, e->st, &e->launches);
+  if (rc) return texture_device_error(fn, rc, n_levels);
+  return 0;
+}
+
+int lm_zone_sizes_plane_dev(lm_engine* e, const uint8_t* d_levels, int n0, int n1, int n2, int axis, int64_t* n_pairs,
+                            int64_t* sizes, int64_t* counts, size_t max_pairs, void* stream) {
+  static const char* fn = "lm_zone_sizes_plane_dev";
+  if (!e || !d_levels || !n_pairs || !sizes || !counts) return fail(-1, "%s: NULL argument", fn);
+  if (axis < 0 || axis > 2) return fail(-1, "%s: axis %d not in [0,2]", fn, axis);
+  RC(check_texture_volume(fn, n0, n1, n2));
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (max_pairs < laa_max_pairs(n))
+    return fail(-1, "%s: max_pairs %zu below lm_laa_max_pairs(%zu) = %zu", fn, max_pairs, n, laa_max_pairs(n));
+  RC(analysis_inputs(e, fn, stream, {{"d_levels", d_levels}}));
+  RC(zone_sizes_plane(e->clusters, d_levels, n0, n1, n2, axis, n_pairs, sizes, counts, max_pairs, e->num_sms, e->st,
+                      &e->launches));
+  return 0;
+}
+
 // The argument checks the two shape calls share: the shape (fewer than 2^32 voxels, every axis below 2^30).
 static int check_shape_volume(const char* fn, int n0, int n1, int n2) {
   if (n0 < 1 || n1 < 1 || n2 < 1) return fail(-1, "%s: empty volume (%d,%d,%d)", fn, n0, n1, n2);

@@ -132,7 +132,8 @@ __global__ void ccl_init_kernel(const uint8_t* __restrict__ vals, uint32_t* __re
   }
 }
 
-// CONN: 26 (3-D full), 6 (3-D faces), 4 (2-D faces within a slice). Only neighbours inside the box count.
+// CONN: 26 (3-D full), 6 (3-D faces), 4 (2-D faces within a slice), 8 (2-D full within a slice: the first backward row
+// of the 26 rule alone). Only neighbours inside the box count.
 // The x-runs are already linked inside every 32-voxel segment (ccl_init_kernel); here lane 0 joins the segments and each
 // voxel is united with its backward neighbours in the four rows (y-1,z), (y-1,z-1), (y,z-1), (y+1,z-1).
 // rule != 0 (CONN == 26; the default): per backward row with a = (x-1), b = (x), c = (x+1) of that row,
@@ -155,9 +156,9 @@ __global__ void ccl_merge_kernel(const uint8_t* __restrict__ vals, uint32_t* __r
     if (!v) continue;
     const bool left = x > b.x0 && vals[i - 1] == v;
     if (left && (threadIdx.x & 31) == 0) uf_union(parent, i, i - 1);  // the run continues across a 32-voxel segment
-    if (CONN == 26) {
+    if (CONN == 26 || CONN == 8) {
 #pragma unroll
-      for (int r = 0; r < 4; ++r) {
+      for (int r = 0; r < (CONN == 8 ? 1 : 4); ++r) {
         const int dy = (r == 3) ? 1 : (r == 2 ? 0 : -1), dz = (r == 0) ? 0 : -1;
         const int yy = y + dy, zz = z + dz;
         if (zz < b.z0 || yy < b.y0 || yy >= b.y1) continue;
@@ -1171,6 +1172,7 @@ int ccl_volume_device(const uint8_t* d_vals, uint32_t* d_parent, int S, int H, i
     case 4: return run_ccl<4>(d_vals, d_parent, d, full, n, num_sms, st, launches);
     case 6: return run_ccl<6>(d_vals, d_parent, d, full, n, num_sms, st, launches);
     case 26: return run_ccl<26>(d_vals, d_parent, d, full, n, num_sms, st, launches);
+    case 8: return run_ccl<8>(d_vals, d_parent, d, full, n, num_sms, st, launches, 0);   // all 3 backward probes
     default: return -1;
   }
 }

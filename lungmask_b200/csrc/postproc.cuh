@@ -56,8 +56,8 @@ int ccl_slab_device(const uint8_t* d_labels, uint32_t* d_parent, int S, int H, i
 int ccl_join_slabs_device(const uint8_t* d_labels, uint32_t* d_parent, int S, int H, int W, const int* first_slices, int n_bounds,
                           int num_sms, cudaStream_t st, int64_t* launches);
 // Equal-value connected components of a whole (S,H,W) uint8 volume (0 = background) into d_parent: a non-zero voxel gets
-// the minimum linear index of its component, a zero voxel 0xFFFFFFFF.  conn: 4 (faces within a slice), 6 (faces) or 26
-// (full, the default pruned neighbour rule).  Fewer than 2^32 voxels.  Returns 0, a cudaError_t, or -1 for another conn.
+// the minimum linear index of its component, a zero voxel 0xFFFFFFFF.  conn: 4 (faces within a slice), 8 (full within a
+// slice), 6 (faces) or 26 (full, the default pruned neighbour rule).  Fewer than 2^32 voxels.  Returns 0, a cudaError_t, or -1 for another conn.
 int ccl_volume_device(const uint8_t* d_vals, uint32_t* d_parent, int S, int H, int W, int conn, int num_sms, cudaStream_t st,
                       int64_t* launches);
 // utils.keep_largest_connected_component on a device-resident (S,H,W) 0/1 mask; -21 if the mask is empty.

@@ -16,6 +16,8 @@
 //   neighbour  the same layout: each ROI voxel reads its 26 neighbours and forms, in registers, W (neighbours in the
 //           ROI), S (the sum of their levels) and c (those within alpha of its level); G(i, c), N(i, W) and
 //           A(i, W) += |W i - S| are warp-aggregated by key into shared counters that hold every level.
+//   glcm_offsets, neighbour_offsets  the glcm and neighbour layouts over a caller's offset list (lm_glcm_offsets_dev,
+//           lm_neighbour_offsets_dev, DESIGN §4.18): distances 1..3 and in-plane neighbourhoods.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -255,6 +257,134 @@ __global__ void __launch_bounds__(kThreads) neighbour_kernel(const uint8_t* __re
   }
 }
 
+// ---- generalised neighbourhoods (DESIGN §4.18) ----------------------------------------------------------------------
+// An offset list travels as a kernel parameter (constant bank): offset k packs (dz, dy, dx) as three signed bytes.
+struct OffsetList {
+  int o[kMaxOffsets];
+};
+__device__ __forceinline__ int off_z(int p) { return (int)(signed char)(p & 0xff); }
+__device__ __forceinline__ int off_y(int p) { return (int)(signed char)((p >> 8) & 0xff); }
+__device__ __forceinline__ int off_x(int p) { return (int)(signed char)((p >> 16) & 0xff); }
+
+// glcm_kernel over the offsets first .. first + count - 1 of `offs`: the same warp layout, key aggregation and shared
+// layout (kTri: the triangle of every offset of the group; otherwise the band j - i < kBand, the rest global).
+template <bool kTri>
+__global__ void __launch_bounds__(kThreads) glcm_offsets_kernel(const uint8_t* __restrict__ lev, int n0, int n1, int n2, int ng,
+                                                                OffsetList offs, int first, int count,
+                                                                uint32_t* __restrict__ counts, int* __restrict__ flag) {
+  extern __shared__ uint32_t s_cnt[];
+  const int t_len = ng * (ng + 1) / 2;
+  const int per_dir = kTri ? t_len : ng * kBand;
+  for (int i = threadIdx.x; i < count * per_dir; i += blockDim.x) s_cnt[i] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const size_t warp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5, n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+  const int runs_x = (n2 + 31) / 32;
+  const size_t runs = (size_t)n0 * n1 * runs_x;
+  for (size_t r = warp; r < runs; r += n_warps) {   // warp-uniform
+    const size_t line = r / runs_x;
+    const int x = (int)(r % runs_x) * 32 + lane, y = (int)(line % n1), z = (int)(line / n1);
+    const size_t v = line * n2 + x;
+    int a = x < n2 ? lev[v] : 0;
+    if (a > ng) { atomicOr(flag, 1); a = 0; }
+    if (!__any_sync(kFull, a != 0)) continue;
+#pragma unroll 1
+    for (int d = 0; d < count; ++d) {
+      const int p = offs.o[first + d], dz = off_z(p), dy = off_y(p), dx = off_x(p);
+      const int zz = z + dz, yy = y + dy, xx = x + dx;
+      int b = 0;
+      if (a && (unsigned)zz < (unsigned)n0 && (unsigned)yy < (unsigned)n1 && (unsigned)xx < (unsigned)n2)
+        b = lev[(size_t)((long long)v + ((long long)dz * n1 + dy) * n2 + dx)];
+      if (b > ng) { atomicOr(flag, 1); b = 0; }
+      if (b) {
+        const int i = min(a, b), j = max(a, b);
+        const bool shared = kTri || j - i < kBand;
+        const int key = kTri ? tri(i, j, ng) : (shared ? (j - i) * ng + i - 1 : per_dir + tri(i, j, ng));
+        const unsigned peers = __match_any_sync(__activemask(), key);
+        if (lane == __ffs(peers) - 1) {
+          if (shared) atomicAdd(&s_cnt[d * per_dir + key], (uint32_t)__popc(peers));
+          else atomicAdd(&counts[(size_t)(first + d) * t_len + (key - per_dir)], (uint32_t)__popc(peers));
+        }
+      }
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < count * per_dir; k += blockDim.x) {
+    if (!s_cnt[k]) continue;
+    const int d = k / per_dir, e = k % per_dir;
+    const int t = kTri ? e : tri(e % ng + 1, e % ng + 1 + e / ng, ng);
+    atomicAdd(&counts[(size_t)(first + d) * t_len + t], s_cnt[k]);
+  }
+}
+
+// neighbour_kernel over the neighbourhood +-offs (K = 2 n neighbours, cols = K + 1 cells per level).  kShared: the
+// counters of every level in shared memory (ng * cols * 16 B); otherwise warp-aggregated global atomics.  Warp sums of
+// |W i - S| < 32 * 342 * 254 < 2^22 fit in 32 bits.
+template <bool kShared>
+__global__ void __launch_bounds__(kThreads) neighbour_offsets_kernel(const uint8_t* __restrict__ lev, int n0, int n1, int n2,
+                                                                     int ng, int alpha, OffsetList offs, int n_offs, int cols,
+                                                                     uint32_t* __restrict__ dep, uint32_t* __restrict__ cnt,
+                                                                     unsigned long long* __restrict__ sums,
+                                                                     int* __restrict__ flag) {
+  extern __shared__ unsigned long long s_sum[];
+  const int cells = ng * cols;
+  uint32_t* s_dep = reinterpret_cast<uint32_t*>(s_sum + cells);
+  uint32_t* s_cnt = s_dep + cells;
+  if (kShared) {
+    for (int i = threadIdx.x; i < cells; i += blockDim.x) s_sum[i] = 0, s_dep[i] = 0, s_cnt[i] = 0;
+    __syncthreads();
+  }
+  const int lane = threadIdx.x & 31;
+  const size_t warp = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5, n_warps = ((size_t)gridDim.x * blockDim.x) >> 5;
+  const int runs_x = (n2 + 31) / 32;
+  const size_t segs = (size_t)n0 * n1 * runs_x;
+  for (size_t r = warp; r < segs; r += n_warps) {   // warp-uniform
+    const size_t line = r / runs_x;
+    const int x = (int)(r % runs_x) * 32 + lane, y = (int)(line % n1), z = (int)(line / n1);
+    const size_t v = line * n2 + x;
+    int a = x < n2 ? lev[v] : 0;
+    if (a > ng) { atomicOr(flag, 1); a = 0; }
+    if (!__any_sync(kFull, a != 0)) continue;
+    int w = 0, s = 0, c = 0;
+    if (a) {
+#pragma unroll 1
+      for (int k = 0; k < n_offs; ++k) {
+        const int p = offs.o[k], dz = off_z(p), dy = off_y(p), dx = off_x(p);
+        const long long step = ((long long)dz * n1 + dy) * n2 + dx;
+#pragma unroll
+        for (int sgn = 1; sgn >= -1; sgn -= 2) {
+          const int zz = z + sgn * dz, yy = y + sgn * dy, xx = x + sgn * dx;
+          int b = 0;
+          if ((unsigned)zz < (unsigned)n0 && (unsigned)yy < (unsigned)n1 && (unsigned)xx < (unsigned)n2)
+            b = lev[(size_t)((long long)v + sgn * step)];
+          if (b > ng) b = 0;   // flagged by the lane that holds it
+          if (b) {
+            ++w;
+            s += b;
+            c += abs(b - a) <= alpha;
+          }
+        }
+      }
+    }
+    const int kd = a ? (a - 1) * cols + c : -1, kn = a ? (a - 1) * cols + w : -1;
+    const unsigned pd = __match_any_sync(kFull, kd), pn = __match_any_sync(kFull, kn);
+    const unsigned sum = __reduce_add_sync(pn, (unsigned)abs(w * a - s));
+    if (a && lane == __ffs(pd) - 1) atomicAdd(kShared ? &s_dep[kd] : &dep[kd], (uint32_t)__popc(pd));
+    if (a && lane == __ffs(pn) - 1) {
+      atomicAdd(kShared ? &s_cnt[kn] : &cnt[kn], (uint32_t)__popc(pn));
+      if (sum) atomicAdd(kShared ? &s_sum[kn] : &sums[kn], (unsigned long long)sum);
+    }
+  }
+  if (kShared) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < cells; k += blockDim.x) {
+      if (s_dep[k]) atomicAdd(&dep[k], s_dep[k]);
+      if (s_cnt[k]) atomicAdd(&cnt[k], s_cnt[k]);
+      if (s_sum[k]) atomicAdd(&sums[k], s_sum[k]);
+    }
+  }
+}
+
 // ---- host -----------------------------------------------------------------------------------------------------------
 #define SC(x)                                   \
   do {                                          \
@@ -408,6 +538,88 @@ int neighbour_counts(TextureWork& w, const uint8_t* d_levels, int n0, int n1, in
   SC(cudaFuncSetAttribute(neighbour_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   neighbour_kernel<<<grid_for(neighbour_kernel, smem, threads, num_sms), kThreads, smem, st>>>(d_levels, n0, n1, n2, n_levels,
                                                                                               alpha, d_dep, d_cnt, d_sums, flag);
+  SC(cudaGetLastError());
+  ++*launches;
+  std::vector<unsigned long long> hs(cells);
+  std::vector<uint32_t> hd(cells), hc(cells);
+  SC(cudaMemcpyAsync(hs.data(), d_sums, cells * 8, cudaMemcpyDeviceToHost, st));
+  SC(cudaMemcpyAsync(hd.data(), d_dep, cells * 4, cudaMemcpyDeviceToHost, st));
+  SC(cudaMemcpyAsync(hc.data(), d_cnt, cells * 4, cudaMemcpyDeviceToHost, st));
+  const int rc = flag_result(flag, st);
+  if (rc) return rc;
+  for (size_t k = 0; k < cells; ++k) dependence[k] = hd[k], ngtdm_counts[k] = hc[k], ngtdm_sums[k] = (int64_t)hs[k];
+  return 0;
+}
+
+namespace {
+OffsetList pack_offsets(const int8_t* offsets, int n) {
+  OffsetList l{};
+  for (int k = 0; k < n; ++k)
+    l.o[k] = (int)(uint8_t)offsets[3 * k] | ((int)(uint8_t)offsets[3 * k + 1] << 8) | ((int)(uint8_t)offsets[3 * k + 2] << 16);
+  return l;
+}
+}  // namespace
+
+int glcm_offsets(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, const int8_t* offsets,
+                 int n_offsets, int64_t* counts, int num_sms, cudaStream_t st, int64_t* launches) {
+  const size_t t_len = (size_t)n_levels * (n_levels + 1) / 2, total = (size_t)n_offsets * t_len;
+  SC((cudaError_t)w.reserve(align256(sizeof(int)) + align256(total * 4)));
+  int* flag = static_cast<int*>(w.d);
+  uint32_t* d_counts = reinterpret_cast<uint32_t*>(static_cast<char*>(w.d) + align256(sizeof(int)));
+  SC(cudaMemsetAsync(flag, 0, sizeof(int), st));
+  SC(cudaMemsetAsync(d_counts, 0, total * 4, st));
+  const OffsetList offs = pack_offsets(offsets, n_offsets);
+  const size_t threads = (size_t)n0 * n1 * ((n2 + 31) / 32) * 32;
+  const bool tri_layout = n_levels <= kSmemLevels;
+  const int per_dir = tri_layout ? (int)t_len : n_levels * kBand;
+  const int group = std::max(1, std::min(n_offsets, kSmemWords / per_dir));   // >= 13: per_dir <= 4095
+  for (int first = 0; first < n_offsets; first += group) {
+    const int count = std::min(group, n_offsets - first);
+    const size_t smem = (size_t)count * per_dir * 4;
+    if (tri_layout) {
+      SC(cudaFuncSetAttribute(glcm_offsets_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      glcm_offsets_kernel<true><<<grid_for(glcm_offsets_kernel<true>, smem, threads, num_sms), kThreads, smem, st>>>(
+          d_levels, n0, n1, n2, n_levels, offs, first, count, d_counts, flag);
+    } else {
+      SC(cudaFuncSetAttribute(glcm_offsets_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      glcm_offsets_kernel<false><<<grid_for(glcm_offsets_kernel<false>, smem, threads, num_sms), kThreads, smem, st>>>(
+          d_levels, n0, n1, n2, n_levels, offs, first, count, d_counts, flag);
+    }
+    SC(cudaGetLastError());
+    ++*launches;
+  }
+  std::vector<uint32_t> h(total);
+  SC(cudaMemcpyAsync(h.data(), d_counts, total * 4, cudaMemcpyDeviceToHost, st));
+  const int rc = flag_result(flag, st);
+  if (rc) return rc;
+  for (size_t k = 0; k < total; ++k) counts[k] = h[k];
+  return 0;
+}
+
+int neighbour_offsets(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                      const int8_t* offsets, int n_offsets, int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums,
+                      int num_sms, cudaStream_t st, int64_t* launches) {
+  const int cols = 2 * n_offsets + 1;
+  const size_t cells = (size_t)n_levels * cols;
+  const size_t sums_at = align256(sizeof(int)), dep_at = sums_at + align256(cells * 8), cnt_at = dep_at + align256(cells * 4);
+  SC((cudaError_t)w.reserve(cnt_at + align256(cells * 4)));
+  char* base = static_cast<char*>(w.d);
+  int* flag = reinterpret_cast<int*>(base);
+  unsigned long long* d_sums = reinterpret_cast<unsigned long long*>(base + sums_at);
+  uint32_t* d_dep = reinterpret_cast<uint32_t*>(base + dep_at);
+  uint32_t* d_cnt = reinterpret_cast<uint32_t*>(base + cnt_at);
+  SC(cudaMemsetAsync(base, 0, cnt_at + cells * 4, st));
+  const OffsetList offs = pack_offsets(offsets, n_offsets);
+  const size_t threads = (size_t)n0 * n1 * ((n2 + 31) / 32) * 32;
+  if (cells * 16 <= (size_t)kSmemWords * 4) {
+    const size_t smem = cells * 16;
+    SC(cudaFuncSetAttribute(neighbour_offsets_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    neighbour_offsets_kernel<true><<<grid_for(neighbour_offsets_kernel<true>, smem, threads, num_sms), kThreads, smem, st>>>(
+        d_levels, n0, n1, n2, n_levels, alpha, offs, n_offsets, cols, d_dep, d_cnt, d_sums, flag);
+  } else {
+    neighbour_offsets_kernel<false><<<grid_for(neighbour_offsets_kernel<false>, 0, threads, num_sms), kThreads, 0, st>>>(
+        d_levels, n0, n1, n2, n_levels, alpha, offs, n_offsets, cols, d_dep, d_cnt, d_sums, flag);
+  }
   SC(cudaGetLastError());
   ++*launches;
   std::vector<unsigned long long> hs(cells);

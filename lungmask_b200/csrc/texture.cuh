@@ -1,5 +1,5 @@
-// Grey-level texture matrices of one ROI (lm_texture_levels_dev, lm_glcm_dev, lm_glrlm_dev, lm_neighbour_counts_dev;
-// see texture.cu, DESIGN §4.9).
+// Grey-level texture matrices of one ROI (lm_texture_levels_dev, lm_glcm_dev, lm_glrlm_dev, lm_neighbour_counts_dev,
+// lm_glcm_offsets_dev, lm_neighbour_offsets_dev; see texture.cu, DESIGN §4.9 and §4.18).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -10,6 +10,7 @@ namespace lm {
 constexpr int kGlcmDirections = 13;    // the offsets of the 26-neighbourhood whose first non-zero component is positive
 constexpr int kTextureMaxLevels = 255;
 constexpr int kNeighbourCells = 27;    // W or c = 0..26 neighbours of the 26-neighbourhood
+constexpr int kMaxOffsets = 171;       // the half-space offsets of Chebyshev norm 1..3 (DESIGN §4.18)
 
 // Device work buffers of the texture calls, grown on demand and reused across calls.
 struct TextureWork {
@@ -48,5 +49,18 @@ int glrlm(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n
 int neighbour_counts(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
                      int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums, int num_sms, cudaStream_t st,
                      int64_t* launches);
+
+// glcm over a caller's list of n_offsets half-space offsets (int8 [n][3] (dz, dy, dx), host, checked by the caller):
+// counts [n][T] int64 (host) in the triangle order of glcm.  The offsets run in groups whose counters fit the shared
+// budget of glcm.  Synchronises `st`.
+int glcm_offsets(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, const int8_t* offsets,
+                 int n_offsets, int64_t* counts, int num_sms, cudaStream_t st, int64_t* launches);
+
+// neighbour_counts over the neighbourhood +-offsets (K = 2 n_offsets neighbours): each output [n_levels][K + 1] int64
+// (host).  The counters sit in shared memory while n_levels (K + 1) 16 B fit glcm's budget, in global memory otherwise.
+// Synchronises `st`.
+int neighbour_offsets(TextureWork& w, const uint8_t* d_levels, int n0, int n1, int n2, int n_levels, int alpha,
+                      const int8_t* offsets, int n_offsets, int64_t* dependence, int64_t* ngtdm_counts, int64_t* ngtdm_sums,
+                      int num_sms, cudaStream_t st, int64_t* launches);
 
 }  // namespace lm

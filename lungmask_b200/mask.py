@@ -476,7 +476,8 @@ class LMInferer:
         return rg.build(labels, present, self.modelname, s.spacing, counts, axis, superior_high, zones, zone_by, shells_mm, q, t,
                         label_zones, lung_zones, zone, zone_lung, shell, shell_lung)
 
-    def texture(self, image, mask, bin_width=25, spacing=None, classes=("glcm", "glszm"), gldm_alpha=0):
+    def texture(self, image, mask, bin_width=25, spacing=None, classes=("glcm", "glszm"), gldm_alpha=0, distances=(1,),
+                force2d=False, force2d_dimension=0, weighting_norm=None):
         """Grey-level texture features of `image` under `mask` -> lungmask_b200.texture.TextureFeatures, with the rows
         of `statistics`: every label value in the mask and every label 1..K-1 of the model (absent ones with 0 voxels and
         NaN features), then "lung" (mask > 0).  A row's ROI is its voxels with a non-NaN value, read in the volume's dtype
@@ -499,6 +500,16 @@ class LMInferer:
         number W of its neighbours in the row and the sum S of their levels; `ngtdm_counts` N(i, W) and `ngtdm_sums`
         A(i, W) = sum |W i - S|, (Ng, 27).  A bad `classes` or `gldm_alpha` raises before any kernel runs.
 
+        PyRadiomics' neighbourhood settings (DESIGN §4.18; the defaults give the matrices above): `distances`, a
+        collection of integers 1..3, and `force2d` with `force2d_dimension` (0, 1 or 2, the axis normal to the planes)
+        set the offsets O of texture.offsets.  GLCM then has one matrix per offset, `glcm_counts` (|O|, T); GLDM and
+        NGTDM use the K = 2 |O| neighbours v +- o, matrices (Ng, K + 1).  GLSZM ignores `distances` and with force2d
+        takes zones 8-connected within the planes; GLRLM ignores `distances` and with force2d uses the 4 in-plane
+        directions of the 13 (`glrlm_runs` directions index texture.Settings.run_offsets()).  `weighting_norm` ("manhattan",
+        "euclidean", "infinity", "no_weighting" or None) merges the GLCM and GLRLM matrices with the weights of
+        texture.weights over the spacing before the features are computed once; a norm other than "no_weighting" needs
+        a spacing.  Bad settings raise before any kernel runs.
+
         `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image, CPU tensors, or CUDA
         tensors on the engine's device read in place after the work queued on the current stream; both are left
         unchanged."""
@@ -508,8 +519,18 @@ class LMInferer:
         bw = tx.check_arguments(bin_width)
         classes = tx.check_classes(classes)
         alpha = tx.check_alpha(gldm_alpha)
+        settings = tx.check_settings(distances, force2d, force2d_dimension, weighting_norm)
         s = self._stage("texture", image, mask, spacing)
+        tx.check_weighting_spacing(settings, s.spacing)
         shape = tuple(s.mask.shape)
+        default = settings.default_neighbourhood()
+        offs = settings.offsets()
+        axis = settings.force2d_dimension
+        glcm_w = glrlm_w = None
+        if settings.weighting_norm is not None:
+            glcm_w = tx.weights(offs, settings.weighting_norm, s.spacing)
+            glrlm_w = tx.weights(settings.run_offsets(), settings.weighting_norm, s.spacing)
+        run_rows = [tx.OFFSETS.index(o) for o in settings.run_offsets()]
         st = self.engine.label_stats_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, (), (), stream=s.stream)
         present = set(int(x) for x in np.nonzero(st["voxels"][1:256])[0] + 1)
         rows = sorted(present | set(range(1, self.engine.n_classes[0]))) + [256]
@@ -524,24 +545,31 @@ class LMInferer:
         levels = torch.empty(shape, dtype=torch.uint8, device=s.mask.device) if plan else None
         for r in rows:
             if r not in plan:
-                out.append(tx.build_row(r, names[r], 0, bw, classes=classes))
+                out.append(tx.build_row(r, names[r], 0, bw, classes=classes, columns=2 * len(offs) + 1))
                 continue
             n, low, ng = plan[r]
             self.engine.texture_levels_dev(s.vol.data_ptr(), s.dtype, s.mask.data_ptr(), shape, r, low, bw, ng,
                                            levels.data_ptr(), stream=s.stream)
             U = zones = runs = neighbours = None
             if "glcm" in classes:
-                U = self.engine.glcm_dev(levels.data_ptr(), shape, ng, stream=s.stream)
+                U = (self.engine.glcm_dev(levels.data_ptr(), shape, ng, stream=s.stream) if default else
+                     self.engine.glcm_offsets_dev(levels.data_ptr(), shape, ng, offs, stream=s.stream))
             if "glszm" in classes:
-                zones = tx.zones_from_native(self.engine.zone_sizes_dev(levels.data_ptr(), shape, stream=s.stream))
+                zones = tx.zones_from_native(
+                    self.engine.zone_sizes_dev(levels.data_ptr(), shape, stream=s.stream) if axis is None else
+                    self.engine.zone_sizes_plane_dev(levels.data_ptr(), shape, axis, stream=s.stream))
             if "glrlm" in classes:
                 runs = self.engine.glrlm_dev(levels.data_ptr(), shape, ng, stream=s.stream)
+                if axis is not None:
+                    runs = runs[run_rows]
             if "gldm" in classes or "ngtdm" in classes:
                 # |level difference| <= ng - 1 always, so a larger alpha counts the same neighbours
-                neighbours = self.engine.neighbour_counts_dev(levels.data_ptr(), shape, ng, min(alpha, tx.MAX_LEVELS),
-                                                              stream=s.stream)
-            out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones, classes, runs, neighbours))
-        return tx.TextureFeatures(s.spacing, bw, out, classes, alpha)
+                a = min(alpha, tx.MAX_LEVELS)
+                neighbours = (self.engine.neighbour_counts_dev(levels.data_ptr(), shape, ng, a, stream=s.stream) if default
+                              else self.engine.neighbour_offsets_dev(levels.data_ptr(), shape, ng, offs, a, stream=s.stream))
+            out.append(tx.build_row(r, names[r], n, bw, low, ng, U, zones, classes, runs, neighbours, glcm_w, glrlm_w,
+                                    2 * len(offs) + 1))
+        return tx.TextureFeatures(s.spacing, bw, out, classes, alpha, settings)
 
     def first_order(self, image, mask, bin_width=25, spacing=None, voxel_array_shift=0):
         """PyRadiomics' 18 default first-order features of `image` under `mask` -> lungmask_b200.first_order.
@@ -915,7 +943,7 @@ class LMInferer:
 
     def wavelet_features(self, image, mask, wavelet="coif1", bin_width=25,
                          classes=("firstorder", "glcm", "glszm", "glrlm", "gldm", "ngtdm"), gldm_alpha=0, spacing=None,
-                         voxel_array_shift=0):
+                         voxel_array_shift=0, distances=(1,), force2d=False, force2d_dimension=0, weighting_norm=None):
         """The first-order and texture features of every wavelet decomposition of `image` under `mask` ->
         lungmask_b200.wavelet.WaveletFeatures: for each of the 8 decompositions of `wavelet` (see `wavelet`), in
         PyRadiomics' order, the FirstOrderFeatures of `first_order` and the TextureFeatures of `texture` run on that
@@ -926,8 +954,9 @@ class LMInferer:
         positive integer, or a dict giving one for every decomposition name ("wavelet-LLL" or "LLL"): wavelet-LLL scales
         values by about 2.8, so it may need a wider bin.  Every decomposition's rows are discretised before any
         first-order or texture kernel runs; a row with more than 255 levels is a ValueError naming the decomposition, the
-        row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`: as for `texture` and
-        `first_order`.  Bad arguments raise before any kernel runs.
+        row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`, and the neighbourhood settings
+        `distances`, `force2d`, `force2d_dimension` and `weighting_norm`: as for `texture` and `first_order`.  Bad
+        arguments raise before any kernel runs.
 
         `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the
         spacing), CPU tensors, or CUDA tensors on the engine's device read in place after the work queued on the current
@@ -941,7 +970,10 @@ class LMInferer:
         first, texture_classes = wv.check_classes(classes)
         alpha = tx.check_alpha(gldm_alpha)
         shift = fo.check_shift(voxel_array_shift)
+        settings = tx.check_settings(distances, force2d, force2d_dimension, weighting_norm)
         s = self._stage("wavelet_features", image, mask, spacing)
+        if texture_classes:
+            tx.check_weighting_spacing(settings, s.spacing)
         shape = wv.check_shape(s.vol.shape, wavelet)
         band = torch.empty(shape, dtype=torch.float64, device=s.mask.device)
 
@@ -950,17 +982,18 @@ class LMInferer:
                                     stream=s.stream)
 
         out = self._image_features("wavelet_features", s, band, wv.NAMES, compute, widths, first, texture_classes, shift,
-                                   alpha)
+                                   alpha, settings)
         computed = (("firstorder",) if first else ()) + texture_classes
         return wv.WaveletFeatures(wavelet, computed, s.spacing, shift, alpha, out)
 
-    def _image_features(self, what, s, image, names, compute, widths, first, texture_classes, shift, alpha):
+    def _image_features(self, what, s, image, names, compute, widths, first, texture_classes, shift, alpha, settings):
         """The feature loop of wavelet_features and filtered_features over the derived images `names`: compute(name)
         writes image `name` to the float64 device tensor `image` of the staged volume's shape.  Every image's rows
         (those of `statistics`) are discretised first with §4.9's rule, so that a row with more than 255 levels is a
         ValueError naming the image, the row and a sufficient bin width before any first-order or texture kernel runs;
-        then each image is recomputed and `first_order` (when `first`) and `texture` (on `texture_classes`) run on it
-        with the staged mask.  -> [wavelet.ImageFeatures] in the order of `names`."""
+        then each image is recomputed and `first_order` (when `first`) and `texture` (on `texture_classes`, with the
+        texture.Settings `settings`) run on it with the staged mask.  -> [wavelet.ImageFeatures] in the order of
+        `names`."""
         from . import texture as tx
         from . import wavelet as wv
         from .statistics import label_name
@@ -984,7 +1017,9 @@ class LMInferer:
             if first:
                 d.first_order = self.first_order(image, s.mask, widths[name], s.spacing, shift)
             if texture_classes:
-                d.texture = self.texture(image, s.mask, widths[name], s.spacing, texture_classes, alpha)
+                d.texture = self.texture(image, s.mask, widths[name], s.spacing, texture_classes, alpha, settings.distances,
+                                         settings.force2d_dimension is not None, settings.force2d_dimension or 0,
+                                         settings.weighting_norm)
             out.append(d)
         return out
 
@@ -1056,7 +1091,8 @@ class LMInferer:
 
     def filtered_features(self, image, mask, image_types=None, bin_width=25,
                           classes=("firstorder", "glcm", "glszm", "glrlm", "gldm", "ngtdm"), gldm_alpha=0, spacing=None,
-                          voxel_array_shift=0, gradient_use_spacing=True):
+                          voxel_array_shift=0, gradient_use_spacing=True, distances=(1,), force2d=False, force2d_dimension=0,
+                          weighting_norm=None):
         """The first-order and texture features of PyRadiomics' Square, SquareRoot, Logarithm, Exponential and Gradient
         image types of `image` under `mask` -> lungmask_b200.filters.FilteredFeatures: for each image type of
         `image_types` (None for all 5; see `filtered`), in PyRadiomics' order, the FirstOrderFeatures of `first_order`
@@ -1066,8 +1102,9 @@ class LMInferer:
         `classes`: a non-empty collection of "firstorder", "glcm", "glszm", "glrlm", "gldm" and "ngtdm".  `bin_width`: a
         positive integer, or a dict giving one for every requested image type.  Every image's rows are discretised
         before any first-order or texture kernel runs; a row with more than 255 levels is a ValueError naming the image
-        type, the row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`: as for `texture` and
-        `first_order`; the spacing is also the gradient's (see `filtered`).  Bad arguments raise before any kernel runs.
+        type, the row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`, and the neighbourhood
+        settings `distances`, `force2d`, `force2d_dimension` and `weighting_norm`: as for `texture` and `first_order`;
+        the spacing is also the gradient's (see `filtered`).  Bad arguments raise before any kernel runs.
 
         `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the
         spacing), CPU tensors, or CUDA tensors on the engine's device read in place after the work queued on the current
@@ -1081,11 +1118,14 @@ class LMInferer:
         first, texture_classes = flt.check_classes(classes)
         alpha = tx.check_alpha(gldm_alpha)
         shift = fo.check_shift(voxel_array_shift)
+        settings = tx.check_settings(distances, force2d, force2d_dimension, weighting_norm)
         s = self._stage("filtered_features", image, mask, spacing)
+        if texture_classes:
+            tx.check_weighting_spacing(settings, s.spacing)
         compute = self._filter_plan(s, names, s.spacing, gradient_use_spacing)
         image_buf = torch.empty(tuple(s.vol.shape), dtype=torch.float64, device=s.mask.device)
         out = self._image_features("filtered_features", s, image_buf, names, lambda n: compute(n, image_buf), widths,
-                                   first, texture_classes, shift, alpha)
+                                   first, texture_classes, shift, alpha, settings)
         computed = (("firstorder",) if first else ()) + texture_classes
         return flt.FilteredFeatures(computed, s.spacing, shift, alpha, bool(gradient_use_spacing), out)
 
