@@ -419,6 +419,38 @@ LM_API int lm_image_filter_dev(lm_engine* e, const void* d_vol, int dtype, int n
 LM_API int lm_gradient_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, const double* spacing_xyz,
                            double* d_out, void* stream);
 
+/* Resampling (no counterpart in the reference; DESIGN §4.19): PyRadiomics' resampleImage with the sitkBSpline or
+ * sitkNearestNeighbor interpolator, for LMInferer.resample.  Both calls take the (n0,n1,n2) volume d_vol (every
+ * LM_DTYPE_* code; bool as LM_DTYPE_U8), fewer than 2^32 voxels, device memory of the engine's device and the caller's
+ * cudaStream_t with the event-wait rule of lm_apply_dev; every argument is checked before any kernel runs and the call
+ * returns after the engine's stream has synchronised.  Work area: one flag.
+ * lm_bspline_coefficients_dev writes the cubic B-spline coefficients (mirror boundaries, pole z = sqrt(3) - 2) of the
+ *   volume, converted to float64, to the float64 (n0,n1,n2) d_coeff (not overlapping d_vol): the 1-D decomposition along
+ *   array axis 2 (x), then 1 (y), then 0 (z); per line of N > 1 samples: times (1 - z)(1 - 1/z); c[0] = c[0] +
+ *   sum_{n=1..17} z^n c[n] (N >= 19) or Thevenaz's full mirror sum (N <= 18, z^(N-1) formed by repeated products);
+ *   c[n] += z c[n-1]; c[N-1] = (z / (z z - 1)) (z c[N-2] + c[N-1]); c[n] = z (c[n+1] - c[n]); each product, sum and the
+ *   one division rounded to float64 on its own, with no fused multiply-add.  A NaN or +-inf anywhere in the volume
+ *   returns LM_ERR_NONFINITE (d_coeff is then not the coefficients).
+ * lm_resample_dev samples the volume at the (m0,m1,m2) points (d_cz[k0], d_cy[k1], d_cx[k2]) of the input's continuous
+ *   index (device float64 tables [m0], [m1], [m2], finite, fewer than 2^32 points): a point with c < -0.5 or
+ *   c >= N - 0.5 along any axis gets 0 in d_out and d_out_mask.  d_out_mask (m0,m1,m2) uint8 gets the uint8 (n0,n1,n2)
+ *   d_mask at floor(c + 0.5) of each axis (clamped to [0, N - 1]); d_out (m0,m1,m2) of `dtype` gets, under
+ *   LM_RESAMPLE_NEAREST, d_vol at that voxel, and under LM_RESAMPLE_BSPLINE the cubic B-spline of d_coeff (the output of
+ *   lm_bspline_coefficients_dev for d_vol): per axis w = c - floor(c), w3 = w^3 / 6, w0 = 1/6 + w (w - 1) / 2 - w3,
+ *   w2 = w + w0 - 2 w3, w1 = 1 - w0 - w2 - w3 on the indices floor(c) - 1 .. floor(c) + 2 mirrored with period 2N - 2
+ *   (0 when N = 1), the 64 taps summed x innermost, then y, then z, each sum from +0.0, rounded as above.  The value is
+ *   stored in `dtype`: integers clamped to the type's range (int64: to 2^63 - 1024) and truncated toward zero, float32 and
+ *   float16 rounded to nearest, bfloat16 rounded to float32 and then to bfloat16, float64 kept.  d_coeff is not read
+ *   (and may be NULL) under LM_RESAMPLE_NEAREST.  The outputs must not overlap each other or any input.  A sampled value
+ *   that is a NaN or +-inf returns LM_ERR_NONFINITE. */
+#define LM_RESAMPLE_BSPLINE 0
+#define LM_RESAMPLE_NEAREST 1
+LM_API int lm_bspline_coefficients_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, double* d_coeff,
+                                       void* stream);
+LM_API int lm_resample_dev(lm_engine* e, const void* d_vol, int dtype, const double* d_coeff, const uint8_t* d_mask, int n0,
+                           int n1, int n2, const double* d_cz, const double* d_cy, const double* d_cx, int m0, int m1,
+                           int m2, int interpolator, void* d_out, uint8_t* d_out_mask, void* stream);
+
 /* Voxel-based first-order feature maps (no counterpart in the reference; DESIGN §4.15): PyRadiomics' voxel-based
  * firstorder extraction of one row, for LMInferer.first_order_maps.  Device memory of the engine's device and the
  * caller's cudaStream_t with the event-wait rule of lm_apply_dev; every argument is checked before any kernel runs and

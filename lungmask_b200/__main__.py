@@ -21,6 +21,9 @@ row, one image per feature with the input's geometry (LMInferer.first_order_maps
 GLCM feature maps the same way (LMInferer.glcm_maps), and `--texture-maps DIR` its voxel-based GLSZM, GLRLM, GLDM and
 NGTDM feature maps (LMInferer.texture_maps).  `--texture-distances`, `--texture-force2d` and `--texture-weighting-norm`
 set PyRadiomics' distances, force2D and weightingNorm for the texture matrices of --texture, --wavelet and --filtered.
+`--resample X,Y,Z` resamples the image and the mask once after segmentation to that spacing in mm (PyRadiomics'
+resampledPixelSpacing, `--resample-interpolator` bspline or nearest; LMInferer.resample), and --texture, --shape,
+--first-order, --wavelet and --filtered then run on the resampled pair; the other analyses stay on the native grid.
 """
 import argparse
 import os
@@ -187,7 +190,34 @@ def build_parser():
                         "maskedKernel=False)")
     p.add_argument("--texture-maps-format", choices=["nii.gz", "nii", "mha", "npy"], default="nii.gz",
                    help="File format of --texture-maps (default nii.gz)")
+    p.add_argument("--resample", metavar="X,Y,Z", type=str, default=None,
+                   help="Resample the image and the mask to this spacing in mm (0 keeps an axis; PyRadiomics' "
+                        "resampledPixelSpacing) before --texture, --shape, --first-order, --wavelet and --filtered. "
+                        "--statistics, --clusters, --regions, --mesh and the feature maps stay on the native grid")
+    p.add_argument("--resample-interpolator", choices=["bspline", "nearest"], default=None,
+                   help="Image interpolator of --resample: cubic B-spline (sitkBSpline, default) or nearest neighbour; "
+                        "the mask is always resampled by nearest neighbour")
     return p
+
+
+RESAMPLED_ANALYSES = ("texture", "shape", "first_order", "wavelet", "filtered")   # the flags --resample applies to
+
+
+def resample_arguments(args):
+    """-> (resampled spacing (x, y, z), interpolator) of --resample, or None without it; exits with a message naming the
+    flag for a bad value."""
+    from .resample import parse_spacing
+    if args.resample is None:
+        if args.resample_interpolator is not None:
+            sys.exit("--resample-interpolator: needs --resample")
+        return None
+    try:
+        spacing = parse_spacing(args.resample)
+    except ValueError as ex:
+        sys.exit("--resample: %s" % ex)
+    if all(getattr(args, a) is None for a in RESAMPLED_ANALYSES):
+        sys.exit("--resample: applies to --texture, --shape, --first-order, --wavelet and --filtered, and none is given")
+    return spacing, args.resample_interpolator or "bspline"
 
 
 def texture_settings_arguments(args):
@@ -373,6 +403,7 @@ def main(argv=None):
         glcm_label, glcm_features = glcm_maps_arguments(args)
     if args.texture_maps is not None:
         tmaps_label, tmaps_classes, tmaps_features = texture_maps_arguments(args)
+    resampling = resample_arguments(args)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
     image = load_input_image(args.input, disable_tqdm=args.noprogress, read_metadata=not args.removemetadata)
@@ -405,25 +436,30 @@ def main(argv=None):
     if args.regions is not None:
         logger.info(f"Save regional statistics to: {args.regions}")
         save_regional_statistics(args.regions, inferer.regional_statistics(image, result))
+    feature_image, feature_mask = image, result   # the pair of --texture, --shape, --first-order, --wavelet, --filtered
+    if resampling is not None:
+        logger.info("Resample to %s mm (%s)" % (",".join("%g" % v for v in resampling[0]), resampling[1]))
+        r = inferer.resample(image, result, resampled_spacing=resampling[0], interpolator=resampling[1])
+        feature_image, feature_mask = r.volume(), r.mask
     if args.texture is not None:
         logger.info(f"Save texture features to: {args.texture}")
-        save_texture(args.texture, inferer.texture(image, result, bin_width=args.texture_bin_width, classes=texture_classes,
+        save_texture(args.texture, inferer.texture(feature_image, feature_mask, bin_width=args.texture_bin_width, classes=texture_classes,
                                                            **settings))
     if args.shape is not None:
         logger.info(f"Save shape features to: {args.shape}")
-        save_shape(args.shape, inferer.shape(result, image=image))
+        save_shape(args.shape, inferer.shape(feature_mask, image=feature_image))
     if args.first_order is not None:
         logger.info(f"Save first-order features to: {args.first_order}")
-        save_first_order(args.first_order, inferer.first_order(image, result, bin_width=args.first_order_bin_width,
+        save_first_order(args.first_order, inferer.first_order(feature_image, feature_mask, bin_width=args.first_order_bin_width,
                                                                voxel_array_shift=args.first_order_shift))
     if args.wavelet is not None:
         logger.info(f"Save wavelet features to: {args.wavelet}")
-        save_wavelet_features(args.wavelet, inferer.wavelet_features(image, result, wavelet=args.wavelet_name,
+        save_wavelet_features(args.wavelet, inferer.wavelet_features(feature_image, feature_mask, wavelet=args.wavelet_name,
                                                                      bin_width=wavelet_bin_width, classes=wavelet_classes,
                                                                      **settings))
     if args.filtered is not None:
         logger.info(f"Save filtered-image features to: {args.filtered}")
-        save_filtered_features(args.filtered, inferer.filtered_features(image, result, image_types=filtered_types,
+        save_filtered_features(args.filtered, inferer.filtered_features(feature_image, feature_mask, image_types=filtered_types,
                                                                         bin_width=filtered_bin_width,
                                                                         classes=filtered_classes, **settings))
     if args.mesh is not None:

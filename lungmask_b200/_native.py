@@ -17,6 +17,7 @@ FILTER_CODES = {"square": 0, "squareroot": 1, "logarithm": 2, "exponential": 3} 
 ERR_TABLE_RANGE = -42                     # LM_ERR_TABLE_RANGE
 MESH_RAS = 1                              # LM_MESH_RAS of lm_mesh_emit_dev
 FOM_FLOAT, FOM_EXACT = 1, 2               # LM_FOM_* modes of lm_first_order_maps_dev
+RESAMPLE_CODES = {"bspline": 0, "nearest": 1}   # LM_RESAMPLE_* of lm_resample_dev
 
 _lib = None
 
@@ -83,6 +84,8 @@ def lib():
         "lm_image_range_dev": ([vp, vp, i32, i32, i32, i32, vp, vp], i32),
         "lm_image_filter_dev": ([vp, vp, i32, i32, i32, i32, i32, vp, vp, C.c_int64, C.c_int64, vp, vp], i32),
         "lm_gradient_dev": ([vp, vp, i32, i32, i32, i32, vp, vp, vp], i32),
+        "lm_bspline_coefficients_dev": ([vp, vp, i32, i32, i32, i32, vp, vp], i32),
+        "lm_resample_dev": ([vp, vp, i32, vp, u8p, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp, u8p, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -113,7 +116,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_glcm_offsets_dev", "lm_neighbour_offsets_dev", "lm_zone_sizes_plane_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_glcm_offsets_dev", "lm_neighbour_offsets_dev", "lm_zone_sizes_plane_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_bspline_coefficients_dev", "lm_resample_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -630,6 +633,41 @@ class Engine:
         rc = lib().lm_gradient_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2, _ptr(sp),
                                    C.c_void_p(d_out_ptr), C.c_void_p(int(stream)) if stream else None)
         _filter_check(rc, "gradient")
+
+    # ---- resampling (lm_bspline_coefficients_dev, lm_resample_dev)
+    @staticmethod
+    def _resample_check(rc, what):
+        """ValueError for an argument refused by the call or a NaN or +-inf; NativeError for a CUDA failure."""
+        if rc in (-1, ERR_NONFINITE):
+            raise ValueError("%s: %s" % (what, lib().lm_last_error().decode()))
+        _check(rc)
+
+    def bspline_coefficients_dev(self, d_vol_ptr, dtype_code, shape, d_coeff_ptr, stream=0):
+        """Writes the float64 cubic B-spline coefficients (mirror boundaries) of a C-contiguous `shape` device volume of
+        element type `dtype_code` to the float64 `shape` device buffer `d_coeff_ptr` (`stream` as for apply_dev).
+        ValueError for a refused argument or a NaN or +-inf in the volume; NativeError for the other failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        rc = lib().lm_bspline_coefficients_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2,
+                                               C.c_void_p(d_coeff_ptr), C.c_void_p(int(stream)) if stream else None)
+        self._resample_check(rc, "bspline_coefficients")
+
+    def resample_dev(self, d_vol_ptr, dtype_code, d_coeff_ptr, d_mask_ptr, shape, d_tables, out_shape, interpolator,
+                     d_out_ptr, d_out_mask_ptr, stream=0):
+        """Samples a C-contiguous `shape` device volume (element type `dtype_code`) and its uint8 mask on the `out_shape`
+        grid of the device float64 tables d_tables = (c_z, c_y, c_x) pointers: the image into `d_out_ptr` (the volume's
+        dtype) from the coefficients `d_coeff_ptr` ("bspline") or the volume ("nearest"), the mask into the uint8
+        `d_out_mask_ptr`.  ValueError for a refused argument or a NaN or +-inf sample; NativeError for the other
+        failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        m0, m1, m2 = (int(x) for x in out_shape)
+        if interpolator not in RESAMPLE_CODES:
+            raise ValueError("resample_dev: unknown interpolator %r (known: %s)" % (interpolator, ", ".join(RESAMPLE_CODES)))
+        cz, cy, cx = (C.c_void_p(int(p)) for p in d_tables)
+        rc = lib().lm_resample_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), C.c_void_p(d_coeff_ptr or None),
+                                   C.c_void_p(d_mask_ptr), n0, n1, n2, cz, cy, cx, m0, m1, m2, RESAMPLE_CODES[interpolator],
+                                   C.c_void_p(d_out_ptr), C.c_void_p(d_out_mask_ptr),
+                                   C.c_void_p(int(stream)) if stream else None)
+        self._resample_check(rc, "resample")
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

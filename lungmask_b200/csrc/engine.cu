@@ -29,6 +29,7 @@
 #include "first_order_maps.cuh"
 #include "glcm_maps.cuh"
 #include "texture_maps.cuh"
+#include "resample.cuh"
 
 using namespace lm;
 
@@ -213,6 +214,7 @@ struct lm_engine {
   FomWork fo_maps;              // lm_first_order_maps_dev: the error flag
   GlcmMapsWork glcm_maps;       // lm_glcm_maps_dev: the error flag
   TextureMapsWork texture_maps; // lm_texture_maps_dev: the error flag
+  ResampleWork resample;        // lm_bspline_coefficients_dev, lm_resample_dev: the non-finite flag
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -946,6 +948,7 @@ void lm_destroy(lm_engine* e) {
   e->fo_maps.release();
   e->glcm_maps.release();
   e->texture_maps.release();
+  e->resample.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1644,6 +1647,63 @@ int lm_gradient_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, 
   if (overlaps(d_vol, n * dtype_bytes(dtype), d_out, n * sizeof(double))) return fail(-1, "%s: d_out overlaps d_vol", fn);
   RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_out", d_out}}));
   return filter_result(fn, gradient_magnitude(e->filters, d_vol, dtype, n0, n1, n2, inv, d_out, e->st, &e->launches));
+}
+
+int lm_bspline_coefficients_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2, double* d_coeff,
+                                void* stream) {
+  static const char* fn = "lm_bspline_coefficients_dev";
+  RC(filter_volume_args(fn, e, d_vol, dtype, n0, n1, n2));
+  if (!d_coeff) return fail(-1, "%s: NULL argument", fn);
+  const size_t n = (size_t)n0 * n1 * n2;
+  if (overlaps(d_vol, n * dtype_bytes(dtype), d_coeff, n * sizeof(double)))
+    return fail(-1, "%s: d_coeff overlaps d_vol", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_coeff", d_coeff}}));
+  return filter_result(fn, bspline_coefficients(e->resample, d_vol, dtype, n0, n1, n2, d_coeff, e->st, &e->launches));
+}
+
+int lm_resample_dev(lm_engine* e, const void* d_vol, int dtype, const double* d_coeff, const uint8_t* d_mask, int n0, int n1,
+                    int n2, const double* d_cz, const double* d_cy, const double* d_cx, int m0, int m1, int m2,
+                    int interpolator, void* d_out, uint8_t* d_out_mask, void* stream) {
+  static const char* fn = "lm_resample_dev";
+  RC(filter_volume_args(fn, e, d_vol, dtype, n0, n1, n2));
+  if (!d_mask || !d_cz || !d_cy || !d_cx || !d_out || !d_out_mask) return fail(-1, "%s: NULL argument", fn);
+  if (interpolator != LM_RESAMPLE_BSPLINE && interpolator != LM_RESAMPLE_NEAREST)
+    return fail(-1, "%s: unknown interpolator code %d", fn, interpolator);
+  if (interpolator == LM_RESAMPLE_BSPLINE && !d_coeff) return fail(-1, "%s: NULL d_coeff for the B-spline", fn);
+  if (m0 < 1 || m1 < 1 || m2 < 1) return fail(-1, "%s: empty output grid (%d,%d,%d)", fn, m0, m1, m2);
+  const size_t n = (size_t)n0 * n1 * n2, m = (size_t)m0 * m1 * m2;
+  if (m >= ((size_t)1 << 32)) return fail(-1, "%s: %zu output voxels, the call takes fewer than 2^32", fn, m);
+  const size_t out_bytes = m * dtype_bytes(dtype);
+  const struct { const char* name; const void* p; size_t bytes; } ins[] = {
+      {"d_vol", d_vol, n * dtype_bytes(dtype)},
+      {"d_coeff", interpolator == LM_RESAMPLE_BSPLINE ? d_coeff : nullptr, n * sizeof(double)},
+      {"d_mask", d_mask, n},
+      {"d_cz", d_cz, (size_t)m0 * sizeof(double)},
+      {"d_cy", d_cy, (size_t)m1 * sizeof(double)},
+      {"d_cx", d_cx, (size_t)m2 * sizeof(double)}};
+  for (const auto& a : ins) {
+    if (!a.p) continue;
+    if (overlaps(a.p, a.bytes, d_out, out_bytes)) return fail(-1, "%s: d_out overlaps %s", fn, a.name);
+    if (overlaps(a.p, a.bytes, d_out_mask, m)) return fail(-1, "%s: d_out_mask overlaps %s", fn, a.name);
+  }
+  if (overlaps(d_out, out_bytes, d_out_mask, m)) return fail(-1, "%s: d_out_mask overlaps d_out", fn);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_coeff", ins[1].p}, {"d_mask", d_mask}, {"d_cz", d_cz},
+                                     {"d_cy", d_cy}, {"d_cx", d_cx}, {"d_out", d_out}, {"d_out_mask", d_out_mask}}));
+  // the tables are checked on the host: the engine's stream has waited for the caller's, so they are complete
+  std::vector<double> tab((size_t)m0 + m1 + m2);
+  CU(cudaMemcpyAsync(tab.data(), d_cz, (size_t)m0 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  CU(cudaMemcpyAsync(tab.data() + m0, d_cy, (size_t)m1 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  CU(cudaMemcpyAsync(tab.data() + m0 + m1, d_cx, (size_t)m2 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  CU(cudaStreamSynchronize(e->st));
+  for (size_t k = 0; k < tab.size(); ++k)
+    if (!isfinite(tab[k])) {
+      const char* t = k < (size_t)m0 ? "d_cz" : (k < (size_t)m0 + m1 ? "d_cy" : "d_cx");
+      return fail(-1, "%s: %s holds a NaN or +-inf", fn, t);
+    }
+  const int rc = resample_volume(e->resample, d_vol, dtype, d_coeff, d_mask, n0, n1, n2, d_cz, d_cy, d_cx, m0, m1, m2,
+                                 interpolator, d_out, d_out_mask, e->st, &e->launches);
+  if (rc == LM_ERR_NONFINITE) return fail(rc, "%s: a sampled value is a NaN or +-inf", fn);
+  return rc;
 }
 
 int lm_first_order_maps_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,

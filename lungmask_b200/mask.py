@@ -1129,6 +1129,77 @@ class LMInferer:
         computed = (("firstorder",) if first else ()) + texture_classes
         return flt.FilteredFeatures(computed, s.spacing, shift, alpha, bool(gradient_use_spacing), out)
 
+    def resample(self, image, mask, resampled_spacing=(1, 1, 1), spacing=None, interpolator="bspline", pad_distance=5):
+        """PyRadiomics' resampling of `image` and `mask` to `resampled_spacing` (x, y, z) mm (resampledPixelSpacing; an
+        entry of 0 keeps that axis) with interpolator "bspline" (sitkBSpline, the default) or "nearest"
+        (sitkNearestNeighbor) for the image and nearest neighbour for the mask -> lungmask_b200.resample.Resampled.  The
+        grid covers the bounding box of mask > 0 padded by `pad_distance` output voxels, clamped to the image; when the
+        spacing already equals the request (np.allclose) the pair is only cropped.  Points outside the input are 0.  The
+        image keeps its dtype (integers clamped, then truncated toward zero) and the mask comes back as uint8;
+        lungmask_b200.resample.resample_host is the numpy statement, and the result equals it bit for bit (DESIGN
+        §4.19).  The result goes straight into the feature calls:
+            r = inferer.resample(image, mask); inferer.texture(r.image, r.mask, spacing=r.spacing)
+
+        `image` and `mask` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the spacing
+        unless `spacing` is given, and makes the result carry the new origin and the direction), CPU tensors, or CUDA
+        tensors on the engine's device read in place after the work queued on the current stream; the image comes back
+        in the same kind and neither input is modified.  The array is taken as given (no reorientation) and the mask
+        must lie on the image's grid.  A NaN or +-inf in the image, an empty mask, a bad spacing or pad, mismatched
+        shapes and 2^32 or more input or output voxels are a ValueError before any image is written.  The B-spline holds
+        one float64 coefficient volume of the input's size on the device during the call."""
+        import torch
+        from . import resample as rsm
+        rsm.check_interpolator(interpolator)
+        pad = rsm.check_pad(pad_distance)
+        requested = rsm.check_resampled_spacing(resampled_spacing)
+        if _is_tensor(image):
+            src_dtype = None
+            is_bool = image.dtype == torch.bool
+        else:   # a numpy array's or a Volume's dtype; a SimpleITK image is read as staged
+            src_dtype = image.dtype if isinstance(image, np.ndarray) else getattr(getattr(image, "array", None), "dtype", None)
+            is_bool = src_dtype == np.bool_
+        if is_bool:
+            raise TypeError("resample: a bool image has no interpolation; give the image as uint8 or pass it as the mask")
+        s = self._stage("resample", image, mask, spacing)
+        ms = rsm.check_spacing(s.spacing)
+        shape = rsm.check_shape(s.vol.shape)
+        counts = [self.engine.plane_label_counts_dev(s.mask.data_ptr(), shape, axis, stream=s.stream)[:, 256]
+                  for axis in (2, 1, 0)]
+        g = rsm.grid(shape, ms, requested, *rsm.bounding_box_of_counts(counts), pad)
+        interp = "nearest" if g.crop else interpolator
+        device = s.vol.device
+        tables = [torch.from_numpy(t).to(device) for t in g.tables[::-1]]   # c_z, c_y, c_x
+        coeff = None
+        if interp == "bspline":
+            coeff = torch.empty(shape, dtype=torch.float64, device=device)
+            self.engine.bspline_coefficients_dev(s.vol.data_ptr(), s.dtype, shape, coeff.data_ptr(), stream=s.stream)
+        elif s.vol.dtype.is_floating_point:
+            self.engine.image_range_dev(s.vol.data_ptr(), s.dtype, shape, stream=s.stream)   # refuses a NaN or +-inf
+        out = torch.empty(g.shape, dtype=s.vol.dtype, device=device)
+        out_mask = torch.empty(g.shape, dtype=torch.uint8, device=device)
+        self.engine.resample_dev(s.vol.data_ptr(), s.dtype, coeff.data_ptr() if coeff is not None else None,
+                                 s.mask.data_ptr(), shape, [t.data_ptr() for t in tables], g.shape, interp, out.data_ptr(),
+                                 out_mask.data_ptr(), stream=s.stream)
+        del coeff
+        img, m = out, out_mask
+        if not (_is_tensor(image) and image.is_cuda):
+            img, m = img.cpu(), m.cpu()
+            if _is_tensor(image):
+                if image.dtype == torch.bfloat16:   # staged as float32: the float32 value rounded once more
+                    img = img.to(torch.bfloat16)
+            else:
+                img = img.numpy()
+                if src_dtype in (np.uint16, np.uint32):   # staged as int32 / int64: the same values clamped once more
+                    img = rsm.cast_host(img, src_dtype)
+            if not _is_tensor(mask):
+                m = m.numpy()
+        origin = direction = None
+        if not isinstance(image, np.ndarray) and not _is_tensor(image):
+            origin = tuple(image.origin) if hasattr(image, "origin") else tuple(image.GetOrigin())
+            direction = tuple(image.GetDirection())
+            origin = rsm.new_origin(origin, direction, ms, g.start)
+        return rsm.Resampled(img, m, g.spacing, g.start, origin, direction)
+
     def _stage(self, what, image, mask, spacing=None, mask_only=False, image_only=False):
         """The inputs of an analysis call as contiguous tensors on the engine's device -> _Staged.  CUDA tensors must be on
         the engine's device and are read in place; a CUDA volume needs a CUDA mask and the reverse.  Everything else is
