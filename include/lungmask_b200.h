@@ -451,6 +451,26 @@ LM_API int lm_resample_dev(lm_engine* e, const void* d_vol, int dtype, const dou
                            int n1, int n2, const double* d_cz, const double* d_cy, const double* d_cx, int m0, int m1,
                            int m2, int interpolator, void* d_out, uint8_t* d_out_mask, void* stream);
 
+/* Laplacian of Gaussian (no counterpart in the reference; DESIGN §4.20): PyRadiomics' LoG image type, ITK's
+ * LaplacianRecursiveGaussianImageFilter with NormalizeAcrossScale, for LMInferer.log_images.  The (n0,n1,n2) volume d_vol
+ * (every LM_DTYPE_* code; bool as LM_DTYPE_U8; converted to float64), every extent >= 4 and fewer than 2^32 voxels, device
+ * memory of the engine's device and the caller's cudaStream_t with the event-wait rule of lm_apply_dev; every argument
+ * is checked before any kernel runs and the call returns after the engine's stream has synchronised.  Work area: one
+ * flag, and the caller's d_work0 and d_work1, float64 (n0,n1,n2) volumes.
+ * spacing_xyz: 3 finite positive sizes in mm (x = array axis 2, y = 1, z = 0); sigma_mm finite and > 0, with every axis
+ * d holding at least ceil(sigma_mm / spacing_xyz[d]) + 1 voxels.  The engine forms the coefficients itself, per axis
+ * with sd = sigma_mm / spacing_xyz[d], by the float64 operations of lungmask_b200.laplacian.coefficients in the same
+ * order (libm sin, cos and exp; Deriche's constants; order 0 normalised to unit sum, order 2 to sd^2 times the second
+ * derivative).  d_out (n0,n1,n2) float64 gets, for d = x, y, z, the order-0 line filter along the two other axes in
+ * x, y, z order and then the order-2 line filter along d, the three terms summed from +0.0 in that order.  A line filter
+ * is the causal and anticausal 4th-order recursion of ITK's RecursiveSeparableImageFilter, the taps outside the line
+ * reading the end sample (rows in lungmask_b200/laplacian.py), every product and sum rounded to float64 on its own with
+ * no fused multiply-add: d_out equals lungmask_b200.laplacian.log_host bit for bit.  d_out, d_work0 and d_work1 must not
+ * overlap each other or d_vol.  A NaN or +-inf in the volume returns LM_ERR_NONFINITE (d_out is then not an image). */
+LM_API int lm_laplacian_of_gaussian_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2,
+                                        const double* spacing_xyz, double sigma_mm, double* d_work0, double* d_work1,
+                                        double* d_out, void* stream);
+
 /* Voxel-based first-order feature maps (no counterpart in the reference; DESIGN §4.15): PyRadiomics' voxel-based
  * firstorder extraction of one row, for LMInferer.first_order_maps.  Device memory of the engine's device and the
  * caller's cudaStream_t with the event-wait rule of lm_apply_dev; every argument is checked before any kernel runs and

@@ -14,16 +14,19 @@ LMInferer.texture), `--shape PATH` the mesh shape features
 deviations, energy, entropy, uniformity) of every label and the whole lung (.json / .csv, LMInferer.first_order), and
 `--wavelet PATH` the first-order and texture features of the 8 coif1 (or haar) wavelet decompositions (.json / .csv,
 LMInferer.wavelet_features), and `--filtered PATH` those of the Square, SquareRoot, Logarithm, Exponential and Gradient
-image types (.json / .csv, LMInferer.filtered_features), and `--mesh DIR` the marching-cubes surface of every present
+image types (.json / .csv, LMInferer.filtered_features), and `--log PATH` those of the LoG image type at each sigma of
+`--log-sigma` (.json / .csv, LMInferer.log_features), and `--mesh DIR` the marching-cubes surface of every present
 label and of the whole lung, one file per row (`--mesh-format` stl, obj or ply, `--mesh-space` lps or ras;
 LMInferer.mesh with the input's geometry), and `--first-order-maps DIR` the voxel-based first-order feature maps of one
 row, one image per feature with the input's geometry (LMInferer.first_order_maps), and `--glcm-maps DIR` its voxel-based
 GLCM feature maps the same way (LMInferer.glcm_maps), and `--texture-maps DIR` its voxel-based GLSZM, GLRLM, GLDM and
 NGTDM feature maps (LMInferer.texture_maps).  `--texture-distances`, `--texture-force2d` and `--texture-weighting-norm`
-set PyRadiomics' distances, force2D and weightingNorm for the texture matrices of --texture, --wavelet and --filtered.
+set PyRadiomics' distances, force2D and weightingNorm for the texture matrices of --texture, --wavelet, --filtered and
+--log.
 `--resample X,Y,Z` resamples the image and the mask once after segmentation to that spacing in mm (PyRadiomics'
 resampledPixelSpacing, `--resample-interpolator` bspline or nearest; LMInferer.resample), and --texture, --shape,
---first-order, --wavelet and --filtered then run on the resampled pair; the other analyses stay on the native grid.
+--first-order, --wavelet, --filtered and --log then run on the resampled pair; the other analyses stay on the native
+grid.
 """
 import argparse
 import os
@@ -31,7 +34,7 @@ import sys
 
 from .io import (check_probabilities_path, check_table_path, load_input_image, save_clusters, save_first_order, save_mask,
                  save_feature_maps, save_mesh, save_probabilities, save_regional_statistics, save_shape, save_statistics, save_texture,
-                 save_filtered_features, save_wavelet_features)
+                 save_filtered_features, save_log_features, save_wavelet_features)
 from .logger import logger
 from .mask import LMInferer
 
@@ -132,6 +135,19 @@ def build_parser():
     p.add_argument("--filtered-classes", metavar="NAMES", type=str, default="firstorder,glcm,glszm,glrlm,gldm,ngtdm",
                    help="Comma-separated feature classes of --filtered: any of firstorder, glcm, glszm, glrlm, gldm, "
                         "ngtdm (default all)")
+    p.add_argument("--log", metavar="PATH", type=str, default=None,
+                   help="Also write the first-order and texture features of PyRadiomics' LoG image type at each sigma of "
+                        "--log-sigma (keys such as log-sigma-1-0-mm-3D_firstorder_Mean) of every label and the whole "
+                        "lung: .json (with the exact sums and matrices) or .csv")
+    p.add_argument("--log-sigma", metavar="SIGMAS", type=str, default=None,
+                   help="Comma-separated sigmas of --log in mm, such as 1,2,3,4,5 (PyRadiomics' LoG sigma; required with "
+                        "--log)")
+    p.add_argument("--log-bin-width", metavar="SPEC", type=str, default="25",
+                   help="Fixed bin width of --log: one positive integer, or a default followed by per-sigma overrides "
+                        "such as 25,3.0=50 (default 25)")
+    p.add_argument("--log-classes", metavar="NAMES", type=str, default="firstorder,glcm,glszm,glrlm,gldm,ngtdm",
+                   help="Comma-separated feature classes of --log: any of firstorder, glcm, glszm, glrlm, gldm, ngtdm "
+                        "(default all)")
     p.add_argument("--mesh", metavar="DIR", type=str, default=None,
                    help="Also write the marching-cubes surface (the mesh of --shape, in patient space) of every present "
                         "label and of the whole lung to DIR, one file per row named after it (right_lung.stl, lung.stl)")
@@ -192,7 +208,7 @@ def build_parser():
                    help="File format of --texture-maps (default nii.gz)")
     p.add_argument("--resample", metavar="X,Y,Z", type=str, default=None,
                    help="Resample the image and the mask to this spacing in mm (0 keeps an axis; PyRadiomics' "
-                        "resampledPixelSpacing) before --texture, --shape, --first-order, --wavelet and --filtered. "
+                        "resampledPixelSpacing) before --texture, --shape, --first-order, --wavelet, --filtered and --log. "
                         "--statistics, --clusters, --regions, --mesh and the feature maps stay on the native grid")
     p.add_argument("--resample-interpolator", choices=["bspline", "nearest"], default=None,
                    help="Image interpolator of --resample: cubic B-spline (sitkBSpline, default) or nearest neighbour; "
@@ -200,7 +216,7 @@ def build_parser():
     return p
 
 
-RESAMPLED_ANALYSES = ("texture", "shape", "first_order", "wavelet", "filtered")   # the flags --resample applies to
+RESAMPLED_ANALYSES = ("texture", "shape", "first_order", "wavelet", "filtered", "log")   # the flags --resample applies to
 
 
 def resample_arguments(args):
@@ -216,8 +232,36 @@ def resample_arguments(args):
     except ValueError as ex:
         sys.exit("--resample: %s" % ex)
     if all(getattr(args, a) is None for a in RESAMPLED_ANALYSES):
-        sys.exit("--resample: applies to --texture, --shape, --first-order, --wavelet and --filtered, and none is given")
+        sys.exit("--resample: applies to --texture, --shape, --first-order, --wavelet, --filtered and --log, and none "
+                 "is given")
     return spacing, args.resample_interpolator or "bspline"
+
+
+def log_arguments(args):
+    """-> (sigmas, bin widths, classes) of --log, or None without it; exits with a message naming the flag for a bad
+    value."""
+    from . import laplacian
+    if args.log is None:
+        if args.log_sigma is not None:
+            sys.exit("--log-sigma: needs --log")
+        return None
+    check_table_path(args.log, "log")
+    if args.log_sigma is None:
+        sys.exit("--log: needs --log-sigma, such as --log-sigma 1,2,3,4,5 (PyRadiomics has no default sigma)")
+    try:
+        sigmas = laplacian.parse_sigmas(args.log_sigma)
+    except (TypeError, ValueError) as ex:
+        sys.exit("--log-sigma: %s" % ex)
+    try:
+        widths = laplacian.parse_bin_widths(args.log_bin_width, sigmas)
+    except (TypeError, ValueError) as ex:
+        sys.exit("--log-bin-width: %s" % ex)
+    classes = [c.strip() for c in args.log_classes.split(",") if c.strip()]
+    try:
+        laplacian.check_classes(classes)
+    except (TypeError, ValueError) as ex:
+        sys.exit("--log-classes: %s" % ex)
+    return sigmas, widths, classes
 
 
 def texture_settings_arguments(args):
@@ -403,6 +447,7 @@ def main(argv=None):
         glcm_label, glcm_features = glcm_maps_arguments(args)
     if args.texture_maps is not None:
         tmaps_label, tmaps_classes, tmaps_features = texture_maps_arguments(args)
+    log = log_arguments(args)
     resampling = resample_arguments(args)
     batchsize = 1 if args.cpu else args.batchsize  # __main__.py:81-83
     logger.info("Load model")
@@ -436,7 +481,7 @@ def main(argv=None):
     if args.regions is not None:
         logger.info(f"Save regional statistics to: {args.regions}")
         save_regional_statistics(args.regions, inferer.regional_statistics(image, result))
-    feature_image, feature_mask = image, result   # the pair of --texture, --shape, --first-order, --wavelet, --filtered
+    feature_image, feature_mask = image, result   # the pair of --texture, --shape, --first-order, --wavelet, --filtered, --log
     if resampling is not None:
         logger.info("Resample to %s mm (%s)" % (",".join("%g" % v for v in resampling[0]), resampling[1]))
         r = inferer.resample(image, result, resampled_spacing=resampling[0], interpolator=resampling[1])
@@ -462,6 +507,10 @@ def main(argv=None):
         save_filtered_features(args.filtered, inferer.filtered_features(feature_image, feature_mask, image_types=filtered_types,
                                                                         bin_width=filtered_bin_width,
                                                                         classes=filtered_classes, **settings))
+    if log is not None:
+        logger.info(f"Save LoG features to: {args.log}")
+        save_log_features(args.log, inferer.log_features(feature_image, feature_mask, sigma=log[0], bin_width=log[1],
+                                                         classes=log[2], **settings))
     if args.mesh is not None:
         logger.info(f"Save meshes to: {args.mesh}")
         os.makedirs(args.mesh, exist_ok=True)

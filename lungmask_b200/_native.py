@@ -86,6 +86,7 @@ def lib():
         "lm_gradient_dev": ([vp, vp, i32, i32, i32, i32, vp, vp, vp], i32),
         "lm_bspline_coefficients_dev": ([vp, vp, i32, i32, i32, i32, vp, vp], i32),
         "lm_resample_dev": ([vp, vp, i32, vp, u8p, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp, u8p, vp], i32),
+        "lm_laplacian_of_gaussian_dev": ([vp, vp, i32, i32, i32, i32, vp, C.c_double, vp, vp, vp, vp], i32),
         "lm_shard_init": ([vp, i32, i32, i32], i32),
         "lm_shard_handle_bytes": ([], C.c_size_t),
         "lm_shard_export": ([vp, vp], i32),
@@ -116,7 +117,7 @@ def lib():
 
 
 EXPORTS = ["lm_create", "lm_destroy", "lm_last_error", "lm_device", "lm_batch_capacity", "lm_weight_blob_floats",
-           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_glcm_offsets_dev", "lm_neighbour_offsets_dev", "lm_zone_sizes_plane_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_bspline_coefficients_dev", "lm_resample_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
+           "lm_load_weights", "lm_apply_volume", "lm_apply_volume_dev", "lm_apply_fused", "lm_apply_fused_dev", "lm_apply_volume_oriented", "lm_apply_volume_probs", "lm_apply_dev", "lm_label_stats_dev", "lm_laa_max_pairs", "lm_laa_clusters_dev", "lm_plane_label_counts_dev", "lm_surface_distance_dev", "lm_region_map_dev", "lm_texture_levels_dev", "lm_glcm_dev", "lm_zone_sizes_dev", "lm_glrlm_dev", "lm_neighbour_counts_dev", "lm_glcm_offsets_dev", "lm_neighbour_offsets_dev", "lm_zone_sizes_plane_dev", "lm_shape_sums_dev", "lm_max_diameters_dev", "lm_mesh_counts_dev", "lm_mesh_emit_dev", "lm_first_order_sums_dev", "lm_first_order_splits_dev", "lm_first_order_maps_dev", "lm_glcm_maps_dev", "lm_texture_maps_dev", "lm_wavelet_dev", "lm_image_range_dev", "lm_image_filter_dev", "lm_gradient_dev", "lm_bspline_coefficients_dev", "lm_resample_dev", "lm_laplacian_of_gaussian_dev", "lm_apply_volume_float", "lm_preprocess_float", "lm_fuse", "lm_preprocess",
            "lm_shard_init", "lm_shard_handle_bytes", "lm_shard_export", "lm_shard_connect", "lm_shard_labels",
            "lm_apply_volume_sharded", "lm_apply_volume_sharded_dev",
            "lm_simple_bodymask", "lm_forward", "lm_forward_dev", "lm_postprocess", "lm_reshape_masks",
@@ -668,6 +669,23 @@ class Engine:
                                    C.c_void_p(d_out_ptr), C.c_void_p(d_out_mask_ptr),
                                    C.c_void_p(int(stream)) if stream else None)
         self._resample_check(rc, "resample")
+
+    # ---- Laplacian of Gaussian (lm_laplacian_of_gaussian_dev)
+    def laplacian_of_gaussian_dev(self, d_vol_ptr, dtype_code, shape, spacing_xyz, sigma_mm, d_work_ptrs, d_out_ptr,
+                                  stream=0):
+        """Writes the LoG image (ITK's LaplacianRecursiveGaussianImageFilter normalised across scale, `sigma_mm` with
+        spacing (x, y, z) in mm) of a C-contiguous `shape` device volume of element type `dtype_code` to the float64
+        `shape` device buffer `d_out_ptr`, with the two float64 `shape` device work volumes d_work_ptrs.  ValueError for
+        a refused argument or a NaN or +-inf in the volume; NativeError for the other failures."""
+        n0, n1, n2 = (int(x) for x in shape)
+        sp = np.array([float(s) for s in spacing_xyz], np.float64)
+        if sp.shape != (3,):
+            raise ValueError("laplacian_of_gaussian_dev: spacing must be (x, y, z), got %s" % (spacing_xyz,))
+        w0, w1 = (C.c_void_p(int(p)) for p in d_work_ptrs)
+        rc = lib().lm_laplacian_of_gaussian_dev(self._h, C.c_void_p(d_vol_ptr), int(dtype_code), n0, n1, n2, _ptr(sp),
+                                                float(sigma_mm), w0, w1, C.c_void_p(d_out_ptr),
+                                                C.c_void_p(int(stream)) if stream else None)
+        self._resample_check(rc, "log")
 
     # ---- one volume over several GPUs (one engine per rank; see include/lungmask_b200.h)
     def shard_init(self, rank, world, max_slices):

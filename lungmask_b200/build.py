@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "liblungmask_b200.so")
-SOURCES = ["conv_tc.cu", "forward_misc.cu", "preproc.cu", "postproc.cu", "shard.cu", "stats.cu", "clusters.cu", "regions.cu", "texture.cu", "shape.cu", "first_order.cu", "wavelet.cu", "filters.cu", "mesh.cu", "first_order_maps.cu", "glcm_maps.cu", "texture_maps.cu", "resample.cu", "engine.cu"]
+SOURCES = ["conv_tc.cu", "forward_misc.cu", "preproc.cu", "postproc.cu", "shard.cu", "stats.cu", "clusters.cu", "regions.cu", "texture.cu", "shape.cu", "first_order.cu", "wavelet.cu", "filters.cu", "mesh.cu", "first_order_maps.cu", "glcm_maps.cu", "texture_maps.cu", "resample.cu", "laplacian.cu", "engine.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 

@@ -30,6 +30,7 @@
 #include "glcm_maps.cuh"
 #include "texture_maps.cuh"
 #include "resample.cuh"
+#include "laplacian.cuh"
 
 using namespace lm;
 
@@ -215,6 +216,7 @@ struct lm_engine {
   GlcmMapsWork glcm_maps;       // lm_glcm_maps_dev: the error flag
   TextureMapsWork texture_maps; // lm_texture_maps_dev: the error flag
   ResampleWork resample;        // lm_bspline_coefficients_dev, lm_resample_dev: the non-finite flag
+  LogWork laplacian;            // lm_laplacian_of_gaussian_dev: the non-finite flag
   cudaEvent_t ev[8] = {};
   cudaEvent_t ev_conv[2] = {};
   std::vector<cudaEvent_t> ev_pool;  // per-launch event pairs when conv timing is on
@@ -949,6 +951,7 @@ void lm_destroy(lm_engine* e) {
   e->glcm_maps.release();
   e->texture_maps.release();
   e->resample.release();
+  e->laplacian.release();
   for (auto& ev : e->ev) cudaEventDestroy(ev);
   for (auto& ev : e->ev_conv) cudaEventDestroy(ev);
   for (auto& ev : e->ev_pool) cudaEventDestroy(ev);
@@ -1704,6 +1707,38 @@ int lm_resample_dev(lm_engine* e, const void* d_vol, int dtype, const double* d_
                                  interpolator, d_out, d_out_mask, e->st, &e->launches);
   if (rc == LM_ERR_NONFINITE) return fail(rc, "%s: a sampled value is a NaN or +-inf", fn);
   return rc;
+}
+
+int lm_laplacian_of_gaussian_dev(lm_engine* e, const void* d_vol, int dtype, int n0, int n1, int n2,
+                                 const double* spacing_xyz, double sigma_mm, double* d_work0, double* d_work1,
+                                 double* d_out, void* stream) {
+  static const char* fn = "lm_laplacian_of_gaussian_dev";
+  RC(filter_volume_args(fn, e, d_vol, dtype, n0, n1, n2));
+  if (!spacing_xyz || !d_work0 || !d_work1 || !d_out) return fail(-1, "%s: NULL argument", fn);
+  if (n0 < 4 || n1 < 4 || n2 < 4) return fail(-1, "%s: extents (%d,%d,%d), every axis needs 4 voxels", fn, n0, n1, n2);
+  if (!(isfinite(sigma_mm) && sigma_mm > 0.0)) return fail(-1, "%s: sigma %g is not a finite size > 0 mm", fn, sigma_mm);
+  const int extent[3] = {n2, n1, n0};   // x, y, z
+  LogLine smooth[3], deriv[3];
+  for (int a = 0; a < 3; ++a) {
+    if (!(isfinite(spacing_xyz[a]) && spacing_xyz[a] > 0.0))
+      return fail(-1, "%s: spacing %g along %c is not a finite positive size", fn, spacing_xyz[a], "xyz"[a]);
+    const double sd = sigma_mm / spacing_xyz[a];
+    if ((double)extent[a] < ceil(sd) + 1.0)
+      return fail(-1, "%s: sigma %g mm needs at least ceil(sigma / spacing) + 1 = %.0f voxels along %c, the volume has %d",
+                  fn, sigma_mm, ceil(sd) + 1.0, "xyz"[a], extent[a]);
+    smooth[a] = log_line_coefficients(sd, 0);
+    deriv[a] = log_line_coefficients(sd, 2);
+  }
+  const size_t n = (size_t)n0 * n1 * n2, f64 = n * sizeof(double);
+  const struct { const char* name; const void* p; size_t bytes; } bufs[] = {
+      {"d_vol", d_vol, n * dtype_bytes(dtype)}, {"d_work0", d_work0, f64}, {"d_work1", d_work1, f64}, {"d_out", d_out, f64}};
+  for (int i = 1; i < 4; ++i)
+    for (int j = 0; j < i; ++j)
+      if (overlaps(bufs[i].p, bufs[i].bytes, bufs[j].p, bufs[j].bytes))
+        return fail(-1, "%s: %s overlaps %s", fn, bufs[i].name, bufs[j].name);
+  RC(analysis_inputs(e, fn, stream, {{"d_vol", d_vol}, {"d_work0", d_work0}, {"d_work1", d_work1}, {"d_out", d_out}}));
+  return filter_result(fn, laplacian_of_gaussian(e->laplacian, d_vol, dtype, n0, n1, n2, smooth, deriv, d_work0, d_work1, d_out,
+                                                 e->st, &e->launches));
 }
 
 int lm_first_order_maps_dev(lm_engine* e, const void* d_vol, int dtype, const uint8_t* d_mask, int n0, int n1, int n2,

@@ -410,8 +410,8 @@ def save_probabilities(path, probs, like=None):
 def check_table_path(path, kind):
     """Refuses, before any work is done, an output path that save_statistics (kind "statistics"), save_clusters
     ("clusters"), save_regional_statistics ("regions"), save_texture ("texture"), save_shape ("shape"),
-    save_first_order ("first_order"), save_wavelet_features ("wavelet") or save_filtered_features ("filtered") cannot
-    write."""
+    save_first_order ("first_order"), save_wavelet_features ("wavelet"), save_filtered_features ("filtered") or
+    save_log_features ("log") cannot write."""
     if not path.lower().endswith((".json", ".csv")):
         raise SystemExit("unsupported %s output format (use .json or .csv): %s" % (kind, path))
 
@@ -571,7 +571,13 @@ def save_filtered_features(path, features):
     and the to_dict() of its first-order and texture features with their exact histograms, sums and matrices, NaN as
     null) or .csv (a header, then one line per row: label, name, voxels, then the row's flat vector
     FilteredFeatures.vector with PyRadiomics' keys such as square_firstorder_Mean; NaN is "nan")."""
-    check_table_path(path, "filtered")
+    _save_image_features(path, features, "filtered")
+
+
+def _save_image_features(path, features, kind):
+    """The writer of save_filtered_features and save_log_features: a result with `images`, `labels`, `voxels` and
+    `vector`."""
+    check_table_path(path, kind)
     if path.lower().endswith(".json"):
         return _save_json(path, features)
     labels = features.labels
@@ -585,6 +591,14 @@ def save_filtered_features(path, features):
         lines.append(",".join(_csv_cell(c) for c in cells))
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")
+
+
+def save_log_features(path, features):
+    """Writes the LogFeatures of LMInferer.log_features: .json (the sigmas, the classes and, per LoG image, its bin width
+    and the to_dict() of its first-order and texture features with their exact histograms, sums and matrices, NaN as
+    null) or .csv (a header, then one line per row: label, name, voxels, then the row's flat vector LogFeatures.vector
+    with PyRadiomics' keys such as log-sigma-1-0-mm-3D_firstorder_Mean; NaN is "nan")."""
+    _save_image_features(path, features, "log")
 
 
 MESH_FORMATS = ("stl", "obj", "ply")

@@ -1129,6 +1129,94 @@ class LMInferer:
         computed = (("firstorder",) if first else ()) + texture_classes
         return flt.FilteredFeatures(computed, s.spacing, shift, alpha, bool(gradient_use_spacing), out)
 
+    def _log_plan(self, s, sigmas, spacing):
+        """Checks the sigmas, the spacing and the staged volume's shape before any image is written -> (compute(sigma,
+        out): writes the LoG image of `sigma` to the float64 device tensor `out`, the two float64 work volumes it uses)."""
+        import torch
+        from . import laplacian as lg
+        sp = lg.check_spacing(spacing)
+        shape = lg.check_shape(s.vol.shape, sp, sigmas)
+        work = [torch.empty(shape, dtype=torch.float64, device=s.vol.device) for _ in range(2)]
+
+        def compute(sigma, out):
+            self.engine.laplacian_of_gaussian_dev(s.vol.data_ptr(), s.dtype, shape, sp, sigma,
+                                                  [w.data_ptr() for w in work], out.data_ptr(), stream=s.stream)
+
+        return compute
+
+    def log_images(self, image, sigma, spacing=None):
+        """PyRadiomics' LoG image type of `image` (getLoGImage: ITK's LaplacianRecursiveGaussianImageFilter normalised
+        across scale) -> {name: float64 image of the image's shape} in the order of `sigma`, named as PyRadiomics names
+        them: log-sigma-1-0-mm-3D for sigma 1.  `sigma`: a size in mm or a non-empty collection of them.  The (S, H, W)
+        array is taken as given (no reorientation), converted to float64, with `spacing` (x, y, z) mm or a Volume's or
+        SimpleITK image's; lungmask_b200.laplacian.log_host is the numpy statement, and the result equals it bit for bit
+        (DESIGN §4.20).  A sigma that is not finite and > 0, a repeated sigma, a missing spacing, an axis under 4 voxels
+        or under ceil(sigma / spacing) + 1 voxels and 2^32 voxels or more are a ValueError before any image is written;
+        a NaN or +-inf in the volume is a ValueError.
+
+        `image`: a numpy array, a Volume or SimpleITK image (numpy images come back), a CPU tensor (CPU tensors come
+        back), or a CUDA tensor on the engine's device, read in place after the work queued on the current stream (CUDA
+        float64 tensors on that device come back).  The input is left unchanged.  The call holds two float64 work
+        volumes of the image's size on the device."""
+        import torch
+        from . import laplacian as lg
+        sigmas = lg.check_sigmas(sigma)
+        if spacing is None and not isinstance(image, np.ndarray) and not _is_tensor(image):
+            spacing = tuple(image.spacing) if hasattr(image, "spacing") else tuple(image.GetSpacing())
+        lg.check_spacing(spacing)
+        s = self._stage("log_images", image, None, image_only=True)
+        compute = self._log_plan(s, sigmas, spacing)
+        in_place = _is_tensor(image) and image.is_cuda
+        out = {}
+        buf = None
+        for sg in sigmas:
+            if buf is None or in_place:   # host results are copied out of one device image; CUDA results are the images
+                buf = torch.empty(tuple(s.vol.shape), dtype=torch.float64, device=s.vol.device)
+            compute(sg, buf)
+            out[lg.image_name(sg)] = s.back(buf)
+        return out
+
+    def log_features(self, image, mask, sigma, bin_width=25,
+                     classes=("firstorder", "glcm", "glszm", "glrlm", "gldm", "ngtdm"), gldm_alpha=0, spacing=None,
+                     voxel_array_shift=0, distances=(1,), force2d=False, force2d_dimension=0, weighting_norm=None):
+        """The first-order and texture features of PyRadiomics' LoG image type of `image` under `mask` ->
+        lungmask_b200.laplacian.LogFeatures: for each sigma of `sigma` (mm; see `log_images`), in that order, the
+        FirstOrderFeatures of `first_order` and the TextureFeatures of `texture` run on that image with the rows of
+        `statistics`.  `vector(label)` gives a row's flat vector with PyRadiomics' keys such as
+        log-sigma-1-0-mm-3D_firstorder_Mean.
+
+        `classes`: a non-empty collection of "firstorder", "glcm", "glszm", "glrlm", "gldm" and "ngtdm".  `bin_width`: a
+        positive integer, or a dict keyed by image name or sigma giving one for every sigma.  Every image's rows are
+        discretised before any first-order or texture kernel runs; a row with more than 255 levels is a ValueError
+        naming the image, the row and a sufficient bin width.  `gldm_alpha`, `voxel_array_shift`, `spacing`, and the
+        neighbourhood settings `distances`, `force2d`, `force2d_dimension` and `weighting_norm`: as for `texture` and
+        `first_order`; the spacing is also the filter's.  Bad arguments raise before any kernel runs.
+
+        `image`, `mask` and `spacing` as for `statistics`: numpy arrays, a Volume or SimpleITK image (which supplies the
+        spacing), CPU tensors, or CUDA tensors on the engine's device read in place after the work queued on the current
+        stream; both are left unchanged.  One float64 image and two float64 work volumes of the volume's size are held
+        on the device."""
+        import torch
+        from . import first_order as fo
+        from . import laplacian as lg
+        from . import texture as tx
+        sigmas = lg.check_sigmas(sigma)
+        widths = lg.check_bin_widths(bin_width, sigmas)
+        first, texture_classes = lg.check_classes(classes)
+        alpha = tx.check_alpha(gldm_alpha)
+        shift = fo.check_shift(voxel_array_shift)
+        settings = tx.check_settings(distances, force2d, force2d_dimension, weighting_norm)
+        s = self._stage("log_features", image, mask, spacing)
+        if texture_classes:
+            tx.check_weighting_spacing(settings, s.spacing)
+        compute = self._log_plan(s, sigmas, s.spacing)
+        by_name = {lg.image_name(sg): sg for sg in sigmas}
+        image_buf = torch.empty(tuple(s.vol.shape), dtype=torch.float64, device=s.mask.device)
+        out = self._image_features("log_features", s, image_buf, list(by_name), lambda n: compute(by_name[n], image_buf),
+                                   widths, first, texture_classes, shift, alpha, settings)
+        computed = (("firstorder",) if first else ()) + texture_classes
+        return lg.LogFeatures(sigmas, computed, s.spacing, shift, alpha, out)
+
     def resample(self, image, mask, resampled_spacing=(1, 1, 1), spacing=None, interpolator="bspline", pad_distance=5):
         """PyRadiomics' resampling of `image` and `mask` to `resampled_spacing` (x, y, z) mm (resampledPixelSpacing; an
         entry of 0 keeps that axis) with interpolator "bspline" (sitkBSpline, the default) or "nearest"
